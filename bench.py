@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py -- SELA hot path on B200: encode + decode MSamples/s (BASELINE.json metric).
+"""bench.py -- SELA hot path on H100: encode + decode MSamples/s (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A step = one pass of the hot path over one batch: fused encode of the batch (PCM ->
@@ -15,7 +15,8 @@ independent; SURVEY.md 8e).
   e2e     same metric through the host-buffer C ABI (selab200_encode_frames /
           selab200_decode_frames) from pinned host memory, H2D + D2H inside the timing.
   --impl reference   the reference's own multithreaded CPU path (oracle/_ref when it was
-          compiled from /root/reference, else the plain-C port in oracle/) on the host cores.
+          was compiled from the reference sources, else the plain-C port in oracle/) on the host cores.
+  --dump-outputs DIR   after the timed steps, what the last step computed, as DIR/<name>.npy (see dump_outputs).
 """
 import argparse
 import ctypes as C
@@ -47,7 +48,7 @@ def measured_peak_hbm():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -104,40 +105,35 @@ def workload_config(n_frames, n_samples):
     """The `config` object of BOTH arms (the driver compares them): what one GPU's workload is."""
     return {"workload": WORKLOAD, "frames_per_gpu": n_frames, "samples_per_gpu": n_samples,
             "l2": "no flush: per step the kernels stream the PCM, the word arena and the residue workspace of the "
-                  "whole file (about 390 MB), larger than the 126 MB L2"}
+                  "whole file (about 390 MB), larger than the 50 MB L2"}
 
 
-def source_hash():
-    """Hash of the kernel sources: ties the ncu-derived numbers in profiles/traffic.json to the code that ran."""
-    import hashlib
-    h = hashlib.sha256()
-    for f in sorted((ROOT / "sela_b200" / "csrc").glob("*")):
-        h.update(f.name.encode())
-        h.update(f.read_bytes())
-    return h.hexdigest()[:16]
+DUMP_PCM_SAMPLES = 1 << 22       # float32: 16 MB
+DUMP_WORD_SAMPLES = 1 << 21      # float64: 16 MB
 
 
-def measured_profile(kernel):
-    """What the committed ncu capture says about `kernel` (profiles/traffic.json): DRAM bytes per launch, pipe
-    utilisation.  Returns (entry or None, stale flag): stale = the kernel sources changed since the capture."""
-    p = ROOT / "profiles" / "traffic.json"
-    try:
-        doc = json.loads(p.read_text())
-        e = doc[kernel]
-        return e, doc.get("source_hash") != source_hash()
-    except Exception:
-        return None, True
-
-
-def measured_traffic(kernel):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture (cannot be taken
-    inside the bench: a number measured under a profiler is never a bench value)."""
-    p = ROOT / "profiles" / "traffic.json"
-    try:
-        return int(json.loads(p.read_text())[kernel]["traffic"])
-    except Exception:
-        return None
-
+def dump_outputs(out_dir, codec, pcm_out, n_frames):
+    """What the device-resident step hands its caller, from the last timed step: the subframe descriptors
+    (every field, one row per subframe), the number of Rice words, a fixed seeded sample of the word arena
+    and of the decoded PCM.  All float64 / float32, so that two builds can be compared array for array."""
+    import torch
+    from sela_b200 import _lib
+    out_dir = pathlib.Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    descs = codec.descs.cpu().numpy().view(_lib.DESC_DTYPE)
+    n_words = int(codec.words_used.item())
+    arrays = {"descs": np.stack([descs[f].astype(np.float64) for f in _lib.DESC_DTYPE.names], axis=1),
+              "words_used": np.array([n_words], np.float64)}
+    rng = np.random.default_rng(20240601)
+    for name, src, n, k, dtype in (("words_sample", codec.words, n_words, DUMP_WORD_SAMPLES, np.float64),
+                                   ("pcm_out_sample", pcm_out, n_frames * FRAME * CHANNELS, DUMP_PCM_SAMPLES, np.float32)):
+        idx = np.sort(rng.choice(n, size=min(k, n), replace=False))
+        vals = src[torch.from_numpy(idx).to(src.device)].cpu().numpy()
+        if name == "words_sample":
+            vals = vals.view(np.uint32)                         # the arena is held as int32 on the device
+        arrays[name] = vals.astype(dtype)
+    for name, a in arrays.items():
+        np.save(out_dir / (name + ".npy"), a)
 
 
 def rice_decode_roofline(codec, n_frames, n_words, dev, peak, tiles=(1, 16)):
@@ -544,6 +540,8 @@ def run_ours(args, rank, world, local_rank):
     enc_ms = statistics.fmean(ev[2 * i].elapsed_time(ev[2 * i + 1]) for i in range(args.steps))
     dec_ms = statistics.fmean(ev[2 * i + 1].elapsed_time(ev[2 * i + 2]) for i in range(args.steps))
     codec.check_status()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, codec, out, n_frames)
 
     # ---------------- end-to-end leg (host buffers through the public C ABI) ----------------
     def pinned(nbytes, dtype):
@@ -570,7 +568,7 @@ def run_ours(args, rank, world, local_rank):
         split[0] += t_b - t_a
         split[1] += time.perf_counter() - t_b
 
-    e2e_steps = max(3, min(args.steps, 20))
+    e2e_steps = args.steps
     for _ in range(3):
         e2e_step()
     if dist:
@@ -608,7 +606,6 @@ def run_ours(args, rank, world, local_rank):
     line = None
     if rank == 0:
         desc_bytes = n_frames * CHANNELS * 32
-        prof, stale = measured_profile("k_encode_units<stereo>")
         enc_bytes = n_samples * 2 + n_words * 4 + desc_bytes              # algorithmic: PCM in, words + descs out
         achieved = enc_bytes / (enc_ms * 1e-3) / 1e9
         line = {
@@ -637,16 +634,11 @@ def run_ours(args, rank, world, local_rank):
             "clocks": clocks,
             "roofline": {"kernel": "k_encode_units<stereo> (fused analysis+FIR+Rice; + scan + gather launches)", "bound": "hbm",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (prof or {}).get("traffic"), "traffic_stale": stale, "peak_source": peak_src,
-                         "algorithmic_bytes_per_launch": enc_bytes,
-                         "compute": {"pipe": "fp64", "busy_frac": (prof or {}).get("fp64_busy_frac"),
-                                     "issue_active_frac": (prof or {}).get("issue_active_frac"),
+                         "peak_source": peak_src, "algorithmic_bytes_per_launch": enc_bytes,
+                         "compute": {"pipe": "fp64",
                                      "fp64_ops_per_launch": n_frames * 3 * (2 * FRAME * 101 + 2 * FRAME),
-                                     "note": "busy_frac / issue_active_frac from the committed ncu capture (profiles/traffic.json); "
-                                             "ops = sequentially rounded multiplies and adds of the 101-lag autocorrelation + mean, 3 units per stereo frame"},
-                         "note": "FP64-latency / instruction-issue bound, not HBM bound (DESIGN.md 4); traffic = dram "
-                                 "read+write per launch from profiles/traffic.json (ncu), traffic_stale = kernel sources "
-                                 "changed since that capture"},
+                                     "note": "ops = sequentially rounded multiplies and adds of the 101-lag autocorrelation + mean, 3 units per stereo frame"},
+                         "note": "FP64-latency / instruction-issue bound, not HBM bound (DESIGN.md 4)"},
             "roofline_rice_decode": rice,
         }
         if world == 1 and not args.no_cpu:
@@ -698,14 +690,17 @@ def run_ours(args, rank, world, local_rank):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-sharded", action="store_true", help="skip the configs[3]/[4] block (profiling runs)")
     ap.add_argument("--sharded-minutes", type=int, default=0, help="length of the config-4 file (default 60)")
     ap.add_argument("--sharded-timeout", type=int, default=240, help="seconds before the sharded block is given up (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))

@@ -1,5 +1,5 @@
 /*
- * sela_b200.h -- C ABI of the B200-native SELA per-frame encode/decode hot path.
+ * sela_b200.h -- C ABI of the H100-native SELA per-frame encode/decode hot path.
  *
  * This is the drop-in boundary (SURVEY.md 8b).  The reference has no FFI; its
  * boundary is a set of C++ classes over std::vector-owning value structs.  Each

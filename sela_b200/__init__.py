@@ -1,6 +1,6 @@
-"""sela_b200 -- B200-native implementation of SELA's per-frame encode/decode hot path.
+"""sela_b200 -- H100-native implementation of SELA's per-frame encode/decode hot path.
 
-CUDA kernels (sm_100a) behind the C ABI of include/sela_b200.h; this package holds
+CUDA kernels (sm_90a) behind the C ABI of include/sela_b200.h; this package holds
 the kernels (csrc/), the C++ mirror of the reference interface (host/) and a thin
 Python mirror used by the tests and bench.py.  No CPU fallback.
 """

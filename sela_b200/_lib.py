@@ -88,7 +88,7 @@ def lib():
     global _lib
     if _lib is None:
         if not LIB_PATH.exists():
-            raise ImportError("%s not built: run `python -m sela_b200.build` (nvcc, sm_100a). "
+            raise ImportError("%s not built: run `python -m sela_b200.build` (nvcc, sm_90a). "
                               "There is no CPU fallback." % LIB_PATH)
         L = C.CDLL(str(LIB_PATH))
         for name, (res, args) in _SIGNATURES.items():

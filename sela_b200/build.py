@@ -1,4 +1,4 @@
-"""Build the CUDA extension in-tree: sela_b200/libsela_b200.so (sm_100a only).
+"""Build the CUDA extension in-tree: sela_b200/libsela_b200.so (sm_90a only).
 
     python -m sela_b200.build [--force] [--verbose]
 
@@ -19,7 +19,7 @@ SOURCES = [CSRC / "c_abi.cu"]
 DEPS = list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + [PKG.parent / "include" / "sela_b200.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
     "-Xcompiler", "-fPIC", "-shared", "--extended-lambda",
     "-Xptxas", "-v",

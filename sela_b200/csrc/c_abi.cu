@@ -72,6 +72,7 @@ constexpr int kLanes = 8; // concurrent compute streams of the pipelined host ca
 struct Context {
     bool ready = false;
     int device = -1;
+    int sms = 0;                                   // streaming multiprocessors of `device`
     cudaStream_t stream = nullptr;                 // stage-level calls
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr; // pipelined batch calls: copy engines ...
     cudaStream_t s_compute[kLanes] = {};           // ... and alternating compute lanes
@@ -146,10 +147,8 @@ struct PipelineDrain {
 
 // Chunking of the pipelined host-buffer calls: enough chunks to overlap PCIe with compute,
 // each still several waves of warps, workspace bounded for huge batches.
-// `parts`: target number of chunks.  Measured on the BASELINE batch (12 919 stereo frames,
-// tools/e2e_chunk_sweep.py): encode is best at 8 chunks (4.2 ms end to end vs 3.8 ms of kernels);
-// decode at 4 -- its Rice kernel is one lane per stream and latency-bound, so a chunk must still be
-// thousands of streams.
+// `parts`: target number of chunks (tools/e2e_chunk_sweep.py sweeps it on the BASELINE batch).  A decode
+// chunk must still be thousands of streams: its Rice kernel is one lane per stream and latency-bound.
 uint32_t chunk_frames_for(uint32_t n_frames, uint32_t parts)
 {
     if (const char *env = std::getenv("SELAB200_CHUNK_FRAMES")) { // tuning / tests only
@@ -172,9 +171,8 @@ uint32_t chunk_frames_for(uint32_t n_frames, uint32_t parts)
 // Chunk boundaries of a pipelined host-buffer call.  Equal chunks; for the encoder the first and
 // the last are cut into shrinking pieces: what its pipeline cannot hide is the upload of the first
 // chunk before any kernel runs and the download of the last chunk after the last kernel, so those
-// two are made small (measured on the BASELINE batch: encode call 4.06 -> 3.93 ms; the decode call,
-// whose small chunks each pay the Rice kernel's fixed latency, gets slower and keeps equal chunks).
-// SELAB200_TAPER=0 switches it off.
+// two are made small.  SELAB200_TAPER=0 switches it off for the encoder, SELAB200_DEC_TAPER=0 for the
+// decoder.
 struct ChunkPlan {
     std::vector<uint32_t> start; // n_chunks + 1 boundaries
     uint32_t max_frames = 0;     // largest chunk (sizes the per-lane workspace)
@@ -192,8 +190,8 @@ uint32_t dec_parts()
 }
 bool dec_taper()
 {
-    // round 1 kept equal chunks for decode (small chunks starved the lane-per-stream Rice kernel); with streams cut
-    // into parts for small batches (rice_vs.cuh) the shrinking first and last chunks pay here too: decode call 3.80 -> 3.67 ms
+    // small chunks would starve a lane-per-stream Rice kernel; with streams cut into parts for small batches
+    // (rice_vs.cuh) the shrinking first and last chunks are worth it for decode as well
     const char *e = std::getenv("SELAB200_DEC_TAPER");
     return !(e && e[0] == '0');
 }
@@ -403,14 +401,15 @@ int rice_split_log2(size_t n_sub)
             l++;
         return l;
     }
-    // Measured on B200 (profiles/r02_rice_decode_roofline.json): from about 12 000 streams up one lane per stream
-    // (S = 1) through k_rice_decode_vs is fastest -- the two split passes cost more than the extra warps bring
-    // once every SM has a few warps of its own; below that the machine is starved and cutting the streams
-    // wins (500 streams: S = 16 is 3.5x the first-generation kernel, 8 000 streams: S = 8 is 1.9x).
-    if (n_sub >= 12000)
+    // One lane per stream (S = 1) through k_rice_decode_vs wins once every SM has a few warps of its own (about
+    // 80 streams per SM): the two split passes then cost more than the extra warps bring.  Below that the
+    // machine is starved and the streams are cut until there are about 270 parts per SM.  Both thresholds
+    // scale with the SM count of the device.
+    const size_t sms = (size_t)g.sms;
+    if (n_sub >= 81 * sms)
         return 0;
     int l = 0;
-    while (l < 4 && (n_sub << l) < (size_t)40000)
+    while (l < 4 && (n_sub << l) < 270 * sms)
         l++;
     return l;
 }
@@ -465,7 +464,7 @@ int launch_rice_residues(const DecodeParams &p, void *aux, cudaStream_t stream)
     const size_t n_vs = n_sub << log2s;
     const unsigned vs_blocks = (unsigned)((n_vs + 32 * kVsWarps - 1) / (32 * kVsWarps));
     // geometry: 3 = rings filled cooperatively, 128-byte segments (default: fastest at every batch size measured);
-    // 0 = per-lane cp.async rings; 1, 2 = the same with half the shared memory; 100+ = ablations (tools/rice_ablation.sh)
+    // 0 = per-lane cp.async rings; 1, 2 = the same with half the shared memory; 100+ = ablations (measurement only)
     int geom = 3;
     if (const char *env = std::getenv("SELAB200_RICE_GEOM"))
         geom = std::atoi(env);
@@ -615,8 +614,8 @@ static int init_slot(int device, int slot)
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
-        return fail(SELAB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this build targets sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0) // sm_90a code loads on compute capability 9.0 only
+        return fail(SELAB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this build targets sm_90a only", device,
                     prop.major, prop.minor);
     CUDA_TRY(cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaStreamCreateWithFlags(&g.s_h2d, cudaStreamNonBlocking));
@@ -636,6 +635,7 @@ static int init_slot(int device, int slot)
         return rc;
     g.spare = &g_spare_store[slot];
     g.device = device;
+    g.sms = prop.multiProcessorCount;
     g.ready = true;
     return 0;
 }
@@ -993,7 +993,7 @@ static int decode_host(const selab200_subframe_desc *descs, uint32_t n_frames, u
         return 0;
     PipelineDrain drain;
     // Every chunk gets its own compute lane (up to kLanes): the Rice kernel is one lane per stream
-    // and latency-bound (about 0.4 ms however small the chunk), so the chunks' Rice kernels must
+    // and latency-bound (a fixed time however small the chunk), so the chunks' Rice kernels must
     // overlap each other and the synthesis kernels of earlier chunks rather than queue up.
     const ChunkPlan plan = plan_chunks(n_frames, dec_parts(), dec_taper());
     const uint32_t n_chunks = plan.chunks();

@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions for the sm_100a kernels of the SELA hot path.
+// common.cuh -- shared definitions for the sm_90a kernels of the SELA hot path.
 //
 // One warp owns one subframe (one channel of one 2048-sample frame).  All
 // floating point that feeds the bitstream goes through the *_rn intrinsics below:

@@ -1,4 +1,4 @@
-// kernels.cuh -- the __global__ kernels of the SELA hot path (sm_100a).
+// kernels.cuh -- the __global__ kernels of the SELA hot path (sm_90a).
 //
 //   encode   k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot)
 //            k_encode_sizes + k_encode_scan (stereo decision, prefix sum, descriptors)

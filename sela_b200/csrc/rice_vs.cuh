@@ -230,13 +230,13 @@ struct VsStream {
 // ------------------------------------------------------------------ the warp's rings, filled together --
 //
 // The per-lane cp.async of VsStream costs a 16-byte request to 32 different lines per instruction: at scale
-// the load/store unit replays of those requests, not the parse, bound the decoder (measured: the decoder
-// with the top-ups removed runs 2.3x faster).  Here the 32 rings of a warp are topped up COOPERATIVELY in
+// the load/store unit replays of those requests, not the parse, bound the decoder (an ablation with the
+// top-ups removed runs far faster).  Here the 32 rings of a warp are topped up COOPERATIVELY in
 // 128-byte segments: a ring is two segments of 32 words; a lane whose parser has left a segment puts its
 // row on a list, and eight lanes copy one row's next segment (8 x 16 bytes = one whole line) -- four rows,
 // four lines per instruction instead of 32 -- and, when it has landed, reverse it the same way.  The copies
-// bypass L1 (cp.async.cg): every line is fetched exactly once, and letting those lines allocate in the 16 KB
-// of L1 the kernel leaves was the second wall (1.43 -> 1.19 ms at 413 k streams).  All calls are
+// bypass L1 (cp.async.cg): every line is fetched exactly once, and letting those lines allocate in the L1
+// the kernel's shared memory leaves was the second wall.  All calls are
 // warp-convergent.
 struct VsCoopMeta { // per warp, in shared memory
     // rows that want a segment, each entry written by the row's owner and read by the eight lanes that copy
@@ -774,7 +774,7 @@ __device__ __noinline__ bool vs_slow_round(const VsRing<RING> rg, uint32_t ce, u
     return true;
 }
 
-// ABLATE (measurement only, tools/rice_ablation.py; results are wrong): 1 = no global stores, 2 = no ring
+// ABLATE (measurement only; results are wrong): 1 = no global stores, 2 = no ring
 // top-ups after the first fill, 4 = no in-place reversal.
 template <int RING, int ROUND, int TILE, int ABLATE = 0>
 __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vs(RiceVsParams p, int log2s)

@@ -74,7 +74,7 @@ int usage(const std::string &prog)
               << "Encoding a file:\n" << prog << " -e path/to/input.wav path/to/output.sela\n\n"
               << "Decoding a file:\n" << prog << " -d path/to/input.sela path/to/output.wav\n\n"
               << "Playing a file:\n" << prog << " -p path/to/input.sela\n\n"
-              << "Many files in one process (B200 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
+              << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
     return 0;
 }
@@ -82,7 +82,7 @@ int usage(const std::string &prog)
 
 int main(int argc, char **argv)
 {
-    std::cout << "SimplE Lossless Audio v2 (B200 build). Released under MIT license" << std::endl;
+    std::cout << "SimplE Lossless Audio v2 (H100 build). Released under MIT license" << std::endl;
     const std::string prog = argv[0];
     if (argc < 2)
         return usage(prog);

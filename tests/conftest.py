@@ -10,15 +10,15 @@ for p in (str(ROOT), str(ROOT / "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "ref: needs oracle/_ref (the compiled reference; built where /root/reference exists)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 with -m gpu)")
+    config.addinivalue_line("markers", "ref: needs oracle/_ref (the compiled reference; built where the reference sources exist)")
 
 
 def pytest_collection_modifyitems(config, items):
     import oracle_lib
     oracle_lib.build()
     if not oracle_lib.have_ref():
-        skip = pytest.mark.skip(reason="oracle/_ref/libsela_ref.so not built (no /root/reference here)")
+        skip = pytest.mark.skip(reason="oracle/_ref/libsela_ref.so not built (no reference sources here)")
         for it in items:
             if "ref" in it.keywords:
                 it.add_marker(skip)

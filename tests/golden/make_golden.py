@@ -14,8 +14,12 @@ They travel to the GPU box, where /root/reference does not exist.
     descs_<case>    structured (32-byte descriptor)   reference encoder output
     words_<case>    uint32                            reference encoder output (arena)
     decoded_<case>  int16                             reference DECODER output for (descs, words)
+
+  lpc_first_order.npy   float64 [128]   the reference's firstOrderCoefficients table (src/include/lpc.hpp),
+                                         written when the reference tree is named: make_golden.py REFERENCE_TREE
 """
 import pathlib
+import re
 import sys
 
 import numpy as np
@@ -52,7 +56,17 @@ def cases():
     return out
 
 
+def write_lpc_table(ref_tree):
+    text = (pathlib.Path(ref_tree) / "src" / "include" / "lpc.hpp").read_text()
+    m = re.search(r"firstOrderCoefficients\[128\]\s*=\s*\{([^}]*)\}", text)
+    vals = np.array([float(t) for t in m.group(1).replace("\n", " ").split(",") if t.strip()], np.float64)
+    assert vals.size == 128
+    np.save(pathlib.Path(__file__).parent / "lpc_first_order.npy", vals)
+
+
 def main():
+    if len(sys.argv) > 1:
+        write_lpc_table(sys.argv[1])
     assert ol.have_ref() or pathlib.Path("/root/reference").exists(), "needs the reference tree"
     R = ol.load("ref")
     assert R.kind == "reference"

@@ -1,5 +1,5 @@
 """GPU parity: the CUDA path (through the C ABI) against the CPU oracle, bit for bit.
-Run on the B200 box:  python -m pytest tests -m gpu -x -q
+Run on the H100:  python -m pytest tests -m gpu -x -q
 """
 import numpy as np
 import pytest
