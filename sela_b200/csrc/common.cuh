@@ -20,10 +20,15 @@ constexpr int kMaxRice  = SELAB200_MAX_RICE_PARAM; // 20 (k searched in [0, 20))
 constexpr int kQ        = 35;                      // CORRECTION_FACTOR, src/include/lpc.hpp:8
 constexpr unsigned kFull = 0xffffffffu;
 
-// Offset that makes every in-domain sample (|s| <= 65535) a non-negative 18-bit
+// Offset that makes every in-domain ENCODER sample (|s| <= 65535) a non-negative 18-bit
 // number, so int64 x int32 products need one IMAD.WIDE.U32 + one IMAD (see lpc.cuh).
+// The decoder does not use it: its samples can be any int32 (kSynthBias).
 constexpr int      kSampleBias = 1 << 17;
 constexpr uint32_t kSampleBiasU = 1u << 17;
+// The decoder's offset, 2^31: s ^ 2^31 == s + 2^31 maps every int32 onto [0, 2^32), so the
+// same unsigned products are exact for any sample a stream can decode to (lpc.cuh, K6).
+constexpr uint32_t kSynthBias = 0x80000000u;
+__device__ __forceinline__ uint32_t synth_biased(int s) { return (uint32_t)s ^ kSynthBias; }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }

@@ -17,7 +17,7 @@ struct CoefSmem {
     int32_t  chi[112];           //   j-1, zero padded: the FIR / IIR read them in blocks of 8
     int32_t  q[104];             // quantised reflection coefficients
 };
-// Decoder only: warm-up bias table of the IIR, 2^34 + 2^17 * sum_{j<=t} c[j]  (t = 0..order)
+// Decoder only: warm-up bias table of the IIR, 2^34 + 2^31 * sum_{j<=t} c[j] mod 2^64  (t = 0..order)
 struct IirSmem {
     unsigned long long pre[104];
 };
@@ -333,6 +333,10 @@ __device__ void warp_coefficients(CoefSmem &cf, double *t, int order)
 // they are non-negative 18-bit numbers: c*s' then needs one IMAD.WIDE.U32 (low word)
 // and one IMAD (high word), and the bias is taken out once per output:
 //   sum_j c[j]*s[i-j] = sum_j c[j]*s'[i-j] - 2^17 * sum_j c[j].
+// The IIR below does the same with a bias of 2^31 (kSynthBias): decoded samples can be
+// any int32, and s + 2^31 covers all of them with a 32-bit unsigned s'.  Products and
+// sums then wrap mod 2^64, which cancels exactly: the result is the reference's int64
+// sum wherever that sum does not overflow.
 // Group g covers samples [8g, 8g+8); negative groups (history before the frame) read
 // the zero padding in front of every channel, i.e. s = 0, as the reference's warm-up
 // loop implies.
@@ -417,7 +421,7 @@ __device__ void warp_fir_residual(const Sig &sig, const CoefSmem &cf, int order,
 // 64-bit subtract, a shift and ONE shuffle -- instead of a five-level reduction.
 __device__ void warp_iir_prepare(const CoefSmem &cf, IirSmem &ii, int order)
 {
-    // pre[t] = 2^34 + 2^17 * sum_{j=1..t} c[j]: removes the sample bias for output t
+    // pre[t] = 2^34 + 2^31 * sum_{j=1..t} c[j] (mod 2^64): removes the sample bias for output t
     // (during warm-up only taps j <= t have seen a real sample)
     const int lane = lane_id();
     long long v[4], run = 0;
@@ -439,7 +443,7 @@ __device__ void warp_iir_prepare(const CoefSmem &cf, IirSmem &ii, int order)
     for (int m = 0; m < 4; m++) {
         const int j = 4 * lane + m + 1;
         if (j < 104)
-            ii.pre[j] = (1ull << (kQ - 1)) + ((excl + (unsigned long long)v[m]) << 17);
+            ii.pre[j] = (1ull << (kQ - 1)) + ((excl + (unsigned long long)v[m]) << 31);
     }
     if (lane == 0)
         ii.pre[0] = 1ull << (kQ - 1);
@@ -473,7 +477,7 @@ __device__ void warp_iir_pair(const CoefSmem &cf, const IirSmem &ii, int order, 
         ahi[m] = 0;
     }
     const unsigned long long steady = ii.pre[order];
-    uint32_t sp = (uint32_t)(buf[0] + kSampleBias); // s[0] = r[0]
+    uint32_t sp = synth_biased(buf[0]); // s[0] = r[0]
     const bool writer = active && hl == 0;
     // step(u, i, base): consumes s'[i] in `sp`, produces s[i+1].  Slot m of this step
     // lives in physical register (m + u) % TPL, so the per-step slot shift is free.
@@ -493,7 +497,7 @@ __device__ void warp_iir_pair(const CoefSmem &cf, const IirSmem &ii, int order, 
             buf[(i) + 1] = vnext;                                                                \
         alo[(u) % TPL] = incoming; /* becomes the top slot of the next step */                   \
         ahi[(u) % TPL] = 0;                                                                      \
-        sp = (uint32_t)(vnext + kSampleBias);                                                    \
+        sp = synth_biased(vnext);                                                                \
     }
     int i = 0;
     const int last = n - 1; // steps i = 0 .. last-1
@@ -598,7 +602,7 @@ __device__ __forceinline__ void quad_block(QuadState<TPL> &st, const IirSmem &ii
         }
         if (writer)
             stage_row[e] = vnext;
-        st.sp = (uint32_t)(vnext + kSampleBias);
+        st.sp = synth_biased(vnext);
     }
 }
 

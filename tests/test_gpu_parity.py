@@ -162,7 +162,10 @@ def _stereo_mix(n_frames, seed):
     return pcm
 
 
-@pytest.mark.parametrize("channels,n_frames", [(1, 9), (2, 24), (3, 5), (8, 4)])
+# every channel count the ABI admits (1..SELAB200_MAX_CHANNELS): k_encode_units stages a channel of an
+# N-channel frame at a stride of N samples
+@pytest.mark.parametrize("channels,n_frames", [(1, 9), (2, 24), (3, 5), (8, 4)] +
+                         [(c, 3) for c in range(4, 17) if c != 8])
 def test_frames_encode_bit_exact_and_roundtrip(O, channels, n_frames):
     pcm = _stereo_mix(n_frames, 3) if channels == 2 else synth.sine_noise(48000, channels, n_frames=n_frames, seed=2)
     d_ref, w_ref = O.encode_frames(pcm, channels)
