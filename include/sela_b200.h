@@ -135,7 +135,8 @@ int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frame
  * workspace: selab200_*_workspace_bytes() bytes of device memory, 256-aligned.  d_words must be
  * 16-byte aligned and readable up to the next 16-byte boundary past its last word (the Rice
  * decoder fetches 16 bytes at a time); cudaMalloc / torch allocations satisfy both.  d_pcm (stereo) must
- * be 16-byte aligned as well. */
+ * be 16-byte aligned as well; any d_pcm is read in whole aligned 16-byte pieces, so the 16-byte blocks
+ * that hold its first and last byte must be readable (every allocation's are). */
 size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels);
 int selab200_encode_frames_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
                                   selab200_subframe_desc *d_descs, uint32_t *d_words,

@@ -302,6 +302,16 @@ int launch_check(const char *what)
     return 0;
 }
 
+// The mean of every analysis unit (k_unit_means<KIND>, a warp per 32 units) into means[n_units].
+template <int KIND>
+int launch_unit_means(const void *src, size_t n_units, uint32_t channels, double *means, cudaStream_t stream)
+{
+    const MeanTiling mt = mean_tiling(KIND, channels);
+    k_unit_means<KIND><<<(unsigned)((n_units + 31) / 32), 32, unit_means_smem_bytes(mt), stream>>>(src, (uint32_t)n_units,
+                                                                                                 channels, means);
+    return launch_check("k_unit_means");
+}
+
 // ---- device-resident cores (no synchronisation) --------------------------
 
 // `fresh`: reset status and the arena fill level first (a stand-alone batch); the pipelined
@@ -339,7 +349,11 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     p.status = d_status;
     p.units = static_cast<UnitRecord *>(d_ws);
     p.slots = reinterpret_cast<uint32_t *>(static_cast<char *>(d_ws) + align256(n_units * sizeof(UnitRecord)));
-    p.residues = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(p.slots) + align256(n_units * (size_t)kSlotWords * 4));
+    p.means = reinterpret_cast<double *>(reinterpret_cast<char *>(p.slots) + align256(n_units * (size_t)kSlotWords * 4));
+    p.residues = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(p.means) + align256(n_units * sizeof(double)));
+    if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
+                        : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
+        return rc;
     if (stereo) {
         constexpr size_t smem = encode_smem_bytes<true>();
         if (int rc = set_smem(k_encode_units<true>, smem))
@@ -785,7 +799,7 @@ size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_units = encode_units(n_frames, channels);
     return align256(n_units * sizeof(UnitRecord)) + align256(n_units * (size_t)kSlotWords * 4) +
-           n_units * (size_t)kFrame * 4 + 256;
+           align256(n_units * sizeof(double)) + n_units * (size_t)kFrame * 4 + 256;
 }
 
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
@@ -1594,11 +1608,14 @@ int selab200_lpc_residues(const int32_t *samples, uint32_t n_sub, uint8_t *order
     const size_t sig = (size_t)n_sub * kFrame * 4;
     if (int rc = g.in.ensure(sig)) return rc;
     if (int rc = g.work.ensure(sig)) return rc;
-    if (int rc = g.aux.ensure((size_t)n_sub * kMaxOrder * 4 + n_sub + 256)) return rc;
-    int32_t *d_q = static_cast<int32_t *>(g.aux.ptr);
+    if (int rc = g.aux.ensure(align256((size_t)n_sub * sizeof(double)) + (size_t)n_sub * kMaxOrder * 4 + n_sub + 256)) return rc;
+    double *d_means = static_cast<double *>(g.aux.ptr);
+    int32_t *d_q = reinterpret_cast<int32_t *>(static_cast<char *>(g.aux.ptr) + align256((size_t)n_sub * sizeof(double)));
     uint8_t *d_order = reinterpret_cast<uint8_t *>(d_q + (size_t)n_sub * kMaxOrder);
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, samples, sig, cudaMemcpyHostToDevice, g.stream));
-    k_lpc_residues<<<n_sub, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), n_sub, d_order, d_q,
+    if (int rc = launch_unit_means<kMeanPlanar>(g.in.ptr, n_sub, 1, d_means, g.stream))
+        return rc;
+    k_lpc_residues<<<n_sub, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_means, n_sub, d_order, d_q,
                                                static_cast<int32_t *>(g.work.ptr));
     if (int rc = launch_check("k_lpc_residues"))
         return rc;
@@ -1655,7 +1672,9 @@ int selab200_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t
             return fail(SELAB200_ERR_ARGUMENT, "counts[%u] exceeds stride", i);
     if (n_streams == 0)
         return 0;
-    const size_t vbytes = (size_t)n_streams * stride * 4, wbytes = (size_t)n_streams * words_stride * 4;
+    // on the device every stream row starts 16-byte aligned (the encoder reads int4, rice_lane_range)
+    const uint32_t pitch = (stride + 3) & ~3u;
+    const size_t vbytes = (size_t)n_streams * pitch * 4, wbytes = (size_t)n_streams * words_stride * 4;
     if (int rc = g.in.ensure(vbytes + 16)) return rc;
     if (int rc = g.words.ensure(wbytes + 16)) return rc;
     if (int rc = g.aux.ensure((size_t)n_streams * 12 + 256)) return rc;
@@ -1663,9 +1682,11 @@ int selab200_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t
     uint32_t *d_k = d_counts + n_streams, *d_nw = d_k + n_streams;
     int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
     CUDA_TRY(cudaMemsetAsync(d_status, 0, 4, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, values, vbytes, cudaMemcpyHostToDevice, g.stream));
+    if (stride)
+        CUDA_TRY(cudaMemcpy2DAsync(g.in.ptr, (size_t)pitch * 4, values, (size_t)stride * 4, (size_t)stride * 4, n_streams,
+                                   cudaMemcpyHostToDevice, g.stream));
     CUDA_TRY(cudaMemcpyAsync(d_counts, counts, (size_t)n_streams * 4, cudaMemcpyHostToDevice, g.stream));
-    k_rice_encode<<<n_streams, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_counts, stride, d_k,
+    k_rice_encode<<<n_streams, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_counts, pitch, d_k,
                                                   d_nw, static_cast<uint32_t *>(g.words.ptr), words_stride, d_status);
     if (int rc = launch_check("k_rice_encode"))
         return rc;

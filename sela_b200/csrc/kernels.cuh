@@ -1,6 +1,7 @@
 // kernels.cuh -- the __global__ kernels of the SELA hot path (sm_90a).
 //
-//   encode   k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot)
+//   encode   k_unit_means<KIND> (lane per analysis unit: the mean of its samples)
+//            k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot)
 //            k_encode_sizes + k_encode_scan (stereo decision, prefix sum, descriptors)
 //            k_encode_gather / k_encode_gather_container (slot -> word arena / .sela byte stream)
 //   decode   k_container_unpack (.sela bytes -> word arena)
@@ -8,7 +9,7 @@
 //            k_rice_decode<RING,BATCH> (lane per stream: reflection streams, flagged residue streams)
 //            k_rice_split_index / k_rice_decode_vc (rice_vs.cuh: residue streams, lane per part of a stream)
 //            k_synthesise_quad (+ k_diff_fixup; k_synthesise for frames the batch kernel declines)
-//   stage-level entry points   k_lpc_residues, k_lpc_samples, k_rice_encode, k_rice_decode_streams
+//   stage-level entry points   k_unit_means + k_lpc_residues, k_lpc_samples, k_rice_encode, k_rice_decode_streams
 #pragma once
 
 #include "lpc.cuh"
@@ -17,9 +18,130 @@
 
 namespace selab200 {
 
+// ------------------------------------------------------------------- means --
+//
+// k_unit_means<KIND>: the mean of every analysis unit (K1a, MeanChain), one LANE per unit, 32 units per
+// warp, a warp per CTA.  All 32 lanes of a warp used to run the same 2048-step chain of dependent adds
+// inside k_encode_units; here each lane runs its own unit's.  The units of a warp cover a few consecutive
+// rows of the input (frames of interleaved PCM, or planar signals); tile by tile (64 samples of every row)
+// the warp copies those rows into shared memory with aligned 16-byte loads, issued one tile ahead of the
+// chains, and each lane reads its own samples from there.
+//   kMeanPcm     unit u = channel u % C of frame u / C, interleaved int16 PCM, any channel count C
+//   kMeanStereo  unit u = ch0, ch1 or ch0 - ch1 of frame u / 3 (interleaved int16, 16-byte aligned)
+//   kMeanPlanar  unit u = int32 row u of 2048 samples (16-byte aligned)
+// A row is read in whole aligned 16-byte pieces, so up to 15 bytes around it: never past the 16-byte
+// block that holds the input's first or last byte.
+enum { kMeanPcm = 0, kMeanStereo = 1, kMeanPlanar = 2 };
+constexpr int kMeanTile = 64;  // samples per row per tile
+constexpr int kMeanSlots = 16; // 16-byte pieces per lane per tile (at most 512 per warp, see mean_tiling)
+
+struct MeanTiling {
+    uint32_t units_per_row; // units that read one row
+    uint32_t step;          // bytes from one sample of a row to the next
+    uint32_t row_stride;    // bytes from one row to the next (a multiple of 16)
+    uint32_t rows_max;      // rows a warp's 32 units can cover
+    uint32_t row_words;     // shared-memory words per staged row
+};
+
+// Row pitch in shared memory: the lanes of one row read at most `span` neighbouring words at a time, and a
+// pitch of d words (mod 32), d >= span and odd, puts the rows of a warp on different banks.
+__host__ __device__ inline MeanTiling mean_tiling(int kind, uint32_t channels)
+{
+    MeanTiling t;
+    uint32_t span = 1;
+    if (kind == kMeanPcm) {
+        t.units_per_row = channels;
+        t.step = 2 * channels;
+        t.row_stride = (uint32_t)kFrame * 2 * channels;
+        t.rows_max = 31 / channels + 2 < 32 ? 31 / channels + 2 : 32;
+        span = (2 * channels + 5) / 4;
+    } else {
+        t.units_per_row = kind == kMeanStereo ? 3 : 1;
+        t.step = 4;
+        t.row_stride = (uint32_t)kFrame * 4;
+        t.rows_max = kind == kMeanStereo ? 12 : 32;
+    }
+    const uint32_t d = span | 1u;
+    const uint32_t need = kMeanTile * t.step / 4 + 4; // the tile plus the piece it may start inside
+    t.row_words = need + ((d - need) & 31u);
+    return t;
+}
+
+template <int KIND>
+__global__ void __launch_bounds__(32) k_unit_means(const void *src, uint32_t n_units, uint32_t channels, double *means)
+{
+    extern __shared__ __align__(16) uint32_t staged[]; // [rows_max][row_words]
+    const MeanTiling mt = mean_tiling(KIND, channels);
+    const int lane = lane_id();
+    const uint32_t u0 = blockIdx.x * 32, u = u0 + lane;
+    const uint32_t u_last = u0 + 31 < n_units ? u0 + 31 : n_units - 1;
+    const uint32_t first = u0 / mt.units_per_row, n_rows = u_last / mt.units_per_row - first + 1;
+    const uint32_t mine = u < n_units ? u : u_last; // lanes past the end shadow the last unit
+    const uint32_t row = mine / mt.units_per_row - first, role = mine % mt.units_per_row;
+
+    // the warp's rows start `mis` bytes into an aligned piece; staged row r holds the tile's bytes from there
+    const char *base = static_cast<const char *>(src) + (size_t)first * mt.row_stride;
+    const uint32_t mis = (uint32_t)reinterpret_cast<uintptr_t>(base) & 15u;
+    const uint4 *pieces = reinterpret_cast<const uint4 *>(base - mis);
+    const uint32_t tile_pieces = kMeanTile * mt.step / 16;
+    const uint32_t per_row = (mis + kMeanTile * mt.step + 15) / 16, total = n_rows * per_row;
+    // slot s of this lane: piece v = lane + 32 s of the tile, i.e. piece v % per_row of row v / per_row
+    uint32_t goff[kMeanSlots], soff[kMeanSlots];
+#pragma unroll
+    for (int s = 0; s < kMeanSlots; s++) {
+        const uint32_t v = lane + 32 * s, r = v / per_row, k = v - r * per_row;
+        goff[s] = r * (mt.row_stride / 16) + k;
+        soff[s] = r * mt.row_words + 4 * k;
+    }
+    uint4 buf[kMeanSlots];
+    auto fetch = [&](int t) {
+#pragma unroll
+        for (int s = 0; s < kMeanSlots; s++)
+            if (lane + 32 * s < total)
+                buf[s] = pieces[goff[s] + t * tile_pieces];
+    };
+    const char *at = reinterpret_cast<const char *>(staged) + row * mt.row_words * 4 + mis + (KIND == kMeanPcm ? 2 * role : 0);
+
+    MeanChain chain;
+    fetch(0);
+    for (int t = 0; t < kFrame / kMeanTile; t++) {
+        __syncwarp();
+#pragma unroll
+        for (int s = 0; s < kMeanSlots; s++)
+            if (lane + 32 * s < total) {
+                staged[soff[s]] = buf[s].x;
+                staged[soff[s] + 1] = buf[s].y;
+                staged[soff[s] + 2] = buf[s].z;
+                staged[soff[s] + 3] = buf[s].w;
+            }
+        __syncwarp();
+        if (t + 1 < kFrame / kMeanTile)
+            fetch(t + 1);
+#pragma unroll 8
+        for (int j = 0; j < kMeanTile; j++) {
+            int x;
+            if (KIND == kMeanPcm) {
+                x = *reinterpret_cast<const int16_t *>(at + j * mt.step);
+            } else if (KIND == kMeanStereo) {
+                const uint32_t pair = *reinterpret_cast<const uint32_t *>(at + 4 * j);
+                const int a = (int)(pair << 16) >> 16, b = (int)pair >> 16;
+                x = role == 0 ? a : role == 1 ? b : a - b;
+            } else {
+                x = *reinterpret_cast<const int32_t *>(at + 4 * j);
+            }
+            chain.add(x);
+        }
+    }
+    if (u < n_units)
+        means[u] = chain.mean();
+}
+
+inline size_t unit_means_smem_bytes(const MeanTiling &mt) { return (size_t)mt.rows_max * mt.row_words * 4; }
+
 // ------------------------------------------------------------------ encode --
 //
-// Four launches, no inter-CTA dependency inside any of them:
+// Five launches, no inter-CTA dependency inside any of them:
+//   k_unit_means     one LANE per analysis unit: the mean of its samples (see above).
 //   k_encode_units   one WARP per analysis unit (a channel, or for stereo the three
 //                    candidates ch0 / ch1 / ch0-ch1 of a frame): PCM -> autocorrelation ->
 //                    Schur -> quantise -> step-up -> FIR -> Rice parameter search -> Rice
@@ -51,6 +173,7 @@ struct EncodeParams {
     int32_t *status;
     UnitRecord *units;             // workspace [n_units]
     uint32_t *slots;               // workspace [n_units][kSlotWords]
+    double *means;                 // workspace [n_units]: k_unit_means
     int32_t *residues;             // workspace [n_units][2048]: FIR output, re-read by the Rice stages (L2-resident)
 };
 
@@ -129,7 +252,9 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p)
 
     // ---- analysis ----
     int32_t *res = p.residues + (size_t)unit * kFrame;
-    warp_autocorrelation(sig, scratch);
+    // one lane loads the mean and the warp gets it by shuffle: a warp-wide load of p.means[unit] moves the unit
+    // index out of the uniform registers, and the stereo kernel then needs 78 registers instead of 72
+    warp_autocorrelation(sig, scratch, shfl_d(lane == 0 ? p.means[unit] : 0.0, 0));
     warp_schur(scratch);
     const int order = warp_order_and_quantise(scratch, cf);
     warp_coefficients(cf, scratch.t(), order);
@@ -141,8 +266,8 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p)
     const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
     uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
     if (!too_large) {
-        warp_rice_pack(cf.q, order, cq.k, cq.words, slot);
-        warp_rice_pack(res, kFrame, cr.k, cr.words, slot + kSlotReflWords);
+        warp_rice_pack(cf.q, order, cq, slot);
+        warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
     }
     // The residue row is dead now.  It only ever lived in L2 (written and re-read by this warp
     // within microseconds); tell L2 to drop the dirty lines instead of writing 8 KB per unit back
@@ -886,9 +1011,10 @@ inline size_t synthesise_smem_bytes(uint32_t ch)
 
 // ------------------------------------------------------------ stage level --
 
-// lpc::ResidueGenerator::process for one signal per (1-warp) CTA.
-__global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, uint32_t n_sub, uint8_t *order_out,
-                                                     int32_t *q_out, int32_t *residues)
+// lpc::ResidueGenerator::process for one signal per (1-warp) CTA; the means come from
+// k_unit_means<kMeanPlanar> over the same samples.
+__global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, const double *means, uint32_t n_sub,
+                                                     uint8_t *order_out, int32_t *q_out, int32_t *residues)
 {
     __shared__ __align__(16) AnalysisScratch scratch;
     __shared__ __align__(16) CoefSmem cf;
@@ -902,7 +1028,7 @@ __global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, uin
         s[i] = samples[(size_t)sub * kFrame + i];
     __syncwarp();
     PlainSignal sig{s};
-    warp_autocorrelation(sig, scratch);
+    warp_autocorrelation(sig, scratch, means[sub]);
     warp_schur(scratch);
     const int order = warp_order_and_quantise(scratch, cf);
     warp_coefficients(cf, scratch.t(), order);
@@ -948,13 +1074,14 @@ __global__ void k_selftest_scaling(uint32_t *mismatches)
         atomicAdd(mismatches, 1u);
 }
 
-// rice::RiceEncoder::process, one stream per (1-warp) CTA.
-__global__ void __launch_bounds__(32) k_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t stride,
+// rice::RiceEncoder::process, one stream per (1-warp) CTA.  Stream rows lie `pitch` values apart,
+// pitch a multiple of 4 and values 16-byte aligned (rice_lane_range).
+__global__ void __launch_bounds__(32) k_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t pitch,
                                                     uint32_t *k_out, uint32_t *n_words_out, uint32_t *words,
                                                     uint32_t words_stride, int32_t *status)
 {
     const uint32_t st = blockIdx.x;
-    const int32_t *v = values + (size_t)st * stride;
+    const int32_t *v = values + (size_t)st * pitch;
     const int n = (int)counts[st];
     RiceChoice c = warp_rice_choose(v, n);
     if (lane_id() == 0) {
@@ -966,7 +1093,7 @@ __global__ void __launch_bounds__(32) k_rice_encode(const int32_t *values, const
             raise_status(status, SELAB200_ERR_CAPACITY);
         return;
     }
-    warp_rice_pack(v, n, c.k, c.words, words + (size_t)st * words_stride);
+    warp_rice_pack(v, n, c, words + (size_t)st * words_stride);
 }
 
 // rice::RiceDecoder::process, one stream per lane.

@@ -24,7 +24,7 @@ struct IirSmem {
 // Analysis scratch (3 KB).  The ring is dead once the autocorrelation is done; the
 // reflection coefficients (kk) and the step-up row (t) then live in its bytes.
 struct AnalysisScratch {
-    double ring[256]; // x tile for the mean pass, then the d = x - mean ring (swizzled)
+    double ring[256]; // the d = x - mean ring of the autocorrelation (swizzled)
     double ac[128];   // autocorrelation (raw, then normalised)
     __device__ __forceinline__ double *kk() { return ring; }        // k[0..99]
     __device__ __forceinline__ double *t() { return ring + 104; }   // step-up scratch [0..99]
@@ -70,11 +70,20 @@ __device__ __forceinline__ double sample_to_x(int s)
 __device__ __forceinline__ double sample_to_x_div(int s) { return ddiv((double)s, 32767.0); }
 
 // ---------------------------------------------------------------------------
+// K1a: the mean of generateAutoCorrelation (residue_generator.cpp:26-30): ONE sequential
+// chain  sum = sum + x[j]  over j = 0..2047, then sum / 2048.  Run by one LANE per signal
+// (k_unit_means, 32 signals per warp): the only definition of the chain.
+struct MeanChain {
+    double sum = 0.0;
+    __device__ __forceinline__ void add(int s) { sum = dadd(sum, sample_to_x(s)); }
+    __device__ __forceinline__ double mean() const { return ddiv(sum, (double)kFrame); } // exact: power of two
+};
+
+// ---------------------------------------------------------------------------
 // K1: mean-removed autocorrelation, lags 0..100, + normalisation.
 // generateAutoCorrelation (residue_generator.cpp:20-45).  Result in sm.ac[0..100].
 //
-//  - mean: ONE sequential chain  sum = sum + x[j]  over j (all lanes compute it
-//    redundantly from a broadcast tile so no final broadcast is needed);
+//  - mean: from k_unit_means (MeanChain), computed before the warp starts;
 //  - lane l owns lags 4l..4l+3 (lanes 0..25 useful).  For step j the four products
 //    are d[j]*d[j-4l-m]; each accumulator is a sequential chain over j, exactly
 //    `ac[i] += d[j]*d[j-i]` with the multiply rounded before the add;
@@ -82,31 +91,10 @@ __device__ __forceinline__ double sample_to_x_div(int s) { return ddiv((double)s
 //    accumulator unchanged, so starting the chain at j = 0 instead of j = i is
 //    bit-identical.
 template <typename Sig>
-__device__ void warp_autocorrelation(const Sig &sig, LpcSmem &sm)
+__device__ void warp_autocorrelation(const Sig &sig, LpcSmem &sm, const double mean)
 {
     const int lane = lane_id();
 
-    // ---- mean ----
-    double sum = 0.0;
-    for (int tile = 0; tile < kFrame / 256; tile++) {
-#pragma unroll
-        for (int r = 0; r < 8; r++) {
-            int j = tile * 256 + r * 32 + lane;
-            sm.ring[r * 32 + lane] = sample_to_x(sig.at(j));
-        }
-        __syncwarp();
-        const double2 *x2 = reinterpret_cast<const double2 *>(sm.ring);
-#pragma unroll 8
-        for (int t = 0; t < 128; t++) {
-            double2 v = x2[t];
-            sum = dadd(sum, v.x);
-            sum = dadd(sum, v.y);
-        }
-        __syncwarp();
-    }
-    const double mean = ddiv(sum, (double)kFrame); // exact: power of two
-
-    // ---- autocorrelation ----
     // logical d[-128..-1] = 0  -> chunks 64..127 (the upper half of the ring)
     {
         double2 *r2 = reinterpret_cast<double2 *>(sm.ring);
