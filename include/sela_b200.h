@@ -254,6 +254,37 @@ int selab200_rice_decode(const uint32_t *words, const uint32_t *n_words, uint32_
                          const uint32_t *rice_param, const uint32_t *counts, uint32_t n_streams,
                          int32_t *out, uint32_t out_stride);
 
+/* --------------------------------------------------- tests: internals -- */
+
+/* The floating-point analysis of one analysis unit of the batch encoder, as the encoder computed it:
+ * the intermediates of lpc::ResidueGenerator (src/lpc/residue_generator.cpp:20-96) and the predictor
+ * of LinearPredictor::generatelinearPredictionCoefficients (src/lpc/linear_predictor.cpp:30-61).
+ * 2 832 bytes, naturally aligned. */
+typedef struct selab200_analysis_trace {
+    double  mean;     /* mean of s/32767                                       */
+    double  ac[101];  /* autocorrelation lags 0..100 after normalisation       */
+    double  k[100];   /* reflection coefficients from the Schur recursion      */
+    int64_t c[101];   /* Q35 predictor, c[0] = 0, zero past the order          */
+    int32_t q[100];   /* quantised k, zero past the order                      */
+    int32_t order;
+    int32_t reserved; /* zero                                                  */
+} selab200_analysis_trace;
+
+/* For tests: selab200_encode_frames on one device and one batch, through the same kernels except that the
+ * analysis kernel is its tracing instantiation, which also writes every analysis unit's intermediates to
+ * trace.  The units are frame after frame; within a frame channel 0..channels-1, or for stereo channel 0,
+ * channel 1 and the difference channel 0 - channel 1.  trace: n_frames*3 records for stereo, else
+ * n_frames*channels.  descs, words and *words_used as selab200_encode_frames. */
+int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                          selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                          size_t *words_used, selab200_analysis_trace *trace);
+
+/* For tests: the encoder's order threshold and reflection-coefficient quantiser on chosen values
+ * (src/lpc/residue_generator.cpp:70-96), the device functions the encoder runs.  For every k[i]:
+ * out[4i+0], out[4i+1], out[4i+2] = q of k[i] as coefficient 0, as coefficient 1 and as any later
+ * coefficient; out[4i+3] = 1 if |k[i]| > 0.05, else 0. */
+int selab200_quantise_probe(const double *k, size_t n, int32_t *out);
+
 #ifdef __cplusplus
 }
 #endif

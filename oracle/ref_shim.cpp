@@ -5,12 +5,15 @@
 // into oracle/_ref/libsela_ref.so.  No reference source is copied into this
 // repository; this file only calls the reference's public classes
 // (frame::FrameEncoder/FrameDecoder, lpc::ResidueGenerator/SampleGenerator,
-// rice::RiceEncoder/RiceDecoder) and, for the multithreaded CPU baseline, the
-// private sela::Encoder/Decoder::processFrames (opened with the usual
-// `#define private public` around the include, nothing else is touched).
+// rice::RiceEncoder/RiceDecoder) and reads some of their private members: the
+// multithreaded CPU baseline's sela::Encoder/Decoder::processFrames, and the
+// normalised autocorrelation ResidueGenerator leaves behind (opened with the
+// usual `#define private public` around the includes, nothing else is touched).
 //
-// It exports the SAME symbols as oracle/sela_oracle.c so tests and bench.py can
-// load either library: sela_oracle_kind() tells them apart ("reference").
+// It exports the same symbols as oracle/sela_oracle.c, except the port-only
+// sela_oracle_lpc_mean and sela_oracle_quantise_probe, so tests and bench.py can load
+// either library: sela_oracle_kind() tells them apart ("reference"), and
+// sela_oracle_internals() says which internals each fills.
 
 #include <chrono>
 #include <cstddef>
@@ -21,11 +24,12 @@
 #include <thread>
 #include <vector>
 
+// Every standard header the reference headers pull in (<cstdint>, <string>, <vector>) is included above, so
+// the define below only reaches the reference's own classes.
+#define private public
 #include "frame.hpp"
 #include "lpc.hpp"
 #include "rice.hpp"
-
-#define private public
 #include "sela/decoder.hpp"
 #include "sela/encoder.hpp"
 #undef private
@@ -102,6 +106,8 @@ extern "C" {
 
 const char *sela_oracle_kind(void) { return "reference"; }
 
+const char *sela_oracle_internals(void) { return "ac"; }
+
 int sela_oracle_online_cores(void)
 {
     unsigned n = std::thread::hardware_concurrency();
@@ -111,10 +117,14 @@ int sela_oracle_online_cores(void)
 void sela_oracle_lpc_analyse(const int32_t *s, size_t n, uint8_t *order, int32_t *q, int64_t *c,
                              int32_t *res, double *refl, double *ac)
 {
+    // Not observable here, so left untouched: dequantizeReflectionCoefficients replaces the raw
+    // reflection coefficients with de-quantised ones.
     (void)refl;
-    (void)ac; // internals are private in the reference; only the port exposes them
     data::LpcDecodedData in(16, std::vector<int32_t>(s, s + n));
-    data::LpcEncodedData enc = lpc::ResidueGenerator(in).process();
+    lpc::ResidueGenerator gen(in);
+    data::LpcEncodedData enc = gen.process();
+    if (ac) // lags 0..100 after normalisation (residue_generator.cpp:40-44); process() leaves them alone
+        std::memcpy(ac, gen.autocorrelationFactors.data(), (SELA_ORACLE_MAX_ORDER + 1) * sizeof(double));
     *order = enc.optimalLpcOrder;
     if (q)
         std::memcpy(q, enc.quantizedReflectionCoefficients.data(), enc.quantizedReflectionCoefficients.size() * 4);

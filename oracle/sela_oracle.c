@@ -99,6 +99,52 @@ void sela_oracle_lpc_coefficients(const int32_t *q, uint8_t order, int64_t *c)
         c[1 + m] = (int64_t)(scale * (-t[m]));
 }
 
+/* quantizeReflectionCoefficients (src/lpc/residue_generator.cpp:80-96) for coefficient i of value k */
+static int32_t quantise_one(int i, double k)
+{
+    const double sqrt2 = 1.4142135623730950488016887242096; /* lpc.hpp:9 */
+    double v;
+    if (i == 0)
+        v = floor(64.0 * (-1.0 + (sqrt2 * sqrt(k + 1.0))));
+    else if (i == 1)
+        v = floor(64.0 * (-1.0 + (sqrt2 * sqrt(-k + 1.0))));
+    else
+        v = floor(64.0 * k);
+    return isnan(v) ? 0 : (int32_t)v;
+}
+
+void sela_oracle_quantise_probe(const double *k, size_t n, int32_t *out)
+{
+    for (size_t i = 0; i < n; i++) {
+        out[4 * i + 0] = quantise_one(0, k[i]);
+        out[4 * i + 1] = quantise_one(1, k[i]);
+        out[4 * i + 2] = quantise_one(2, k[i]);
+        out[4 * i + 3] = fabs(k[i]) > 0.05; /* generateoptimalLpcOrder, :73 */
+    }
+}
+
+const char *sela_oracle_internals(void) { return "ac refl mean quantise"; }
+
+/* quantizeSamples (src/lpc/residue_generator.cpp:12-18) into x[n] and the mean of
+ * generateAutoCorrelation (:26-30): true division by INT16_MAX (lpc.hpp:93), one sequential sum */
+static double samples_and_mean(const int32_t *s, size_t n, double *x)
+{
+    for (size_t j = 0; j < n; j++)
+        x[j] = (double)s[j] / 32767.0;
+    double sum = 0.0;
+    for (size_t j = 0; j < n; j++)
+        sum = sum + x[j];
+    return sum / (double)n;
+}
+
+double sela_oracle_lpc_mean(const int32_t *s, size_t n)
+{
+    double *x = (double *)malloc(n * sizeof(double));
+    const double mean = samples_and_mean(s, n, x);
+    free(x);
+    return mean;
+}
+
 /* src/lpc/residue_generator.cpp:12-134 */
 void sela_oracle_lpc_analyse(const int32_t *s, size_t n, uint8_t *order_out, int32_t *q,
                              int64_t *c, int32_t *res, double *refl_out, double *ac_out)
@@ -111,15 +157,8 @@ void sela_oracle_lpc_analyse(const int32_t *s, size_t n, uint8_t *order_out, int
     int32_t q_local[MAXO];
     int64_t c_local[MAXO + 1];
 
-    /* quantizeSamples (:12-18): true division by INT16_MAX (lpc.hpp:93) */
-    for (size_t j = 0; j < n; j++)
-        x[j] = (double)s[j] / 32767.0;
-
     /* generateAutoCorrelation (:20-45): sequential sum, sequential lags */
-    double sum = 0.0;
-    for (size_t j = 0; j < n; j++)
-        sum = sum + x[j];
-    double mean = sum / (double)n;
+    const double mean = samples_and_mean(s, n, x);
     for (size_t j = 0; j < n; j++)
         d[j] = x[j] - mean;            /* same value every time the reference recomputes it */
     for (size_t i = 0; i <= MAXO; i++) {
@@ -165,19 +204,8 @@ void sela_oracle_lpc_analyse(const int32_t *s, size_t n, uint8_t *order_out, int
     }
 
     /* quantizeReflectionCoefficients (:80-96) */
-    const double sqrt2 = 1.4142135623730950488016887242096; /* lpc.hpp:9 */
-    if (order > 0) {
-        double v = floor(64.0 * (-1.0 + (sqrt2 * sqrt(k[0] + 1.0))));
-        q_local[0] = isnan(v) ? 0 : (int32_t)v;
-    }
-    if (order > 1) {
-        double v = floor(64.0 * (-1.0 + (sqrt2 * sqrt(-k[1] + 1.0))));
-        q_local[1] = isnan(v) ? 0 : (int32_t)v;
-    }
-    for (int i = 2; i < order; i++) {
-        double v = floor(64.0 * k[i]);
-        q_local[i] = isnan(v) ? 0 : (int32_t)v;
-    }
+    for (int i = 0; i < order; i++)
+        q_local[i] = quantise_one(i, k[i]);
 
     sela_oracle_lpc_coefficients(q_local, order, c_local);
 

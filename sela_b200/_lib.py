@@ -32,6 +32,13 @@ INFO_DTYPE = np.dtype([
 ], align=True)
 assert INFO_DTYPE.itemsize == 32
 
+# mirrors selab200_analysis_trace, 2832 bytes
+TRACE_DTYPE = np.dtype([
+    ("mean", "<f8"), ("ac", "<f8", (101,)), ("k", "<f8", (100,)), ("c", "<i8", (101,)),
+    ("q", "<i4", (100,)), ("order", "<i4"), ("reserved", "<i4"),
+], align=True)
+assert TRACE_DTYPE.itemsize == 2832
+
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
 
@@ -76,6 +83,8 @@ _SIGNATURES = {
     "selab200_lpc_samples": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_rice_encode": (_I, [_V, _V, _U32, _U32, _V, _V, _V, _U32]),
     "selab200_rice_decode": (_I, [_V, _V, _U32, _V, _V, _U32, _V, _U32]),
+    "selab200_encode_trace": (_I, [_V, _U32, _U32, _V, _V, _SZ, _V, _V]),
+    "selab200_quantise_probe": (_I, [_V, _SZ, _V]),
 }
 
 

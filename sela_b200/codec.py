@@ -11,6 +11,8 @@ error behaviour as in include/sela_b200.h):
                                     sela::Encoder::process + file::SelaFile::writeToFile, and
                                     file::SelaFile::readFromFile + sela::Decoder::processFrames,
                                     on the byte-packed .sela stream
+    encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, and its
+                                    order threshold and quantiser on chosen values
 
 Everything computes on the GPU through the C ABI; NumPy only carries host buffers.
 The C++ mirror of the same interface (data::, frame::, file::, sela:: classes and
@@ -21,7 +23,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import DESC_DTYPE, FRAME, INFO_DTYPE, MAX_ORDER, SelaB200Error, check, init, lib  # noqa: F401
+from ._lib import DESC_DTYPE, FRAME, INFO_DTYPE, MAX_ORDER, TRACE_DTYPE, SelaB200Error, check, init, lib  # noqa: F401
 
 
 def _c(a, dtype):
@@ -43,6 +45,37 @@ def encode_frames(pcm, channels, words_capacity=None, device=0):
     check(L.selab200_encode_frames(pcm.ctypes.data, n_frames, channels, descs.ctypes.data, words.ctypes.data,
                                    cap, C.addressof(used)))
     return descs, words[:used.value].copy()
+
+
+def encode_trace(pcm, channels, device=0):
+    """encode_frames on one batch through the tracing analysis kernel -> (descs, words, trace).
+
+    trace: TRACE_DTYPE[n_units], one record per analysis unit, frame after frame; within a frame the channels,
+    or for stereo ch0, ch1 and ch0 - ch1."""
+    init(device)
+    pcm = _c(pcm, np.int16).reshape(-1)
+    n_frames = pcm.size // (FRAME * channels)
+    if n_frames * FRAME * channels != pcm.size:
+        raise ValueError("pcm must hold whole 2048-sample frames")
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    trace = np.zeros(n_frames * (3 if channels == 2 else channels), TRACE_DTYPE)
+    used = C.c_size_t(0)
+    check(L.selab200_encode_trace(pcm.ctypes.data, n_frames, channels, descs.ctypes.data, words.ctypes.data, cap,
+                                  C.addressof(used), trace.ctypes.data))
+    return descs, words[:used.value].copy(), trace
+
+
+def quantise_probe(k, device=0):
+    """float64 k[n] -> int32 [n, 4]: the encoder's q of each k as coefficient 0, 1 and any later one, and
+    whether |k| > 0.05 (the coefficient counts for the order)."""
+    init(device)
+    k = _c(k, np.float64).reshape(-1)
+    out = np.zeros((k.size, 4), np.int32)
+    check(lib().selab200_quantise_probe(k.ctypes.data, k.size, out.ctypes.data))
+    return out
 
 
 def decode_frames(descs, words, channels, device=0):

@@ -312,6 +312,17 @@ int launch_unit_means(const void *src, size_t n_units, uint32_t channels, double
     return launch_check("k_unit_means");
 }
 
+// k_encode_units<STEREO, TRACE>, a warp per analysis unit.
+template <bool STEREO, bool TRACE>
+int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis_trace *d_trace, cudaStream_t stream)
+{
+    constexpr size_t smem = encode_smem_bytes<STEREO>();
+    if (int rc = set_smem(k_encode_units<STEREO, TRACE>, smem))
+        return rc;
+    k_encode_units<STEREO, TRACE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace);
+    return launch_check("k_encode_units");
+}
+
 // ---- device-resident cores (no synchronisation) --------------------------
 
 // `fresh`: reset status and the arena fill level first (a stand-alone batch); the pipelined
@@ -321,7 +332,8 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
                   uint32_t *d_words, size_t capacity, uint64_t *d_used, int32_t *d_status, void *d_ws,
                   size_t ws_bytes, cudaStream_t stream, bool fresh = true, cudaEvent_t before_scan = nullptr,
                   cudaEvent_t after_scan = nullptr, unsigned long long *h_fill_after = nullptr,
-                  uint8_t *d_container = nullptr, unsigned long long sub_base = 0)
+                  uint8_t *d_container = nullptr, unsigned long long sub_base = 0,
+                  selab200_analysis_trace *d_trace = nullptr)
 {
     if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
         return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
@@ -354,19 +366,12 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
                         : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
         return rc;
-    if (stereo) {
-        constexpr size_t smem = encode_smem_bytes<true>();
-        if (int rc = set_smem(k_encode_units<true>, smem))
-            return rc;
-        k_encode_units<true><<<(unsigned)n_units, 32, smem, stream>>>(p);
-    } else {
-        constexpr size_t smem = encode_smem_bytes<false>();
-        if (int rc = set_smem(k_encode_units<false>, smem))
-            return rc;
-        k_encode_units<false><<<(unsigned)n_units, 32, smem, stream>>>(p);
-    }
-    if (int rc = launch_check("k_encode_units"))
-        return rc;
+    const int rc_units = stereo ? (d_trace ? launch_encode_units<true, true>(p, n_units, d_trace, stream)
+                                           : launch_encode_units<true, false>(p, n_units, nullptr, stream))
+                                : (d_trace ? launch_encode_units<false, true>(p, n_units, d_trace, stream)
+                                           : launch_encode_units<false, false>(p, n_units, nullptr, stream));
+    if (rc_units)
+        return rc_units;
     const unsigned scan_ctas = (unsigned)((n_sub + kScanTile - 1) / kScanTile);
     k_encode_sizes<<<scan_ctas, kScanTile, 0, stream>>>(p);
     if (int rc = launch_check("k_encode_sizes"))
@@ -904,6 +909,8 @@ int selab200_rice_decode_flagged(uint32_t *n_flagged)
 }
 
 } // extern "C"
+
+static_assert(sizeof(selab200_analysis_trace) == 2832, "selab200_analysis_trace layout (include/sela_b200.h)");
 
 // Bytes of container in front of frame f when `words` Rice words precede it.
 static unsigned long long container_frame_byte(unsigned long long f, uint32_t channels, unsigned long long words)
@@ -1588,6 +1595,76 @@ int selab200_selftest(uint32_t *mismatches)
     CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d, 4, cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaStreamSynchronize(g.stream));
     *mismatches = (uint32_t)g.h_small[8];
+    return 0;
+}
+
+// For tests: one unpipelined batch through encode_device with the tracing unit kernel (include/sela_b200.h).
+int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
+                          uint32_t *words, size_t words_capacity, size_t *words_used, selab200_analysis_trace *trace)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !trace)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    *words_used = 0;
+    if (n_frames == 0)
+        return 0;
+    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
+    const size_t ws_bytes = selab200_encode_workspace_bytes(n_frames, channels);
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
+    if (int rc = g.work.ensure(ws_bytes)) return rc;
+    if (int rc = g.aux.ensure(n_units * sizeof(selab200_analysis_trace))) return rc;
+    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
+    selab200_analysis_trace *d_trace = static_cast<selab200_analysis_trace *>(g.aux.ptr);
+    CUDA_TRY(cudaMemsetAsync(d_trace, 0, n_units * sizeof(selab200_analysis_trace), g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
+                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
+                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, true, nullptr,
+                               nullptr, nullptr, nullptr, 0, d_trace))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(trace, d_trace, n_units * sizeof(selab200_analysis_trace), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    uint64_t used;
+    memcpy(&used, g.h_small + 2, 8);
+    *words_used = (size_t)used;
+    if (g.h_small[0] != 0)
+        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (used > words_capacity)
+        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    return 0;
+}
+
+int selab200_quantise_probe(const double *k, size_t n, int32_t *out)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!k || !out)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (n == 0)
+        return 0;
+    if (n > 0xffffffffu)
+        return fail(SELAB200_ERR_ARGUMENT, "at most 2^32 - 1 values per call");
+    if (int rc = g.in.ensure(n * sizeof(double))) return rc;
+    if (int rc = g.work.ensure(n * 4 * sizeof(int32_t))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, k, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
+    k_quantise_probe<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(static_cast<const double *>(g.in.ptr), (uint32_t)n,
+                                                                       static_cast<int32_t *>(g.work.ptr));
+    if (int rc = launch_check("k_quantise_probe"))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(out, g.work.ptr, n * 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
     return 0;
 }
 

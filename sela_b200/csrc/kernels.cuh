@@ -182,8 +182,12 @@ __host__ __device__ inline uint32_t encode_units(uint32_t n_frames, uint32_t cha
     return channels == 2 ? n_frames * 3u : n_frames * channels;
 }
 
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p)
+// TRACE (tests only, selab200_encode_trace): the same kernel, which also copies each unit's analysis
+// intermediates to trace[unit] as they are produced.  Production runs TRACE = false, where none of it exists and
+// `trace` is null.  `trace` is a kernel argument of its own rather than a field of EncodeParams: a longer
+// EncodeParams would move the parameter offsets of the kernels that take arguments after it.
+template <bool STEREO, bool TRACE = false>
+__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_analysis_trace *trace)
 {
     constexpr int kRow = kHistoryPad + kFrame;
     constexpr int kLoWords = (kHistoryPad + kFrame) / 32; // parity bits of a difference signal
@@ -255,9 +259,27 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p)
     // one lane loads the mean and the warp gets it by shuffle: a warp-wide load of p.means[unit] moves the unit
     // index out of the uniform registers, and the stereo kernel then needs 78 registers instead of 72
     warp_autocorrelation(sig, scratch, shfl_d(lane == 0 ? p.means[unit] : 0.0, 0));
+    if constexpr (TRACE) { // before warp_schur: the predictor overlays ac[] from warp_order_and_quantise on
+        selab200_analysis_trace &tr = trace[unit];
+        if (lane == 0)
+            tr.mean = p.means[unit];
+        for (int i = lane; i <= kMaxOrder; i += 32)
+            tr.ac[i] = scratch.ac[i];
+    }
     warp_schur(scratch);
     const int order = warp_order_and_quantise(scratch, cf);
     warp_coefficients(cf, scratch.t(), order);
+    if constexpr (TRACE) { // k[] (ring[0, 100)) is still intact: t[] and the predictor lie behind it
+        selab200_analysis_trace &tr = trace[unit];
+        for (int i = lane; i < kMaxOrder; i += 32) {
+            tr.k[i] = scratch.kk()[i];
+            tr.q[i] = cf.q[i];
+        }
+        for (int i = lane; i <= kMaxOrder; i += 32)
+            tr.c[i] = i == 0 ? 0 : coef_at(cf, i);
+        if (lane == 0)
+            tr.order = order;
+    }
     warp_fir_residual(sig, cf, order, res);
 
     // ---- Rice: parameter search, then pack into this unit's slot ----
@@ -1062,6 +1084,19 @@ __global__ void __launch_bounds__(32) k_lpc_samples(const int32_t *residues, uin
     warp_iir_synthesis_pair(cf, ii, order, buf, lane < 16, kFrame); // upper half shadows, never stores
     for (int i = lane; i < kFrame; i += 32)
         samples[(size_t)sub * kFrame + i] = buf[i];
+}
+
+// selab200_quantise_probe: the encoder's order threshold and quantiser on chosen k, a thread per value.
+__global__ void k_quantise_probe(const double *k, uint32_t n, int32_t *out)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const double kv = k[i];
+    out[4 * (size_t)i + 0] = quantise_reflection(0, kv);
+    out[4 * (size_t)i + 1] = quantise_reflection(1, kv);
+    out[4 * (size_t)i + 2] = quantise_reflection(2, kv);
+    out[4 * (size_t)i + 3] = reflection_significant(kv) ? 1 : 0;
 }
 
 // Exhaustive device check of sample_to_x against IEEE division over |s| <= 65535.

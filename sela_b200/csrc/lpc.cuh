@@ -227,6 +227,27 @@ __device__ void warp_schur(LpcSmem &sm)
 // ---------------------------------------------------------------------------
 // K2b: order selection + 7-bit quantisation
 // generateoptimalLpcOrder / quantizeReflectionCoefficients (residue_generator.cpp:70-96).
+// The threshold and the quantiser of one coefficient are also run on their own, on chosen inputs, by the test
+// entry selab200_quantise_probe (k_quantise_probe).
+
+// Whether k counts for the order: the order is one past the last such coefficient (residue_generator.cpp:73).
+__device__ __forceinline__ bool reflection_significant(double kv) { return fabs(kv) > 0.05; }
+
+// q of coefficient i with value kv: i = 0 and i = 1 through the square-root companding, the rest linearly.
+// k outside [-1, 1] makes the square root NaN, and a NaN quantises to 0 (residue_generator.cpp:85-94).
+__device__ __forceinline__ int quantise_reflection(int i, double kv)
+{
+    const double sqrt2 = 1.4142135623730950488016887242096; // src/include/lpc.hpp:9
+    double v;
+    if (i == 0)
+        v = floor(dmul(64.0, dadd(-1.0, dmul(sqrt2, dsqrt(dadd(kv, 1.0))))));
+    else if (i == 1)
+        v = floor(dmul(64.0, dadd(-1.0, dmul(sqrt2, dsqrt(dadd(-kv, 1.0))))));
+    else
+        v = floor(dmul(64.0, kv));
+    return isnan(v) ? 0 : __double2int_rz(v);
+}
+
 __device__ int warp_order_and_quantise(LpcSmem &sm, CoefSmem &cf)
 {
     const int lane = lane_id();
@@ -235,26 +256,17 @@ __device__ int warp_order_and_quantise(LpcSmem &sm, CoefSmem &cf)
 #pragma unroll
     for (int t = 0; t < 4; t++) {
         int i = lane + 32 * t;
-        if (i < kMaxOrder && fabs(kk[i]) > 0.05)
+        if (i < kMaxOrder && reflection_significant(kk[i]))
             best = i;
     }
     best = __reduce_max_sync(kFull, best);
     const int order = best < 0 ? 1 : best + 1; // default 1 (src/include/lpc.hpp:76)
 
-    const double sqrt2 = 1.4142135623730950488016887242096; // src/include/lpc.hpp:9
 #pragma unroll
     for (int t = 0; t < 4; t++) {
         int i = lane + 32 * t;
         if (i < order) {
-            double kv = kk[i];
-            double v;
-            if (i == 0)
-                v = floor(dmul(64.0, dadd(-1.0, dmul(sqrt2, dsqrt(dadd(kv, 1.0))))));
-            else if (i == 1)
-                v = floor(dmul(64.0, dadd(-1.0, dmul(sqrt2, dsqrt(dadd(-kv, 1.0))))));
-            else
-                v = floor(dmul(64.0, kv));
-            cf.q[i] = isnan(v) ? 0 : __double2int_rz(v);
+            cf.q[i] = quantise_reflection(i, kk[i]);
         } else if (i < 104) {
             cf.q[i] = 0;
         }

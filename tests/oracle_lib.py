@@ -35,11 +35,28 @@ DESC_DTYPE = np.dtype([
 assert DESC_DTYPE.itemsize == C.sizeof(Desc) == 32, (DESC_DTYPE.itemsize, C.sizeof(Desc))
 
 
+def _predates_internals(lib):
+    """A library built from sources older than sela_oracle_internals() (e.g. a prebuilt copy whose file time is
+    newer than the sources, so make keeps it) lacks the symbol."""
+    return lib.exists() and b"sela_oracle_internals" not in lib.read_bytes()
+
+
 def build(force=False):
     """make -C oracle (liboracle.so always; _ref only where /root/reference exists)."""
     if force or not (ORACLE_DIR / "liboracle.so").exists() or (
             os.path.isdir("/root/reference") and not (ORACLE_DIR / "_ref" / "libsela_ref.so").exists()):
         subprocess.run(["make", "-C", str(ORACLE_DIR)], check=True, capture_output=True)
+    # Rebuild a library that predates its sources' internals query, where its sources are here.  Best effort: a
+    # library that cannot be rebuilt (read-only tree, no reference sources) is used as it is, and
+    # Oracle.internals then says what it lacks.
+    stale = []
+    if _predates_internals(ORACLE_DIR / "liboracle.so"):
+        stale.append(ORACLE_DIR / "sela_oracle.c")
+    if os.path.isdir("/root/reference") and _predates_internals(ORACLE_DIR / "_ref" / "libsela_ref.so"):
+        stale.append(ORACLE_DIR / "ref_shim.cpp")
+    if stale:
+        cmd = ["make", "-C", str(ORACLE_DIR)] + [a for f in stale for a in ("-W", str(f))]
+        subprocess.run(cmd, check=False, capture_output=True)
 
 
 def have_ref():
@@ -72,23 +89,45 @@ class Oracle:
         L.sela_oracle_frame_decode_i32.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
         self.kind = L.sela_oracle_kind().decode()
         self.cores = L.sela_oracle_online_cores()
+        # what the library exposes of the analysis' internals (nothing, if it was built before it could say)
+        has = hasattr(L, "sela_oracle_internals")
+        if has:
+            L.sela_oracle_internals.restype = C.c_char_p
+        self.internals = frozenset(L.sela_oracle_internals().decode().split()) if has else frozenset()
+        if "mean" in self.internals:
+            L.sela_oracle_lpc_mean.restype = C.c_double
+            L.sela_oracle_lpc_mean.argtypes = [C.c_void_p, C.c_size_t]
+        if "quantise" in self.internals:
+            L.sela_oracle_quantise_probe.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]
 
     # ---- stage level ------------------------------------------------------
     def lpc_analyse(self, s, want_internals=False):
+        """want_internals adds ac (normalised lags 0..100), refl (raw k[0..99]) and mean, each None where the
+        library does not expose it (self.internals): the compiled reference exposes ac only."""
         s = np.ascontiguousarray(s, dtype=np.int32)
         n = s.size
         order = C.c_uint8(0)
         q = np.zeros(100, np.int32)
         c = np.zeros(101, np.int64)
         res = np.zeros(n, np.int32)
-        refl = np.zeros(100, np.float64)
-        ac = np.zeros(101, np.float64)
+        refl = np.full(100, np.nan)
+        ac = np.full(101, np.nan)
         self.lib.sela_oracle_lpc_analyse(s.ctypes.data, n, C.addressof(order), q.ctypes.data, c.ctypes.data,
                                          res.ctypes.data, refl.ctypes.data, ac.ctypes.data)
         o = order.value
         out = dict(order=o, q=q[:o].copy(), c=c[:o + 1].copy(), res=res)
         if want_internals:
-            out.update(refl=refl, ac=ac)
+            has = self.internals
+            mean = self.lib.sela_oracle_lpc_mean(s.ctypes.data, n) if "mean" in has else None
+            out.update(ac=ac if "ac" in has else None, refl=refl if "refl" in has else None, mean=mean)
+        return out
+
+    def quantise_probe(self, k):
+        """float64 k[n] -> int32 [n, 4]: q of k as coefficient 0, 1 and any later one, and |k| > 0.05
+        (the port: "quantise" in self.internals)."""
+        k = np.ascontiguousarray(k, dtype=np.float64)
+        out = np.zeros((k.size, 4), np.int32)
+        self.lib.sela_oracle_quantise_probe(k.ctypes.data, k.size, out.ctypes.data)
         return out
 
     def lpc_coefficients(self, q, order):

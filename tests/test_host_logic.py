@@ -47,6 +47,13 @@ def test_no_cpu_fallback_without_device():
     rc = L.selab200_encode_frames(pcm.ctypes.data, 1, 1, descs.ctypes.data, words.ctypes.data, 4096,
                                   C.addressof(used))
     assert rc == -7          # NOT_INIT: nothing silently computed on the CPU
+    trace = np.zeros(1, _lib.TRACE_DTYPE)
+    rc = L.selab200_encode_trace(pcm.ctypes.data, 1, 1, descs.ctypes.data, words.ctypes.data, 4096,
+                                 C.addressof(used), trace.ctypes.data)
+    assert rc == -7
+    k = np.zeros(4)
+    q = np.zeros(16, np.int32)
+    assert L.selab200_quantise_probe(k.ctypes.data, 4, q.ctypes.data) == -7
     import sela_b200
     with pytest.raises(sela_b200.SelaB200Error):
         sela_b200.encode_frames(pcm, 1)
