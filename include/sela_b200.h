@@ -285,6 +285,14 @@ int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channe
  * coefficient; out[4i+3] = 1 if |k[i]| > 0.05, else 0. */
 int selab200_quantise_probe(const double *k, size_t n, int32_t *out);
 
+/* For tests: the encoder's FIR residual (src/lpc/residue_generator.cpp:98-119), the device function the encoder
+ * runs, on chosen signals and predictors.  samples: [n][2048]; wide = 0 stages them as the int16 row of a channel
+ * unit (-32768..32767), wide != 0 as the row and parity bits of a 17-bit unit (|s| <= 65535); anything outside
+ * -> SELAB200_ERR_RANGE.  orders[n] in 0..100; c: [n][101], the Q35 predictor, c[i][1..orders[i]] used (any int64).
+ * residues: [n][2048], s[t] - (int32)((2^34 + sum_j c[j] * s[t-j]) >> 35) with the sum taken mod 2^64. */
+int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                       int32_t *residues);
+
 #ifdef __cplusplus
 }
 #endif

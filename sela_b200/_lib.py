@@ -85,6 +85,7 @@ _SIGNATURES = {
     "selab200_rice_decode": (_I, [_V, _V, _U32, _V, _V, _U32, _V, _U32]),
     "selab200_encode_trace": (_I, [_V, _U32, _U32, _V, _V, _SZ, _V, _V]),
     "selab200_quantise_probe": (_I, [_V, _SZ, _V]),
+    "selab200_fir_probe": (_I, [_V, _V, _V, _U32, _I, _V]),
 }
 
 

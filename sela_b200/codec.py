@@ -11,8 +11,9 @@ error behaviour as in include/sela_b200.h):
                                     sela::Encoder::process + file::SelaFile::writeToFile, and
                                     file::SelaFile::readFromFile + sela::Decoder::processFrames,
                                     on the byte-packed .sela stream
-    encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, and its
-                                    order threshold and quantiser on chosen values
+    encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
+    / fir_probe                     order threshold and quantiser on chosen values, and its FIR residual
+                                    on chosen signals and predictors
 
 Everything computes on the GPU through the C ABI; NumPy only carries host buffers.
 The C++ mirror of the same interface (data::, frame::, file::, sela:: classes and
@@ -76,6 +77,21 @@ def quantise_probe(k, device=0):
     out = np.zeros((k.size, 4), np.int32)
     check(lib().selab200_quantise_probe(k.ctypes.data, k.size, out.ctypes.data))
     return out
+
+
+def fir_probe(samples, orders, c, wide, device=0):
+    """The encoder's FIR residual on chosen signals: samples int32 [n, 2048] (-32768..32767 as a channel row, or
+    |s| <= 65535 with wide=True as a 17-bit row), orders [n], c int64 [n, 101] (the Q35 predictor, c[:, 0] unused)
+    -> residues int32 [n, 2048]."""
+    init(device)
+    samples = _c(samples, np.int32).reshape(-1, FRAME)
+    n = samples.shape[0]
+    orders = _c(orders, np.int32).reshape(n)
+    c = _c(c, np.int64).reshape(n, MAX_ORDER + 1)
+    res = np.zeros((n, FRAME), np.int32)
+    check(lib().selab200_fir_probe(samples.ctypes.data, orders.ctypes.data, c.ctypes.data, n, int(bool(wide)),
+                                   res.ctypes.data))
+    return res
 
 
 def decode_frames(descs, words, channels, device=0):

@@ -1668,6 +1668,41 @@ int selab200_quantise_probe(const double *k, size_t n, int32_t *out)
     return 0;
 }
 
+int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                       int32_t *residues)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!samples || !orders || !c || !residues)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (n == 0)
+        return 0;
+    const int hi = wide ? 65535 : 32767, lo = wide ? -65535 : -32768;
+    for (size_t i = 0; i < (size_t)n * kFrame; i++)
+        if (samples[i] > hi || samples[i] < lo)
+            return fail(SELAB200_ERR_RANGE, "sample %zu = %d outside the domain of the row form", i, samples[i]);
+    for (uint32_t i = 0; i < n; i++)
+        if (orders[i] < 0 || orders[i] > kMaxOrder)
+            return fail(SELAB200_ERR_RANGE, "order %d of signal %u outside 0..%d", orders[i], i, kMaxOrder);
+    const size_t sig = (size_t)n * kFrame * 4, cb = (size_t)n * (kMaxOrder + 1) * 8;
+    if (int rc = g.in.ensure(sig)) return rc;
+    if (int rc = g.work.ensure(sig)) return rc;
+    if (int rc = g.aux.ensure(cb + (size_t)n * 4)) return rc;
+    long long *d_c = static_cast<long long *>(g.aux.ptr);
+    int32_t *d_orders = reinterpret_cast<int32_t *>(d_c + (size_t)n * (kMaxOrder + 1));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, samples, sig, cudaMemcpyHostToDevice, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(d_c, c, cb, cudaMemcpyHostToDevice, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(d_orders, orders, (size_t)n * 4, cudaMemcpyHostToDevice, g.stream));
+    k_fir_probe<<<n, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_orders, d_c, wide,
+                                        static_cast<int32_t *>(g.work.ptr));
+    if (int rc = launch_check("k_fir_probe"))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(residues, g.work.ptr, sig, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    return 0;
+}
+
 // ---------------------------------------------------------------- stages --
 
 int selab200_lpc_residues(const int32_t *samples, uint32_t n_sub, uint8_t *order, int32_t *q, int32_t *residues)

@@ -280,7 +280,13 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
         if (lane == 0)
             tr.order = order;
     }
-    warp_fir_residual(sig, cf, order, res);
+    // the digit planes of the FIR overlay k[] and the step-up row, dead now (the trace has copied k)
+    static_assert(kPlaneBytes <= kCoefAlias, "FIR digit planes");
+    uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
+    if (STEREO && role == 2)
+        warp_fir_residual<true>(sig, cf, order, planes, res);
+    else
+        warp_fir_residual<false>(sig, cf, order, planes, res);
 
     // ---- Rice: parameter search, then pack into this unit's slot ----
     const RiceChoice cq = warp_rice_choose(cf.q, order);
@@ -1033,6 +1039,24 @@ inline size_t synthesise_smem_bytes(uint32_t ch)
 
 // ------------------------------------------------------------ stage level --
 
+// A 17-bit signal staged as a Signal in static shared memory (the stage-level kernels): the row, the parity bits, and
+// kHistoryPad zeros in front of both.
+struct Row17 {
+    __align__(16) int16_t a[kHistoryPad + kFrame];
+    uint32_t lo[(kHistoryPad + kFrame) / 32];
+    __device__ __forceinline__ Signal stage(const int32_t *src)
+    {
+        const int lane = lane_id();
+        for (int i = lane; i < kHistoryPad / 2; i += 32)
+            reinterpret_cast<uint32_t *>(a)[i] = 0;
+        if (lane < kHistoryPad / 32)
+            lo[lane] = 0;
+        stage_17bit_row(src, a + kHistoryPad, lo + kHistoryPad / 32);
+        __syncwarp();
+        return Signal{a + kHistoryPad, lo + kHistoryPad / 32};
+    }
+};
+
 // lpc::ResidueGenerator::process for one signal per (1-warp) CTA; the means come from
 // k_unit_means<kMeanPlanar> over the same samples.
 __global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, const double *means, uint32_t n_sub,
@@ -1040,25 +1064,51 @@ __global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, con
 {
     __shared__ __align__(16) AnalysisScratch scratch;
     __shared__ __align__(16) CoefSmem cf;
-    __shared__ __align__(16) int32_t s_pad[kHistoryPad + kFrame];
+    __shared__ __align__(16) Row17 row;
     const uint32_t sub = blockIdx.x;
     const int lane = lane_id();
-    int32_t *s = s_pad + kHistoryPad;
-    for (int i = lane; i < kHistoryPad; i += 32)
-        s_pad[i] = 0;
-    for (int i = lane; i < kFrame; i += 32)
-        s[i] = samples[(size_t)sub * kFrame + i];
-    __syncwarp();
-    PlainSignal sig{s};
+    const Signal sig = row.stage(samples + (size_t)sub * kFrame);
     warp_autocorrelation(sig, scratch, means[sub]);
     warp_schur(scratch);
     const int order = warp_order_and_quantise(scratch, cf);
     warp_coefficients(cf, scratch.t(), order);
-    warp_fir_residual(sig, cf, order, residues + (size_t)sub * kFrame);
+    warp_fir_residual<true>(sig, cf, order, reinterpret_cast<uint32_t *>(scratch.ring), residues + (size_t)sub * kFrame);
     for (int i = lane; i < kMaxOrder; i += 32)
         q_out[(size_t)sub * kMaxOrder + i] = i < order ? cf.q[i] : 0;
     if (lane == 0)
         order_out[sub] = (uint8_t)order;
+}
+
+// selab200_fir_probe: the encoder's FIR on chosen samples and predictors, a warp per signal.  wide = 0: the int16 row
+// of a channel unit (|s| <= 32767), else the row + parity bits of a 17-bit unit (|s| <= 65535).
+__global__ void __launch_bounds__(32) k_fir_probe(const int32_t *samples, const int32_t *orders, const long long *c,
+                                                  int wide, int32_t *residues)
+{
+    __shared__ __align__(16) AnalysisScratch scratch;
+    __shared__ __align__(16) CoefSmem cf;
+    __shared__ __align__(16) Row17 row;
+    const uint32_t sub = blockIdx.x;
+    const int lane = lane_id();
+    const int32_t *src = samples + (size_t)sub * kFrame;
+    Signal sig = row.stage(src);
+    if (!wide) {
+        for (int j = lane; j < kFrame; j += 32)
+            row.a[kHistoryPad + j] = (int16_t)src[j];
+        sig.lo = nullptr;
+    }
+    const int order = orders[sub];
+    for (int i = lane; i < 112; i += 32) { // c[1..order] as the step-up leaves it: zero past the order
+        const long long v = i < order ? c[(size_t)sub * (kMaxOrder + 1) + i + 1] : 0;
+        cf.clo[i] = (uint32_t)v;
+        cf.chi[i] = (int32_t)(v >> 32);
+    }
+    __syncwarp();
+    uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
+    int32_t *res = residues + (size_t)sub * kFrame;
+    if (wide)
+        warp_fir_residual<true>(sig, cf, order, planes, res);
+    else
+        warp_fir_residual<false>(sig, cf, order, planes, res);
 }
 
 // lpc::SampleGenerator::process for one signal per (1-warp) CTA.

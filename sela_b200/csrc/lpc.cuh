@@ -329,81 +329,170 @@ __device__ void warp_coefficients(CoefSmem &cf, double *t, int order)
     __syncwarp();
 }
 
-// Signals hand the filters 8 consecutive samples at a time, biased by 2^17 so that
-// they are non-negative 18-bit numbers: c*s' then needs one IMAD.WIDE.U32 (low word)
-// and one IMAD (high word), and the bias is taken out once per output:
-//   sum_j c[j]*s[i-j] = sum_j c[j]*s'[i-j] - 2^17 * sum_j c[j].
-// The IIR below does the same with a bias of 2^31 (kSynthBias): decoded samples can be
-// any int32, and s + 2^31 covers all of them with a 32-bit unsigned s'.  Products and
-// sums then wrap mod 2^64, which cancels exactly: the result is the reference's int64
-// sum wherever that sum does not overflow.
-// Group g covers samples [8g, 8g+8); negative groups (history before the frame) read
-// the zero padding in front of every channel, i.e. s = 0, as the reference's warm-up
-// loop implies.
 // ---------------------------------------------------------------------------
 // K3: integer FIR residual.  generateResidues (residue_generator.cpp:98-119):
 //   r[i] = s[i] - (int32)((2^34 + sum_{j=1..order} c[j]*s[i-j]) >> 35),  s[<0] = 0
-// Integer adds wrap identically in any order.  Lane l computes 8 consecutive outputs
-// per pass with a 16-sample register window that slides 8 taps per iteration: per 64
-// multiply-accumulates the lane issues 128 IMADs, one 16-byte sample load and four
-// broadcast coefficient loads.
-template <typename Sig>
-__device__ void warp_fir_residual(const Sig &sig, const CoefSmem &cf, int order, int32_t *res)
-{
-    const int lane = lane_id();
-    const int nblk = (order + 7) >> 3;
-    long long csum = 0;
-    for (int j = lane + 1; j <= order; j += 32)
-        csum += coef_at(cf, j);
-    csum = (long long)warp_sum_u64((unsigned long long)csum);
-    const unsigned long long corr = (1ull << (kQ - 1)) - ((unsigned long long)csum << 17);
-    const uint4 *clo4 = reinterpret_cast<const uint4 *>(cf.clo);
-    const int4 *chi4 = reinterpret_cast<const int4 *>(cf.chi);
+// on the tensor cores.  With the outputs folded as i = 8a + b (a < 256, b < 8) the Toeplitz product is a GEMM,
+//   Y[a][b] = sum_m A[a][m] * B[m][b],   A[a][m] = s[8a + 7 - m],   B[m][b] = c[m + b - 7] (0 outside 1..order),
+// over K = order + 8 rounded up to 32: 1-4 k-steps of mma.sync m16n8k32 for each of the 16 M-tiles (16 rows a,
+// 128 outputs) of a signal.  It is made exact with byte limbs:
+//  - a coefficient is split into L signed digits, c = sum_{p<L} e_p * 256^p (mod 2^64) with e_p in [-128, 128):
+//    e_p is byte p of (c + H) ^ H, H = 0x8080...80.  L (0..8) is the largest number any tap needs, so it is the
+//    same for the whole warp;
+//  - a 16-bit sample is u8 + 256 * s8 (its two bytes); a 17-bit one is u8 + 256 * u8 + 65536 * s8 (the top limb
+//    is 0 or -1);
+//  - all limb products of weight 256^k (k < 8) go into one int32 accumulator T[k]: at most 3 * 128 products of
+//    magnitude <= 255 * 128, so |T[k]| < 2^24 and every T[k] is exact;
+//  - the sum is sum_k T[k] * 256^k, formed mod 2^64; weights 256^k with k >= 8 are multiples of 2^64.
+// So every int64 coefficient, saturated ones included, gives the same sum mod 2^64 as the reference's int64
+// arithmetic: bit-identical residues.  Integer adds wrap identically in any order.
+// Group g = lane / 4 and t = lane % 4 of the mma fragments: the A-register of rows (a, m..m+3), m = 4t (+16), holds
+// samples 8a + 4 - m .. 8a + 7 - m in reverse order -- one 8-byte load at a 4-aligned sample, bytes picked by PRMT.
+// The B-register of column g, rows m..m+3, holds e_p(c[m + g - 7 ..]): 4 bytes at offset m + g of digit plane p.
+constexpr int kPlaneWords = 34; // a digit plane: bytes x = m + b < 135 of B, byte x = e_p(c[x - 7])
+constexpr size_t kPlaneBytes = 8 * kPlaneWords * 4;
 
-    for (int pass = 0; pass < kFrame / 256; pass++) {
-        const int g0 = pass * 32 + lane;
-        uint32_t hi[8], own[8];
-        sig.load8(g0, hi);
+// The digit planes of c[1..112] into planes[8][kPlaneWords]; returns L.  planes may overlay anything but cf once
+// every lane is past its last read of it (the __syncwarp below).
+__device__ int warp_fir_planes(const CoefSmem &cf, uint32_t *planes)
+{
+    const unsigned long long H = 0x8080808080808080ull;
+    const int lane = lane_id();
+    __syncwarp();
+    int nd = 0;
+    for (int w = lane; w < kPlaneWords; w += 32) {
+        unsigned long long e[4];
 #pragma unroll
-        for (int r = 0; r < 8; r++)
-            own[r] = hi[r];
-        unsigned long long alo[8];
-        uint32_t ahi[8];
-#pragma unroll
-        for (int r = 0; r < 8; r++) {
-            alo[r] = 0;
-            ahi[r] = 0;
+        for (int i = 0; i < 4; i++) {
+            const int j = 4 * w + i - 7;
+            const unsigned long long c = (j >= 1 && j <= 112) ? (unsigned long long)coef_at(cf, j) : 0ull;
+            e[i] = (c + H) ^ H;
+            nd = max(nd, (64 - __clzll((long long)e[i]) + 7) >> 3);
         }
-        for (int t = 0; t < nblk; t++) {
-            uint32_t lo[8];
-            sig.load8(g0 - t - 1, lo);
-            const uint4 l0 = clo4[2 * t], l1 = clo4[2 * t + 1];
-            const int4 h0 = chi4[2 * t], h1 = chi4[2 * t + 1];
-            const uint32_t cl[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-            const int32_t ch[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
 #pragma unroll
-            for (int tau = 0; tau < 8; tau++) {
+        for (int p = 0; p < 8; p++) {
+            uint32_t v = 0;
 #pragma unroll
-                for (int r = 0; r < 8; r++) {
-                    const int idx = 7 + r - tau; // window position of s[i0 + r - (8t + 1 + tau)]
-                    const uint32_t w = idx < 8 ? lo[idx] : hi[idx - 8];
-                    alo[r] = mad_wide_u32(cl[tau], w, alo[r]);
-                    ahi[r] += (uint32_t)ch[tau] * w;
+            for (int i = 0; i < 4; i++)
+                v |= (uint32_t)((e[i] >> (8 * p)) & 0xffu) << (8 * i);
+            planes[p * kPlaneWords + w] = v;
+        }
+    }
+    __syncwarp();
+    return __reduce_max_sync(kFull, nd);
+}
+
+__device__ __forceinline__ uint32_t prmt(uint32_t x, uint32_t y, uint32_t sel) // selector bit 3: replicate the sign
+{
+    uint32_t d;
+    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(y), "r"(sel));
+    return d;
+}
+
+// d += A * B on one m16n8k32 tile: A bytes unsigned or signed, B bytes signed.
+template <bool ASIGNED>
+__device__ __forceinline__ void mma_s8(int32_t (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    if constexpr (ASIGNED)
+        asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+    else
+        asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+__device__ __forceinline__ unsigned long long mad_wide_s32(int32_t a, int32_t b, unsigned long long c)
+{
+    unsigned long long d;
+    asm("mad.wide.s32 %0, %1, %2, %3;" : "=l"(d) : "r"(a), "r"(b), "l"(c));
+    return d;
+}
+
+// WIDE: sig is a 17-bit signal (sig.lo != nullptr).  planes: 1088 bytes of scratch (see warp_fir_planes).
+template <bool WIDE>
+__device__ void warp_fir_residual(const Signal &sig, const CoefSmem &cf, int order, uint32_t *planes, int32_t *res)
+{
+    constexpr int NL = WIDE ? 3 : 2; // sample limbs: u8, (u8,) s8
+    const int lane = lane_id();
+    const int g = lane >> 2, t = lane & 3;
+    const int nd = warp_fir_planes(cf, planes);
+    const int ksteps = (order + 8 + 31) >> 5;
+    const uint32_t *pg = planes + t + (g >> 2); // word of byte 4t + g of a plane; shifted by 8 * (g & 3) bits
+    const uint32_t sh = 8 * (g & 3);
+    for (int mt = 0; mt < kFrame / 128; mt++) {
+        int32_t T[8][4];
+#pragma unroll
+        for (int k = 0; k < 8; k++)
+            T[k][0] = T[k][1] = T[k][2] = T[k][3] = 0;
+        for (int ks = 0; ks < ksteps; ks++) {
+            // A-registers 0..3: rows a = 16mt + g (+8), k = 32ks + 4t (+16): samples from s0 + kOff[r]
+            const int s0 = 128 * mt + 8 * g + 4 - 4 * t - 32 * ks;
+            constexpr int kOff[4] = {0, 64, -16, 48};
+            uint32_t A[NL][4];
+#pragma unroll
+            for (int r = 0; r < 4; r++) {
+                const int j = s0 + kOff[r];
+                const uint2 v = *reinterpret_cast<const uint2 *>(sig.a + j);
+                if constexpr (WIDE) {
+                    // d = 2h + p: the bytes of 2h (bit 15 of the lower h moves into bit 0 of the upper one: masked),
+                    // the parity bits p[j + 3 - i] into bit 0 of byte i, and the sign of h as the top limb
+                    const uint32_t x = v.x << 1, y = v.y << 1;
+                    const uint32_t nib = (sig.lo[j >> 5] >> (j & 31)) & 0xfu;
+                    const uint32_t par = ((nib * 0x08040201u) >> 3) & 0x01010101u;
+                    A[0][r] = (prmt(x, y, 0x0246) & 0xfefefefeu) | par;
+                    A[1][r] = prmt(x, y, 0x1357);
+                    A[2][r] = prmt(v.x, v.y, 0x9bdf);
+                } else {
+                    A[0][r] = prmt(v.x, v.y, 0x0246);
+                    A[1][r] = prmt(v.x, v.y, 0x1357);
                 }
             }
+            const uint32_t *pk = pg + 8 * ks;
 #pragma unroll
-            for (int r = 0; r < 8; r++)
-                hi[r] = lo[r];
+            for (int p = 0; p < 8; p++) {
+                if (p < nd) {
+                    const uint32_t *w = pk + p * kPlaneWords;
+                    const uint32_t b0 = __funnelshift_r(w[0], w[1], sh);
+                    const uint32_t b1 = __funnelshift_r(w[4], w[5], sh);
+                    // limb l of the sample has weight 256^l: its products with e_p go to T[p + l]
+                    mma_s8<false>(T[p], A[0], b0, b1);
+                    if (p + 1 < 8)
+                        mma_s8<!WIDE>(T[p + 1], A[1], b0, b1);
+                    if constexpr (WIDE)
+                        if (p + 2 < 8)
+                            mma_s8<true>(T[p + 2], A[2], b0, b1);
+                }
+            }
         }
-        int32_t out[8];
+        // T[k][r]: output i = 128mt + 8g + 2t + (r & 1) + 64 * (r >> 1)
+        const int i0 = 128 * mt + 8 * g + 2 * t;
 #pragma unroll
-        for (int r = 0; r < 8; r++) {
-            const unsigned long long p = alo[r] + ((unsigned long long)ahi[r] << 32) + corr;
-            out[r] = ((int)own[r] - kSampleBias) - (int32_t)((long long)p >> kQ);
+        for (int h = 0; h < 2; h++) {
+            const int i = i0 + 64 * h;
+            const uint32_t pair = *reinterpret_cast<const uint32_t *>(sig.a + i);
+            int s[2] = {(int)(pair << 16) >> 16, (int)pair >> 16};
+            if constexpr (WIDE) {
+                const uint32_t bits = sig.lo[i >> 5] >> (i & 31);
+                s[0] = 2 * s[0] + (int)(bits & 1u);
+                s[1] = 2 * s[1] + (int)((bits >> 1) & 1u);
+            }
+            int32_t out[2];
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int r = 2 * h + e;
+                unsigned long long sum = 1ull << (kQ - 1);
+#pragma unroll
+                for (int k = 0; k < 4; k++)
+                    sum = mad_wide_s32(T[k][r], 1 << (8 * k), sum);
+                const uint32_t top = (uint32_t)T[4][r] + ((uint32_t)T[5][r] << 8) + ((uint32_t)T[6][r] << 16) +
+                                     ((uint32_t)T[7][r] << 24); // weights 2^32 .. 2^56: only the high word
+                sum += (unsigned long long)top << 32;
+                out[e] = s[e] - (int32_t)((long long)sum >> kQ);
+            }
+            *reinterpret_cast<int2 *>(res + i) = make_int2(out[0], out[1]);
         }
-        int4 *dst = reinterpret_cast<int4 *>(res + 8 * g0);
-        dst[0] = make_int4(out[0], out[1], out[2], out[3]);
-        dst[1] = make_int4(out[4], out[5], out[6], out[7]);
     }
     __syncwarp();
 }
@@ -412,6 +501,12 @@ __device__ void warp_fir_residual(const Sig &sig, const CoefSmem &cf, int order,
 // K6: integer IIR synthesis.  SampleGenerator::generateSamples
 // (src/lpc/sample_generator.cpp:11-30):
 //   s[i] = r[i] - (int)((2^34 - sum_{j=1..order} c[j]*s[i-j]) >> 35),  s[<0] = 0
+// Decoded samples can be any int32: they enter the products biased by 2^31 (kSynthBias), so that
+// c*s' needs one IMAD.WIDE.U32 (low word of c) and one IMAD (high word), and the bias is taken
+// out once per output (the prefix table below):
+//   sum_j c[j]*s[i-j] = sum_j c[j]*s'[i-j] - 2^31 * sum_j c[j].
+// Products and sums wrap mod 2^64, which cancels exactly: the result is the reference's int64
+// sum wherever that sum does not overflow.
 // A true recurrence, evaluated in TRANSPOSED form: lane l owns taps TPL*l+1..TPL*l+TPL
 // and the partial sums of the outputs those taps will feed next.  When s[i] becomes
 // known every lane adds c[j]*s'[i] to the accumulator of output i+j; the accumulator
