@@ -15,19 +15,22 @@
 //                           the next lane's boundaries are the true ones.  A prefix sum of the
 //                           per-lane symbol counts then names the lane (and, through sparse
 //                           checkpoints, the bit) where symbol t*2048/S begins.
-//   k_rice_decode_vs        one lane per virtual stream, decoding values.
+//   k_rice_decode_vc        one lane per virtual stream, decoding values.
 //
-// Both kernels read the stream the same way: every lane owns a small ring in shared memory that it tops
-// up itself with 16-byte cp.async copies (no cooperation, no registers held across the load latency),
-// and parses from a three-word register window, so that no shared-memory load sits on the
-// symbol-to-symbol dependency chain.  The decoder stages its values in a shared tile and writes them as
+// Both kernels parse from a three-word register window over a ring in shared memory, so that no
+// shared-memory load sits on the symbol-to-symbol dependency chain; they fill their rings differently.
+// In the split index every lane owns a small ring that it tops up itself with 16-byte cp.async copies
+// (VsStream: no cooperation, no registers held across the load latency) and reads the words as they lie
+// in memory.  The decoder's rings are topped up by the whole warp together, eight lanes copying one
+// ring's next 128-byte segment (VsCoopStream), and bit-reversed in place once landed, so that its value
+// parser reads the stream MSB first.  The decoder stages its values in a shared tile and writes them as
 // whole row segments (128-byte lines) instead of one 16-byte store per lane.
 //
 // Nothing is taken on trust: part l must end exactly where the table says part l+1 begins (part 0
 // starts at bit 0, so by induction every part is the sequential parse); a stream that fails that
 // check, cannot be split, or meets a symbol the fast paths do not handle is flagged, and the
 // general lane-per-stream kernel (k_rice_decode, rice.cuh) decodes it again afterwards.  With S = 1
-// the second kernel alone is the large-batch decoder.
+// the decoder alone is the large-batch decoder.
 #pragma once
 
 #include "rice.cuh"
@@ -80,14 +83,16 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr)
     return v;
 }
 
-// ------------------------------------------------------------------ the lane's ring --
+// ------------------------------------------------------------------ the split index's ring --
 //
-// RING words in one row of shared memory, word w of the stream (counted from its 16-byte aligned base) at
-// byte ((4w + rot) & (4*RING - 1)) of the row; rot = 16 * lane spreads the lanes over the banks.  Rows are
-// 4*RING-aligned in the shared window: addresses are formed with OR.
-template <int RING>
+// kSplitRing words in one row of shared memory, word w of the stream (counted from its 16-byte aligned base)
+// at byte ((4w + rot) & (4*kSplitRing - 1)) of the row; rot = 16 * lane spreads the lanes over the banks.
+// Rows are 4*kSplitRing-aligned in the shared window: addresses are formed with OR.
+constexpr int kSplitRing = 32;  // words per lane
+constexpr int kSplitRound = 16; // symbols parsed between two top-ups
+
 struct VsRing {
-    static constexpr uint32_t kMask = RING * 4 - 1;
+    static constexpr uint32_t kMask = kSplitRing * 4 - 1;
     uint32_t row, rot;  // shared-space byte address of the row; rotation
     const uint4 *gvec;  // the stream from its 16-byte aligned base
     int total_bytes;    // bytes from gvec to the end of the stream; everything behind reads as zero
@@ -105,34 +110,6 @@ struct VsRing {
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(reinterpret_cast<const char *>(gvec) + (sz ? off : 0u)), "r"(sz) : "memory");
         }
     }
-    // The value parser wants the stream MSB first (a leading-zero count finds the terminator, the payload
-    // reads as a number); the words are reversed once, in place, when their vector has landed -- one BREV per
-    // word instead of one per symbol.  (Behind an inline-asm shared load ptxas lowers BREV to three instructions;
-    // VsCoopStream::reverse_list uses plain loads for that reason.)
-    __device__ __forceinline__ void reverse(uint32_t v) const
-    {
-        const uint32_t a = row | ((16 * v + rot) & kMask);
-        uint32_t x, y, z, w;
-        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(a));
-        x = __brev(x), y = __brev(y), z = __brev(z), w = __brev(w);
-        asm volatile("st.shared.v4.u32 [%4], {%0, %1, %2, %3};" ::"r"(x), "r"(y), "r"(z), "r"(w), "r"(a) : "memory");
-    }
-    // vectors [lo, hi): two loads in flight before the first BREV
-    __device__ __forceinline__ void reverse_range(uint32_t lo, uint32_t hi) const
-    {
-        for (; lo + 1 < hi; lo += 2) {
-            const uint32_t a = row | ((16 * lo + rot) & kMask), b = row | ((16 * lo + 16 + rot) & kMask);
-            uint32_t x0, y0, z0, w0, x1, y1, z1, w1;
-            asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(x0), "=r"(y0), "=r"(z0), "=r"(w0) : "r"(a));
-            asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(x1), "=r"(y1), "=r"(z1), "=r"(w1) : "r"(b));
-            x0 = __brev(x0), y0 = __brev(y0), z0 = __brev(z0), w0 = __brev(w0);
-            asm volatile("st.shared.v4.u32 [%4], {%0, %1, %2, %3};" ::"r"(x0), "r"(y0), "r"(z0), "r"(w0), "r"(a) : "memory");
-            x1 = __brev(x1), y1 = __brev(y1), z1 = __brev(z1), w1 = __brev(w1);
-            asm volatile("st.shared.v4.u32 [%4], {%0, %1, %2, %3};" ::"r"(x1), "r"(y1), "r"(z1), "r"(w1), "r"(b) : "memory");
-        }
-        if (lo < hi)
-            reverse(lo);
-    }
 };
 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
@@ -140,22 +117,20 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // The streaming state of a lane: a window of three words in registers (r0 = word wb - 1 holds the current
-// bit, r1, and r2 loaded one word ahead of its first use) over the ring.  ROUND symbols of at most 32 bits
-// are parsed between two boundaries; at a boundary the ring is topped up as far as the words still needed
-// allow, and the copies issued at the previous boundary are retired (and, for the value parser, reversed).
-// A round reads at most ROUND + 2 words past r1.  With RING >= 2 * ROUND + 16 what landed a boundary ago
-// always covers that; a smaller ring (half the shared memory, twice the warps per SM) covers it for
-// ordinary streams and otherwise waits for the copies just issued (RING >= ROUND + 16 suffices then).
-template <int RING, int ROUND, bool REVERSED>
+// bit, r1, and r2 loaded one word ahead of its first use) over the ring.  kSplitRound symbols of at most 32
+// bits are parsed between two boundaries; at a boundary the ring is topped up as far as the words still needed
+// allow, and the copies issued at the previous boundary are retired.  A round reads at most kSplitRound + 2
+// words past r1.  What landed a boundary ago covers that for ordinary streams; in a dense stretch the boundary
+// also waits for the copies just issued (a ring of kSplitRound + 16 words suffices then).
 struct VsStream {
-    static_assert(RING >= ROUND + 16 && (RING & (RING - 1)) == 0, "ring too small for the round");
-    VsRing<RING> rg;
+    static_assert(kSplitRing >= kSplitRound + 16 && (kSplitRing & (kSplitRing - 1)) == 0, "ring too small for the round");
+    VsRing rg;
     uint32_t pos;         // current bit, counted from the aligned base
     uint32_t r0, r1, r2;  // window
     uint32_t wa;          // running byte offset (rotated) of r2's word
-    uint32_t fv, rv;      // next vector to request / first vector not yet landed (and reversed)
+    uint32_t fv, rv;      // next vector to request / first vector not yet landed
     uint32_t cv_next;     // vectors below cv_next have been requested by the previous boundary
-    uint32_t ce;          // words below ce have landed (and are reversed)
+    uint32_t ce;          // words below ce have landed
 
     __device__ __forceinline__ uint32_t wb() const { return (pos >> 5) + 1; }
     __device__ __forceinline__ void load_window()
@@ -169,8 +144,6 @@ struct VsStream {
     __device__ __forceinline__ void retire(uint32_t upto) // vectors below `upto` have landed
     {
         if (upto > rv) {
-            if (REVERSED)
-                rg.reverse_range(rv, upto);
             rv = upto;
             ce = 4 * upto;
         }
@@ -181,14 +154,14 @@ struct VsStream {
         pos = p;
         const uint32_t w = wb();
         fv = rv = (w - 1) >> 2;
-        const uint32_t first = (w + ROUND + 2) >> 2; // last vector the first round can touch
+        const uint32_t first = (w + kSplitRound + 2) >> 2; // last vector the first round can touch
         while (fv <= first) {
             rg.issue(fv);
             fv++;
         }
         cp_async_commit();
         const uint32_t landed = fv;
-        const uint32_t lim = (w + RING - 5) >> 2; // vector v overwrites words [4v - RING, 4v - RING + 3]; below w - 1 all is dead
+        const uint32_t lim = (w + kSplitRing - 5) >> 2; // vector v overwrites words [4v - kSplitRing, 4v - kSplitRing + 3]; below w - 1 all is dead
         while (fv <= lim) {
             rg.issue(fv);
             fv++;
@@ -203,7 +176,7 @@ struct VsStream {
     __device__ __forceinline__ void boundary()
     {
         const uint32_t w = wb();
-        const uint32_t lim = (w + RING - 5) >> 2;
+        const uint32_t lim = (w + kSplitRing - 5) >> 2;
         while (fv <= lim) {
             rg.issue(fv);
             fv++;
@@ -212,7 +185,7 @@ struct VsStream {
         cp_async_wait<1>(); // everything but the group just committed has landed
         retire(cv_next);
         cv_next = fv;
-        if (RING < 2 * ROUND + 16 && ce < w + ROUND + 3) { // a dense stretch: the round may outrun what has landed
+        if (ce < w + kSplitRound + 3) { // a dense stretch: the round may outrun what has landed
             cp_async_wait<0>();
             retire(fv);
         }
@@ -223,15 +196,15 @@ struct VsStream {
         r0 = r1;
         r1 = r2;
         wa += 4;
-        r2 = lds_u32(rg.row | (wa & VsRing<RING>::kMask));
+        r2 = lds_u32(rg.row | (wa & VsRing::kMask));
     }
 };
 
 // ------------------------------------------------------------------ the warp's rings, filled together --
 //
 // The per-lane cp.async of VsStream costs a 16-byte request to 32 different lines per instruction: at scale
-// the load/store unit replays of those requests, not the parse, bound the decoder (an ablation with the
-// top-ups removed runs far faster).  Here the 32 rings of a warp are topped up COOPERATIVELY in
+// the load/store unit replays of those requests, not the parse, bound the decoder (with the top-ups removed
+// it ran far faster).  Here the 32 rings of a warp are topped up COOPERATIVELY in
 // 128-byte segments: a ring is two segments of 32 words; a lane whose parser has left a segment puts its
 // row on a list, and eight lanes copy one row's next segment (8 x 16 bytes = one whole line) -- four rows,
 // four lines per instruction instead of 32 -- and, when it has landed, reverse it the same way.  The copies
@@ -260,11 +233,13 @@ __device__ __forceinline__ uint32_t fma_sub(uint32_t a, uint32_t b) // a - b
     return d;
 }
 
-template <int ROUND, bool REVERSED, bool NOCOPY = false>
+constexpr int kVcRound = 16; // symbols a lane decodes between two top-ups of its ring
+constexpr int kVcTile = 32;  // symbols per lane staged in shared memory before they leave as 128-byte row segments
+
 struct VsCoopStream {
     static constexpr int kRing = 64, kSeg = 32;     // words
     static constexpr uint32_t kMask = kRing * 4 - 1;
-    static_assert(ROUND <= 16, "a round must not outrun one segment's slack");
+    static_assert(kVcRound <= 16, "a round must not outrun one segment's slack");
     uint32_t row, rot;     // this lane's ring row (shared byte address, 256-aligned) and rotation
     uint32_t rows0;        // shared byte address of the warp's row 0
     unsigned char *sbase;  // the kernel's dynamic shared memory as a pointer, and its shared byte address
@@ -337,31 +312,30 @@ struct VsCoopStream {
                 const unsigned long long src = (((unsigned long long)e.y << 32) | e.x) + (sz ? piece : 0u);
                 // the segment may wrap inside the row only at its end: it starts on a 128-byte boundary of the rotated row
                 const uint32_t dst = (e.w & ~kMask) | ((e.w + piece) & kMask);
-                if (!NOCOPY || sz == 77u)
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
             }
         }
         return n;
     }
     // The segments of list `which` have landed: the lanes that copied them reverse them, one 16-byte piece each
-    // (all 32 lanes busy -- a lane reversing its own whole segment would leave the other 31 idle).  Convergent.
+    // (all 32 lanes busy -- a lane reversing its own whole segment would leave the other 31 idle).  The value
+    // parser wants the stream MSB first (a leading-zero count finds the terminator, the payload reads as a
+    // number): one BREV per word here instead of one per symbol.  Convergent.
     __device__ __forceinline__ void reverse_list(int which, int n) const
     {
-        if (REVERSED) {
-            const int lane = lane_id();
-            const uint4 *list = meta->list[which];
-            const uint32_t piece = 16u * (lane & 7);
-            for (int it = 0; it * 4 < n; it++) {
-                const int idx = it * 4 + (lane >> 3);
-                if (idx < n) {
-                    const uint32_t w0 = list[idx].w;
-                    const uint32_t a = (w0 & ~kMask) | ((w0 + piece) & kMask);
-                    // (plain loads through the shared array: behind an inline-asm load ptxas lowers BREV to three instructions)
-                    uint4 *q = reinterpret_cast<uint4 *>(sbase + (a - s0));
-                    uint4 v = *q;
-                    v.x = __brev(v.x), v.y = __brev(v.y), v.z = __brev(v.z), v.w = __brev(v.w);
-                    *q = v;
-                }
+        const int lane = lane_id();
+        const uint4 *list = meta->list[which];
+        const uint32_t piece = 16u * (lane & 7);
+        for (int it = 0; it * 4 < n; it++) {
+            const int idx = it * 4 + (lane >> 3);
+            if (idx < n) {
+                const uint32_t w0 = list[idx].w;
+                const uint32_t a = (w0 & ~kMask) | ((w0 + piece) & kMask);
+                // (plain loads through the shared array: behind an inline-asm load ptxas lowers BREV to three instructions)
+                uint4 *q = reinterpret_cast<uint4 *>(sbase + (a - s0));
+                uint4 v = *q;
+                v.x = __brev(v.x), v.y = __brev(v.y), v.z = __brev(v.z), v.w = __brev(v.w);
+                *q = v;
             }
         }
         __syncwarp(); // reversed words visible to their owners; the list is free again
@@ -410,9 +384,9 @@ struct VsCoopStream {
         pending = ready;
         if (ready)
             fs++;
-        // A round reads at most ROUND + 2 words past r1.  A parser that entered its last landed segment late in
+        // A round reads at most kVcRound + 2 words past r1.  A parser that entered its last landed segment late in
         // a dense stretch needs the segment requested just now: wait for it (rare).
-        if (__any_sync(kFull, ready && ce < w + ROUND + 3)) {
+        if (__any_sync(kFull, ready && ce < w + kVcRound + 3)) {
             cp_async_wait<0>();
             __syncwarp();
             reverse_list(cur, n_cur);
@@ -439,25 +413,23 @@ __device__ __forceinline__ uint32_t cp_index(uint32_t j) { return j < 64 ? j >> 
 __device__ __forceinline__ uint32_t cp_count(uint32_t n) { return n == 0 ? 0u : cp_index(n - 1) + 1; } // checkpoints among symbols 0..n-1
 
 // Random access for the short walks (merge search, table look-up, the tail of a chunk, long symbols):
-// RING consecutive words at a time, fetched on demand.  Every earlier copy of the lane must have landed.
-template <int RING>
+// kSplitRing consecutive words at a time, fetched on demand.  Every earlier copy of the lane must have landed.
 struct VsReader {
-    VsRing<RING> rg;
+    VsRing rg;
     uint32_t base_w, end_w;
 };
-template <int RING>
-__device__ __noinline__ uint32_t reader_next_boundary(VsReader<RING> *rd, uint32_t total_bits, uint32_t q, uint32_t kp1)
+__device__ __noinline__ uint32_t reader_next_boundary(VsReader *rd, uint32_t total_bits, uint32_t q, uint32_t kp1)
 {
     while (q < total_bits) {
         const uint32_t w = q >> 5;
         if (w < rd->base_w || w + 1 >= rd->end_w) {
             const uint32_t fv0 = w >> 2;
-            for (uint32_t i = 0; i < RING / 4; i++)
+            for (uint32_t i = 0; i < kSplitRing / 4; i++)
                 rd->rg.issue(fv0 + i);
             cp_async_commit();
             cp_async_wait<0>();
             rd->base_w = 4 * fv0;
-            rd->end_w = rd->base_w + RING;
+            rd->end_w = rd->base_w + kSplitRing;
         }
         const uint32_t win = __funnelshift_r(rd->rg.word(w), rd->rg.word(w + 1), q);
         const uint32_t c = bfind_u32(~win & (win + 1)); // trailing ones; 0xffffffff: 32 or more
@@ -468,17 +440,17 @@ __device__ __noinline__ uint32_t reader_next_boundary(VsReader<RING> *rd, uint32
     return total_bits + kp1; // ran off the end: the zero padding terminates the run
 }
 
-template <int LOG2S, int RING, int ROUND>
+template <int LOG2S>
 __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams p)
 {
-    static_assert(ROUND % 4 == 0 && 64 % ROUND == 0, "geometry");
+    static_assert(kSplitRound % 4 == 0 && 64 % kSplitRound == 0, "geometry");
     constexpr int S = 1 << LOG2S;
     constexpr uint32_t kPart = kFrame >> LOG2S;
     extern __shared__ __align__(16) unsigned char split_smem[];
     const int lane = lane_id(), warp = warp_id();
     const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(split_smem);
-    const uint32_t pad = (RING * 4 - (smem0 & (RING * 4 - 1))) & (RING * 4 - 1);
-    uint16_t *cps = reinterpret_cast<uint16_t *>(split_smem + pad + kVsWarps * 32 * RING * 4) + (size_t)warp * kCpMax * 32;
+    const uint32_t pad = (kSplitRing * 4 - (smem0 & (kSplitRing * 4 - 1))) & (kSplitRing * 4 - 1);
+    uint16_t *cps = reinterpret_cast<uint16_t *>(split_smem + pad + kVsWarps * 32 * kSplitRing * 4) + (size_t)warp * kCpMax * 32;
 
     const uint32_t l = lane & (S - 1), gb = lane & ~(S - 1);
     const uint32_t st = ((blockIdx.x * kVsWarps + warp) * 32 + lane) >> LOG2S;
@@ -494,13 +466,12 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
     const uint32_t total = ok ? (uint32_t)d.res_words + skip : 0u; // words from the aligned base
     const uint32_t k = ok ? d.res_rice_param : 0u, kp1 = k + 1;
 
-    using Stream = VsStream<RING, ROUND, false>;
-    Stream s;
-    s.rg.row = smem0 + pad + (uint32_t)(warp * 32 + lane) * (RING * 4);
-    s.rg.rot = (16u * lane) & (RING * 4 - 1);
+    VsStream s;
+    s.rg.row = smem0 + pad + (uint32_t)(warp * 32 + lane) * (kSplitRing * 4);
+    s.rg.rot = (16u * lane) & (kSplitRing * 4 - 1);
     s.rg.gvec = reinterpret_cast<const uint4 *>(addr & ~(uintptr_t)15);
     s.rg.total_bytes = (int)(total * 4);
-    VsReader<RING> rd;
+    VsReader rd;
     rd.rg = s.rg;
     rd.base_w = rd.end_w = 0;
 
@@ -532,7 +503,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
             }
             uint32_t mx = 0;
 #pragma unroll
-            for (int e = 0; e < ROUND; e++) {
+            for (int e = 0; e < kSplitRound; e++) {
                 if (dense && (e & 3) == 0) { // uniform over the active lanes
                     const uint32_t rel = s.pos - cstart;
                     if (rel < 0xffffu)
@@ -555,8 +526,8 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
                 uint32_t q = pos_s;
                 bool crossed = false;
 #pragma unroll 1
-                for (int e = 0; e < ROUND; e++) {
-                    q = reader_next_boundary<RING>(&rd, total_bits, q, kp1);
+                for (int e = 0; e < kSplitRound; e++) {
+                    q = reader_next_boundary(&rd, total_bits, q, kp1);
                     crossed |= q >= cend;
                 }
                 if (crossed) {
@@ -564,18 +535,18 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
                     active = false;
                 } else {
                     s.prime(q);
-                    j += ROUND;
+                    j += kSplitRound;
                 }
-            } else if (s.pos >= cend || j + ROUND >= (uint32_t)kFrame + 64) {
+            } else if (s.pos >= cend || j + kSplitRound >= (uint32_t)kFrame + 64) {
                 s.pos = pos_s; // the chunk ends inside this round: the tail loop below finds where
                 active = false;
             } else {
-                j += ROUND;
+                j += kSplitRound;
             }
         }
     }
-    // One boundary forward, keeping the streaming state valid (a top-up every ROUND symbols); a symbol longer
-    // than the window goes through the on-demand reader and restarts the stream behind it.
+    // One boundary forward, keeping the streaming state valid (a top-up every kSplitRound symbols); a symbol
+    // longer than the window goes through the on-demand reader and restarts the stream behind it.
     uint32_t since = 0;
     auto step = [&]() {
         const uint32_t win = __funnelshift_r(s.r0, s.r1, s.pos);
@@ -583,7 +554,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
         if (ones + kp1 > 32u) {
             cp_async_wait<0>();
             rd.base_w = rd.end_w = 0;
-            const uint32_t q = reader_next_boundary<RING>(&rd, total_bits, s.pos, kp1);
+            const uint32_t q = reader_next_boundary(&rd, total_bits, s.pos, kp1);
             s.prime(q);
             since = 0;
         } else {
@@ -591,7 +562,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
             if ((s.pos ^ pn) >= 32u)
                 s.advance();
             s.pos = pn;
-            if (++since == ROUND) {
+            if (++since == kSplitRound) {
                 s.boundary();
                 since = 0;
             }
@@ -602,7 +573,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
     bool found = !(ok && cstart < cend);
     if (!found)
         s.load_window(); // back at the start of that round; the ring still holds it
-    for (int e = 0; e <= ROUND && __ballot_sync(kFull, !found); e++) {
+    for (int e = 0; e <= kSplitRound && __ballot_sync(kFull, !found); e++) {
         if (!found) {
             if (s.pos >= cend) {
                 found = true;
@@ -727,25 +698,19 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
     }
 }
 
-template <int RING>
-constexpr size_t split_smem_bytes()
-{
-    return RING * 4 + (size_t)kVsWarps * 32 * RING * 4 + (size_t)kVsWarps * kCpMax * 32 * 2;
-}
+constexpr size_t kSplitSmemBytes = kSplitRing * 4 + (size_t)kVsWarps * 32 * kSplitRing * 4 + (size_t)kVsWarps * kCpMax * 32 * 2;
 
 // --------------------------------------------------------------- virtual streams --
 //
-// Geometry (template parameters; the launch picks one):
-//   RING   words per lane in the shared-memory ring
-//   ROUND  symbols a lane decodes between two ring top-ups
-//   TILE   symbols per lane staged in shared memory before they leave as 4*TILE-byte row segments
+// One lane per virtual stream on the cooperative rings (VsCoopStream): kVcRound symbols between two top-ups,
+// kVcTile symbols per lane staged in a shared tile before they leave as 4*kVcTile-byte row segments.
 
-// General decode of `count` symbols from bit `pos`, ring words (reversed) only up to `ce` (exclusive).
-// Out of line: runs for the rare round that holds a symbol longer than one 32-bit window.
-// Returns false if it would need words the ring does not hold (the stream is then flagged).
-template <int RING>
-__device__ __noinline__ bool vs_slow_round(const VsRing<RING> rg, uint32_t ce, uint32_t *pos, uint32_t k, int32_t *dst, int count)
+// General decode of `count` symbols from bit `pos`, reading the lane's ring (its row and rotation; words
+// reversed) only up to word `ce` (exclusive).  Out of line: runs for the rare round that holds a symbol longer
+// than one 32-bit window.  Returns false if it would need words the ring does not hold (the stream is then flagged).
+__device__ __noinline__ bool vc_slow_round(uint32_t row, uint32_t rot, uint32_t ce, uint32_t *pos, uint32_t k, int32_t *dst, int count)
 {
+    const auto word = [row, rot](uint32_t w) { return lds_u32(row | ((4 * w + rot) & VsCoopStream::kMask)); };
     uint32_t q = *pos;
     for (int e = 0; e < count; e++) {
         uint32_t ones = 0;
@@ -753,7 +718,7 @@ __device__ __noinline__ bool vs_slow_round(const VsRing<RING> rg, uint32_t ce, u
             const uint32_t w = q >> 5;
             if (w + 2 > ce)
                 return false;
-            const uint32_t c = __clz(~__funnelshift_l(rg.word(w + 1), rg.word(w), q));
+            const uint32_t c = __clz(~__funnelshift_l(word(w + 1), word(w), q));
             ones += c;
             q += c;
             if (c < 32)
@@ -763,7 +728,7 @@ __device__ __noinline__ bool vs_slow_round(const VsRing<RING> rg, uint32_t ce, u
         const uint32_t w = q >> 5;
         if (w + 2 > ce)
             return false;
-        const uint32_t win = __funnelshift_l(rg.word(w + 1), rg.word(w), q);
+        const uint32_t win = __funnelshift_l(word(w + 1), word(w), q);
         const uint32_t pay = __funnelshift_rc(win, 0u, 32 - k);
         q += k;
         dst[e] = unzigzag((ones << k) | pay); // uint32 shift as in rice_decoder.cpp:37
@@ -774,151 +739,13 @@ __device__ __noinline__ bool vs_slow_round(const VsRing<RING> rg, uint32_t ce, u
     return true;
 }
 
-// ABLATE (measurement only; results are wrong): 1 = no global stores, 2 = no ring
-// top-ups after the first fill, 4 = no in-place reversal.
-template <int RING, int ROUND, int TILE, int ABLATE = 0>
-__global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vs(RiceVsParams p, int log2s)
-{
-    static_assert(TILE % ROUND == 0 && TILE % 4 == 0 && ROUND % 4 == 0 && TILE <= 32, "tile geometry");
-    constexpr int kTilePitch = TILE + 4;       // words: rows stay 16-byte aligned, banks rotate by 4 per row
-    constexpr int kRowLanes = TILE / 4;        // lanes that move one row segment (16 bytes each)
-    constexpr int kRowsPerIt = 32 / kRowLanes; // rows per store instruction
-    extern __shared__ __align__(16) unsigned char vs_smem[];
-    const int lane = lane_id(), warp = warp_id();
-    const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(vs_smem);
-    const uint32_t pad = (RING * 4 - (smem0 & (RING * 4 - 1))) & (RING * 4 - 1);
-    int32_t *tile = reinterpret_cast<int32_t *>(vs_smem + pad + kVsWarps * 32 * RING * 4) + warp * 32 * kTilePitch;
-
-    const uint32_t S = 1u << log2s, part = (uint32_t)kFrame >> log2s;
-    const uint32_t v0 = (blockIdx.x * kVsWarps + warp) * 32;
-    const uint32_t v = v0 + lane, st = v >> log2s, l = v & (S - 1);
-    const bool exists = st < p.n_sub;
-    selab200_subframe_desc d;
-    memset(&d, 0, sizeof d);
-    if (exists)
-        d = p.descs[st];
-    bool ok = exists && rice_desc_ok(d, p.channels, p.n_words);
-    if (exists && !ok && l == 0)
-        raise_status(p.status, SELAB200_ERR_BITSTREAM);
-    const bool store_row = ok; // rows of flagged streams may hold garbage: the general kernel rewrites them
-    uint32_t sb = 0, expect_end = kNoSplit;
-    if (ok && S > 1) {
-        const uint32_t *tb = p.table + (size_t)st * (S - 1);
-        if (tb[0] == kNoSplit) {
-            ok = false; // not split: the general kernel decodes it
-        } else {
-            if (l > 0)
-                sb = tb[l - 1];
-            if (l < S - 1)
-                expect_end = tb[l];
-        }
-    }
-    const uintptr_t addr = reinterpret_cast<uintptr_t>(p.words + (ok ? d.res_offset : 0));
-    const uint32_t skip = (uint32_t)(addr >> 2) & 3u;
-    const uint32_t total = ok && d.res_words ? (uint32_t)d.res_words + skip : 0u;
-    using Stream = VsStream<RING, ROUND, !(ABLATE & 4)>;
-    Stream s;
-    s.rg.row = smem0 + pad + (uint32_t)(warp * 32 + lane) * (RING * 4);
-    s.rg.rot = (16u * lane) & (RING * 4 - 1);
-    s.rg.gvec = reinterpret_cast<const uint4 *>(addr & ~(uintptr_t)15);
-    s.rg.total_bytes = (int)(total * 4);
-    const uint32_t k = ok ? d.res_rice_param : 0u, kp1 = k + 1, kk = 32 - k, kpow = 1u << k;
-    const uint32_t row_mask = __ballot_sync(kFull, store_row);
-
-    uint32_t p0 = sb + 32 * skip;
-    if (p0 > total * 32 + 64)
-        p0 = total * 32 + 64; // a nonsense table entry: parse zeros, fail the end check
-    s.prime(p0);
-    bool dead = false;
-
-    int32_t *out_warp = p.out + (size_t)v0 * part;
-    const uint32_t n_rounds = part / ROUND;
-    const uint32_t c_pn = kp1 + 31;
-#pragma unroll 1
-    for (uint32_t r = 0; r < n_rounds; r++) {
-        if (r && !dead && !(ABLATE & 2))
-            s.boundary();
-        uint32_t pos_s = s.pos;
-        int mn = 31; // lowest FLO result of the round; below k: a symbol longer than the window
-        int32_t *trow = tile + lane * kTilePitch + (r % (TILE / ROUND)) * ROUND;
-#pragma unroll
-        for (int e4 = 0; e4 < ROUND; e4 += 4) {
-            int32_t val[4];
-#pragma unroll
-            for (int e = 0; e < 4; e++) {
-                const uint32_t win = __funnelshift_l(s.r1, s.r0, s.pos);
-                const uint32_t f = bfind_u32(~win);   // 31 - ones; 0xffffffff: the window is all ones
-                const uint32_t pn = s.pos + c_pn - f; // pos + ones + 1 + k
-                mn = min(mn, (int)f);
-                const uint32_t ones = 31 - f;
-                const uint32_t t = __funnelshift_lc(0u, win, ones + 1);
-                const uint32_t pay = __funnelshift_rc(t, 0u, kk);
-                val[e] = unzigzag3(ones * kpow + pay);
-                if ((s.pos ^ pn) >= 32u)
-                    s.advance();
-                s.pos = pn;
-            }
-            *reinterpret_cast<int4 *>(trow + e4) = make_int4(val[0], val[1], val[2], val[3]);
-        }
-        if (mn < (int)k && !dead && !(ABLATE & 6)) { // a symbol longer than the window: redo the round with the general parser
-            if (vs_slow_round<RING>(s.rg, s.ce, &pos_s, k, trow, ROUND)) {
-                s.pos = pos_s;
-                s.load_window();
-            } else {
-                dead = true;
-            }
-        }
-        // ---- a full tile: TILE symbols per lane leave as row segments of 4*TILE bytes ----
-        if (r % (TILE / ROUND) == TILE / ROUND - 1) {
-            __syncwarp();
-            int32_t *dst = out_warp + (size_t)(r / (TILE / ROUND)) * TILE + (lane % kRowLanes) * 4;
-#pragma unroll
-            for (int it = 0; it < 32 / kRowsPerIt; it++) {
-                const int row = kRowsPerIt * it + lane / kRowLanes;
-                if ((row_mask >> row) & 1u) {
-                    const int4 q = *reinterpret_cast<const int4 *>(tile + row * kTilePitch + (lane % kRowLanes) * 4);
-                    if (!(ABLATE & 1) || q.x == 0x7fffffff)
-                        *reinterpret_cast<int4 *>(dst + (size_t)row * part) = q;
-                }
-            }
-            __syncwarp();
-        }
-    }
-    cp_async_wait<0>();
-    if (exists && store_row) {
-        bool bad = dead;
-        if (ok) {
-            if (expect_end != kNoSplit)
-                bad |= s.pos - 32 * skip != expect_end;
-            else
-                bad |= s.pos > total * 32;
-        }
-        if (bad && !(ABLATE & 6))
-            p.flags[st] = 1u; // (several parts may say so: idempotent)
-    }
-}
-
-// The decoder on the cooperative rings (VsCoopStream): same parse, same tile, warp-wide top-ups.
-template <int RING>
-__device__ __noinline__ bool vc_slow_round(uint32_t row, uint32_t rot, uint32_t ce, uint32_t *pos, uint32_t k, int32_t *dst, int count)
-{
-    VsRing<RING> rg;
-    rg.row = row;
-    rg.rot = rot;
-    rg.gvec = nullptr;
-    rg.total_bytes = 0;
-    return vs_slow_round<RING>(rg, ce, pos, k, dst, count);
-}
-
-template <int ROUND, int TILE, int ABLATE = 0>
 __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p, int log2s)
 {
-    using Stream = VsCoopStream<ROUND, !(ABLATE & 4), (ABLATE & 8) != 0>;
-    constexpr int RING = Stream::kRing;
-    static_assert(TILE % ROUND == 0 && TILE % 4 == 0 && ROUND % 4 == 0 && TILE <= 128, "tile geometry");
-    constexpr int kTilePitch = TILE + 4;
-    constexpr int kRowLanes = TILE / 4;
-    constexpr int kRowsPerIt = 32 / kRowLanes;
+    constexpr int RING = VsCoopStream::kRing;
+    static_assert(kVcTile % kVcRound == 0 && kVcTile % 4 == 0 && kVcRound % 4 == 0 && kVcTile <= 128, "tile geometry");
+    constexpr int kTilePitch = kVcTile + 4;    // words: rows stay 16-byte aligned, banks rotate by 4 per row
+    constexpr int kRowLanes = kVcTile / 4;     // lanes that move one row segment (16 bytes each)
+    constexpr int kRowsPerIt = 32 / kRowLanes; // rows per store instruction
     extern __shared__ __align__(16) unsigned char vc_smem[];
     const int lane = lane_id(), warp = warp_id();
     const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(vc_smem);
@@ -953,7 +780,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
     const uintptr_t addr = reinterpret_cast<uintptr_t>(p.words + (ok ? d.res_offset : 0));
     const uint32_t skip = (uint32_t)(addr >> 2) & 3u;
     const uint32_t total = ok && d.res_words ? (uint32_t)d.res_words + skip : 0u;
-    Stream s;
+    VsCoopStream s;
     s.setup(vc_smem, smem0 + pad + (uint32_t)(warp * 32) * (RING * 4), meta, reinterpret_cast<const uint4 *>(addr & ~(uintptr_t)15), (int)(total * 4));
     const uint32_t k = ok ? d.res_rice_param : 0u, kp1 = k + 1, kk = 32 - k, kpow = 1u << k;
     const uint32_t row_mask = __ballot_sync(kFull, store_row);
@@ -965,17 +792,17 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
     bool dead = false;
 
     int32_t *out_warp = p.out + (size_t)v0 * part;
-    const uint32_t n_rounds = part / ROUND;
+    const uint32_t n_rounds = part / kVcRound;
     const uint32_t c_pn = kp1 + 31;
 #pragma unroll 1
     for (uint32_t r = 0; r < n_rounds; r++) {
-        if (r && !(ABLATE & 2))
+        if (r)
             s.boundary(!dead);
         uint32_t pos_s = s.pos;
         int mn = 31; // lowest FLO result of the round; below k: a symbol longer than the window
-        int32_t *trow = tile + lane * kTilePitch + (r % (TILE / ROUND)) * ROUND;
+        int32_t *trow = tile + lane * kTilePitch + (r % (kVcTile / kVcRound)) * kVcRound;
 #pragma unroll
-        for (int e4 = 0; e4 < ROUND; e4 += 4) {
+        for (int e4 = 0; e4 < kVcRound; e4 += 4) {
             int32_t val[4];
 #pragma unroll
             for (int e = 0; e < 4; e++) {
@@ -993,8 +820,8 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
             }
             *reinterpret_cast<int4 *>(trow + e4) = make_int4(val[0], val[1], val[2], val[3]);
         }
-        if (mn < (int)k && !dead && !(ABLATE & 14)) { // a symbol longer than the window: redo the round with the general parser
-            if (vc_slow_round<RING>(s.row, s.rot, s.ce, &pos_s, k, trow, ROUND)) {
+        if (mn < (int)k && !dead) { // a symbol longer than the window: redo the round with the general parser
+            if (vc_slow_round(s.row, s.rot, s.ce, &pos_s, k, trow, kVcRound)) {
                 s.pos = pos_s;
                 s.load_window();
             } else {
@@ -1003,20 +830,16 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
         }
         if (dead)
             s.pos = pos_s; // parked: its ring is not topped up any more
-        if (r % (TILE / ROUND) == TILE / ROUND - 1) {
+        // ---- a full tile: kVcTile symbols per lane leave as row segments of 4*kVcTile bytes ----
+        if (r % (kVcTile / kVcRound) == kVcTile / kVcRound - 1) {
             __syncwarp();
-            int32_t *dst = out_warp + (size_t)(r / (TILE / ROUND)) * TILE + (lane % kRowLanes) * 4;
+            int32_t *dst = out_warp + (size_t)(r / (kVcTile / kVcRound)) * kVcTile + (lane % kRowLanes) * 4;
 #pragma unroll
             for (int it = 0; it < 32 / kRowsPerIt; it++) {
                 const int row = kRowsPerIt * it + lane / kRowLanes;
                 if ((row_mask >> row) & 1u) {
                     const int4 q = *reinterpret_cast<const int4 *>(tile + row * kTilePitch + (lane % kRowLanes) * 4);
-                    if (!(ABLATE & 1) || q.x == 0x7fffffff) {
-                        if (ABLATE & 16)
-                            __stcs(reinterpret_cast<int4 *>(dst + (size_t)row * part), q);
-                        else
-                            *reinterpret_cast<int4 *>(dst + (size_t)row * part) = q;
-                    }
+                    *reinterpret_cast<int4 *>(dst + (size_t)row * part) = q;
                 }
             }
             __syncwarp();
@@ -1031,21 +854,12 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
             else
                 bad |= s.pos > total * 32;
         }
-        if (bad && !(ABLATE & 14))
-            p.flags[st] = 1u;
+        if (bad)
+            p.flags[st] = 1u; // (several parts may say so: idempotent)
     }
 }
 
-template <int TILE>
-constexpr size_t vc_smem_bytes()
-{
-    return 64 * 4 + (size_t)kVsWarps * 32 * 64 * 4 + (size_t)kVsWarps * 32 * (TILE + 4) * 4 + kVsWarps * sizeof(VsCoopMeta);
-}
-
-template <int RING, int TILE>
-constexpr size_t vs_smem_bytes()
-{
-    return RING * 4 + (size_t)kVsWarps * 32 * RING * 4 + (size_t)kVsWarps * 32 * (TILE + 4) * 4;
-}
+constexpr size_t kVcSmemBytes = VsCoopStream::kRing * 4 + (size_t)kVsWarps * 32 * VsCoopStream::kRing * 4 +
+                                (size_t)kVsWarps * 32 * (kVcTile + 4) * 4 + kVsWarps * sizeof(VsCoopMeta);
 
 } // namespace selab200
