@@ -486,25 +486,25 @@ int decode_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint
     p.status = d_status;
     p.ws_q = static_cast<int32_t *>(d_ws);
     p.ws_res = reinterpret_cast<int32_t *>(static_cast<char *>(d_ws) + align256(n_sub * 128 * 4));
-    p.order_index = reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(p.ws_res) + align256(n_sub * kFrame * 4));
+    p.seg_index = reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(p.ws_res) + align256(n_sub * kFrame * 4));
     p.rice_flags = nullptr;
-    void *rice_aux = reinterpret_cast<char *>(p.order_index) + align256((n_sub + 16) * 4);
-    const size_t n_slots = (n_sub + 12 + 3) / 4 * 4; // every class segment starts on a warp boundary
-    CUDA_TRY(cudaMemsetAsync(p.order_index, 0xff, n_slots * 4, stream));
-    const unsigned class_ctas = (unsigned)((n_sub + kScanTile - 1) / kScanTile);
-    k_decode_class_counts<<<class_ctas, kScanTile, 0, stream>>>(p, static_cast<ClassCounts *>(rice_aux));
-    if (int rc = launch_check("k_decode_class_counts"))
+    const size_t n_warps = synthesis_warps(n_sub);
+    void *rice_aux = reinterpret_cast<char *>(p.seg_index) + align256(n_warps * 32 * 4);
+    CUDA_TRY(cudaMemsetAsync(p.seg_index, 0xff, n_warps * 32 * 4, stream));
+    const unsigned plan_ctas = (unsigned)((n_sub + kScanTile - 1) / kScanTile);
+    k_decode_width_counts<<<plan_ctas, kScanTile, 0, stream>>>(p, static_cast<WidthCounts *>(rice_aux));
+    if (int rc = launch_check("k_decode_width_counts"))
         return rc;
-    k_decode_classify<<<class_ctas, kScanTile, 0, stream>>>(p, static_cast<const ClassCounts *>(rice_aux));
-    if (int rc = launch_check("k_decode_classify"))
+    k_decode_plan<<<plan_ctas, kScanTile, 0, stream>>>(p, static_cast<const WidthCounts *>(rice_aux));
+    if (int rc = launch_check("k_decode_plan"))
         return rc;
     if (int rc = launch_rice_decode(p, 0, stream))
         return rc;
     if (int rc = launch_rice_residues(p, rice_aux, stream))
         return rc;
     p.fallback_only = 1;
-    k_synthesise_quad<<<(unsigned)(n_slots / 4), 32, 0, stream>>>(p);
-    if (int rc = launch_check("k_synthesise_quad"))
+    k_synthesise_segments<<<(unsigned)n_warps, 32, 0, stream>>>(p);
+    if (int rc = launch_check("k_synthesise_segments"))
         return rc;
     if (channels == 2) { // every stereo frame is handled by the batch kernel + the difference fix-up
         k_diff_fixup<<<n_frames, 128, 0, stream>>>(p);
@@ -717,7 +717,8 @@ size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_sub = (size_t)n_frames * channels;
-    return align256(n_sub * 128 * 4) + align256(n_sub * kFrame * 4) + align256((n_sub + 16) * 4) + align256(n_sub * 64) + 256;
+    return align256(n_sub * 128 * 4) + align256(n_sub * kFrame * 4) + align256(synthesis_warps(n_sub) * 32 * 4) +
+           align256(n_sub * 64) + 256;
 }
 
 int selab200_encode_frames_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
@@ -779,7 +780,7 @@ int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, ui
     p.status = d_status;
     p.ws_q = nullptr;
     p.ws_res = d_residues;
-    p.order_index = nullptr;
+    p.seg_index = nullptr;
     p.fallback_only = 0;
     p.rice_flags = nullptr;
     if (int rc = g.aux.ensure((size_t)n_frames * channels * 64 + 256))

@@ -5,10 +5,10 @@
 //            k_encode_sizes + k_encode_scan (stereo decision, prefix sum, descriptors)
 //            k_encode_gather / k_encode_gather_container (slot -> word arena / .sela byte stream)
 //   decode   k_container_unpack (.sela bytes -> word arena)
-//            k_decode_class_counts + k_decode_classify (subframes grouped by predictor-order class)
+//            k_decode_width_counts + k_decode_plan (subframes packed into synthesis warps by segment width)
 //            k_rice_decode<RING,BATCH> (lane per stream: reflection streams, flagged residue streams)
 //            k_rice_split_index / k_rice_decode_vc (rice_vs.cuh: residue streams, lane per part of a stream)
-//            k_synthesise_quad (+ k_diff_fixup; k_synthesise for frames the batch kernel declines)
+//            k_synthesise_segments (+ k_diff_fixup; k_synthesise for frames the batch kernel declines)
 //   stage-level entry points   k_unit_means + k_lpc_residues, k_lpc_samples, k_rice_encode, k_rice_decode_streams
 #pragma once
 
@@ -664,7 +664,7 @@ struct DecodeParams {
     int32_t *status;
     int32_t *ws_q;   // [n_sub][128]
     int32_t *ws_res; // [n_sub][2048]
-    uint32_t *order_index; // [n_sub + 16]: subframe ids grouped by predictor-order class (k_decode_classify)
+    uint32_t *seg_index; // [synthesis_warps(n_sub)][32]: subframe whose segment starts at that lane (k_decode_plan)
     int fallback_only;
     const uint32_t *rice_flags; // residue pass of k_rice_decode: when set, only streams with a non-zero flag (rice_vs.cuh)
 };
@@ -752,7 +752,7 @@ __global__ void k_synthesise(DecodeParams p)
     const bool valid = meta[2 * ch];
     int16_t *out = p.pcm_out + (size_t)frame * kFrame * ch;
     if (p.fallback_only) {
-        // launched behind k_synthesise_quad: only frames it declines (difference coding with a
+        // launched behind k_synthesise_segments: only frames it declines (difference coding with a
         // channel count other than 2) are left to do
         unsigned type_mask = 0;
         for (uint32_t c = 0; c < ch; c++)
@@ -806,139 +806,193 @@ __global__ void k_synthesise(DecodeParams p)
     }
 }
 
-// Predictor-order classes of the batch synthesis kernel: taps per lane (8 lanes per subframe)
-// 4 / 8 / 16, i.e. orders up to 28 / 56 / 112 (the last lane of a quarter must only hold taps
-// beyond the order).  A warp runs all four of its subframes with the taps of the largest order
-// among them, so subframes are first grouped by class: on the BASELINE synthetic (orders spread
-// evenly over 17..100) that removes about a quarter of the multiplies.
-__device__ __forceinline__ int order_class(int order) { return order <= 28 ? 0 : order <= 56 ? 1 : 2; }
+// Packing plan of the batch synthesis kernel: which subframes share a warp, and on which lanes.  A warp holds
+// segments of widths 1..kMaxWidth lanes (segment_width) summing to at most 32.  Subframes of the same width are
+// interchangeable, so the plan is made from the width counts alone, as a short list of warp TEMPLATES: the widest
+// width left opens a warp, which is then filled greedily, widest first, with whatever still fits; the template is
+// repeated as often as the counts allow.  Templates are laid out widest first, so the warps with the most lanes in
+// use start first.  Every template either takes the last subframes of some width or is followed by one that does
+// (after a template limited by room, the first width it exhausted to below its copies is taken whole by the next),
+// so there are at most 2 * kMaxWidth templates.  Every warp but the last holds at least two segments, so there are
+// at most n_sub / 2 + 1 warps.  On the BASELINE synthetic 93 % of the issued multiply slots are predictor taps.
+//   k_decode_width_counts  CTA b: how many of its subframes have each width -> tmp[b]
+//   k_decode_plan          CTA b: width totals of all CTAs -> templates (every CTA computes them, one thread);
+//                          counts of the CTAs before it + the rank inside the CTA -> the subframe's rank among its
+//                          width -> template, repeat and lane: seg_index[warp][first lane] = subframe.
+// tmp is the head of the Rice decoder's scratch, which is not in use yet.  seg_index is pre-set to kNoSegment.
+constexpr uint32_t kNoSegment = 0xffffffffu;
+constexpr int kMaxTemplates = 2 * kMaxWidth;
 
-// Stable counting sort of the subframes by class into p.order_index; every class segment
-// starts on a warp boundary (4 subframes), widest class first; gaps hold 0xffffffff (pre-set by the host side).
-// Two launches of 1024 subframes per CTA (coalesced descriptor loads in both):
-//   k_decode_class_counts  CTA b: how many of its subframes fall in each class -> tmp[b] (classes 0|1 and 2|3 packed
-//                          as the 32-bit halves of two words)
-//   k_decode_classify      CTA b: totals of all CTAs (-> where each class segment starts; widest class first) + counts
-//                          of the CTAs before it + a block scan -> order_index.  Ascending subframe order inside a
-//                          class is kept (stable), so the two subframes of a stereo frame stay neighbours.
-// tmp is the head of the Rice decoder's scratch, which is not in use yet.
-struct ClassCounts {
-    unsigned long long c01, c23;
+struct WidthCounts {
+    uint32_t n[16]; // by segment width; [0]: no subframe
 };
-__device__ __forceinline__ ClassCounts class_one(int c)
-{
-    ClassCounts v;
-    const unsigned long long one = 1ull << (32 * (c & 1));
-    v.c01 = (c >> 1) ? 0ull : one;
-    v.c23 = (c >> 1) ? one : 0ull;
-    return v;
-}
-__device__ __forceinline__ uint32_t class_get(const ClassCounts &v, int c)
-{
-    return (uint32_t)(((c >> 1) ? v.c23 : v.c01) >> (32 * (c & 1)));
-}
-__device__ __forceinline__ int subframe_class(const DecodeParams &p, uint32_t u)
+struct SegTemplate {
+    uint32_t repeats, first_warp;
+    uint8_t copies[16], lane0[16]; // by width: segments per warp, first lane of the first of them
+};
+
+__device__ __forceinline__ int subframe_width(const DecodeParams &p, uint32_t u)
 {
     const int order = p.descs[u].lpc_order;
-    return order_class(order > kMaxOrder ? 0 : order);
+    return segment_width(order > kMaxOrder ? 0 : order);
 }
 
-__global__ void __launch_bounds__(kScanTile) k_decode_class_counts(DecodeParams p, ClassCounts *tmp)
+// Per-warp width counts of a 1024-thread CTA into cnt[warp][width]; returns the thread's rank among the threads of
+// its warp with the same width.
+__device__ __forceinline__ uint32_t warp_width_counts(int w, uint32_t (*cnt)[16])
 {
-    __shared__ ClassCounts warp_cnt[32];
-    const uint32_t n_units = p.n_frames * p.channels;
-    const uint32_t u = blockIdx.x * kScanTile + threadIdx.x;
-    ClassCounts v = {0ull, 0ull};
-    if (u < n_units)
-        v = class_one(subframe_class(p, u));
-    v.c01 = warp_sum_u64(v.c01);
-    v.c23 = warp_sum_u64(v.c23);
-    if (lane_id() == 0)
-        warp_cnt[warp_id()] = v;
-    __syncthreads();
-    if (warp_id() == 0) {
-        v = warp_cnt[lane_id()];
-        v.c01 = warp_sum_u64(v.c01);
-        v.c23 = warp_sum_u64(v.c23);
-        if (lane_id() == 0)
-            tmp[blockIdx.x] = v;
-    }
-}
-
-__global__ void __launch_bounds__(kScanTile) k_decode_classify(DecodeParams p, const ClassCounts *tmp)
-{
-    __shared__ unsigned long long warp_tot[2][32];
-    __shared__ ClassCounts total, before;
-    const uint32_t n_units = p.n_frames * p.channels;
-    const uint32_t u = blockIdx.x * kScanTile + threadIdx.x;
-    const int lane = lane_id(), warp = warp_id();
-    if (warp == 0) {
-        ClassCounts all = {0ull, 0ull}, pre = {0ull, 0ull};
-        for (uint32_t b = lane; b < gridDim.x; b += 32) {
-            const ClassCounts v = tmp[b];
-            all.c01 += v.c01, all.c23 += v.c23;
-            if (b < blockIdx.x)
-                pre.c01 += v.c01, pre.c23 += v.c23;
-        }
-        all.c01 = warp_sum_u64(all.c01), all.c23 = warp_sum_u64(all.c23);
-        pre.c01 = warp_sum_u64(pre.c01), pre.c23 = warp_sum_u64(pre.c23);
+    const int lane = lane_id();
+    uint32_t rank = 0;
+#pragma unroll
+    for (int v = 0; v < 16; v++) {
+        const unsigned b = __ballot_sync(kFull, w == v);
+        if (w == v)
+            rank = __popc(b & ((1u << lane) - 1u));
         if (lane == 0)
-            total = all, before = pre;
+            cnt[warp_id()][v] = __popc(b);
     }
-    const bool have = u < n_units;
-    const int c = have ? subframe_class(p, u) : 0;
-    ClassCounts mine = {0ull, 0ull};
-    if (have)
-        mine = class_one(c);
-    ClassCounts incl;
-    incl.c01 = block_scan_inclusive_u64(mine.c01, warp_tot[0]); // the barriers in here also publish total / before
-    incl.c23 = block_scan_inclusive_u64(mine.c23, warp_tot[1]);
-    if (!have)
-        return;
-    // widest class first: a synthesis warp runs its four subframes start to finish (hundreds of microseconds), so
-    // the longest-running warps must be scheduled first and the short ones left to fill the tail; every class
-    // segment starts on a multiple of the four subframes a warp takes
-    uint32_t base = 0;
-    for (int k = 3; k > c; k--)
-        base += (class_get(total, k) + 3u) / 4u * 4u;
-    ClassCounts excl;
-    excl.c01 = before.c01 + incl.c01 - mine.c01;
-    excl.c23 = before.c23 + incl.c23 - mine.c23;
-    p.order_index[base + class_get(excl, c)] = u;
+    return rank;
 }
 
-// K6, batch form: one warp = four subframes of one predictor-order class (stereo: two whole
-// frames, the pair of a frame in neighbouring quarters).  Handles every frame except those with
-// difference-coded subframes and a channel count other than 2 (the reference's encoder never
-// produces those; k_synthesise above picks them up).
-struct QuadSmem {
-    IirSmem ii[4];
-    double t[104];
-    CoefSmem cf[4];
-    // staging rows [2][16] of the four quarters at word offsets 0, 48, 104, 152: the four writer lanes (one per
-    // quarter, same row and column) then hit banks 0 / 16 / 8 / 24 apart, and the 8-byte reads of a half-warp
-    // (two quarters) cover 32 distinct banks; a plain [4][2][16] puts all four writers on one bank
-    int32_t stage[184];
-};
-__device__ __forceinline__ int quad_stage_offset(int q) { return 48 * q + 8 * (q >> 1); }
-
-__global__ void __launch_bounds__(32) k_synthesise_quad(DecodeParams p)
+__global__ void __launch_bounds__(kScanTile) k_decode_width_counts(DecodeParams p, WidthCounts *tmp)
 {
-    __shared__ __align__(16) QuadSmem sm;
-    const uint32_t ch = p.channels;
-    const uint32_t n_sub = p.n_frames * ch;
-    const int lane = lane_id(), q = lane >> 3, hl = lane & 7;
-    const uint32_t sub = p.order_index[blockIdx.x * 4 + q]; // grouped by order class; stereo pairs stay adjacent
-    const bool exists = sub < n_sub;
-    const uint32_t frame = exists ? sub / ch : 0, pos = exists ? sub % ch : 0;
+    __shared__ uint32_t cnt[32][16];
+    const uint32_t u = blockIdx.x * kScanTile + threadIdx.x;
+    warp_width_counts(u < p.n_frames * p.channels ? subframe_width(p, u) : 0, cnt);
+    __syncthreads();
+    if (threadIdx.x < 16) {
+        uint32_t s = 0;
+        for (int w = 0; w < 32; w++)
+            s += cnt[w][threadIdx.x];
+        tmp[blockIdx.x].n[threadIdx.x] = s;
+    }
+}
 
-    // ---- per-quarter validation of the whole frame (all eight lanes redundantly) ----
+// The templates for the width counts c[1..kMaxWidth]; returns how many.
+__device__ int segment_templates(uint32_t (&c)[16], SegTemplate *tpl)
+{
+    int nt = 0;
+    uint32_t warp = 0;
+    for (;;) {
+        SegTemplate t;
+        int room = 32;
+        uint32_t rep = 0xffffffffu;
+#pragma unroll
+        for (int v = 15; v >= 1; v--) {
+            const uint32_t k = v > kMaxWidth ? 0u : min(c[v], (uint32_t)(room / v));
+            t.copies[v] = (uint8_t)k;
+            t.lane0[v] = (uint8_t)(32 - room);
+            room -= (int)k * v;
+            if (k)
+                rep = min(rep, c[v] / k);
+        }
+        if (room == 32)
+            return nt;
+#pragma unroll
+        for (int v = 1; v < 16; v++)
+            c[v] -= rep * t.copies[v];
+        t.copies[0] = t.lane0[0] = 0;
+        t.repeats = rep;
+        t.first_warp = warp;
+        warp += rep;
+        tpl[nt++] = t;
+    }
+}
+
+__global__ void __launch_bounds__(kScanTile) k_decode_plan(DecodeParams p, const WidthCounts *tmp)
+{
+    __shared__ uint32_t cnt[32][16];
+    __shared__ uint32_t part_all[kScanTile / 16][16], part_before[kScanTile / 16][16];
+    __shared__ uint32_t total[16], before[16];
+    __shared__ SegTemplate tpl[kMaxTemplates];
+    const uint32_t n_units = p.n_frames * p.channels;
+    const uint32_t u = blockIdx.x * kScanTile + threadIdx.x;
+    const int w = u < n_units ? subframe_width(p, u) : 0;
+    const uint32_t rank = warp_width_counts(w, cnt);
+    {
+        const int v = threadIdx.x & 15, g = threadIdx.x >> 4;
+        uint32_t all = 0, pre = 0;
+        for (uint32_t b = g; b < gridDim.x; b += kScanTile / 16) {
+            const uint32_t x = tmp[b].n[v];
+            all += x;
+            if (b < blockIdx.x)
+                pre += x;
+        }
+        part_all[g][v] = all;
+        part_before[g][v] = pre;
+    }
+    __syncthreads();
+    if (threadIdx.x < 16) {
+        const int v = threadIdx.x;
+        uint32_t all = 0, pre = 0, run = 0;
+        for (int g = 0; g < kScanTile / 16; g++)
+            all += part_all[g][v], pre += part_before[g][v];
+        total[v] = all;
+        before[v] = pre;
+        for (int x = 0; x < 32; x++) { // exclusive prefix over the warps of this CTA
+            const uint32_t c = cnt[x][v];
+            cnt[x][v] = run;
+            run += c;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t c[16];
+#pragma unroll
+        for (int v = 0; v < 16; v++)
+            c[v] = v ? total[v] : 0u;
+        segment_templates(c, tpl);
+    }
+    __syncthreads();
+    if (u >= n_units)
+        return;
+    const uint32_t r = before[w] + cnt[warp_id()][w] + rank; // rank among all subframes of width w
+    uint32_t acc = 0;
+    int t = 0;
+    for (;; t++) {
+        const uint32_t m = tpl[t].repeats * tpl[t].copies[w];
+        if (r < acc + m)
+            break;
+        acc += m;
+    }
+    const uint32_t k = tpl[t].copies[w], j = r - acc, rep = j / k;
+    const uint32_t lane = tpl[t].lane0[w] + (j - rep * k) * (uint32_t)w;
+    p.seg_index[((size_t)tpl[t].first_warp + rep) * 32 + lane] = u;
+}
+
+// Upper bound of the number of synthesis warps (see above).
+__host__ __device__ inline size_t synthesis_warps(size_t n_sub) { return n_sub / 2 + 1; }
+
+// K6, batch form: one warp = the segments k_decode_plan put there.  Handles every frame except those with
+// difference-coded subframes and a channel count other than 2 (the reference's encoder never produces those;
+// k_synthesise above picks them up).  Residues arrive kSegBlock at a time per segment through cp.async (whole
+// 64-byte pieces of every row, two blocks ahead); finished samples are parked in a staging row per segment and
+// leave kSegBlock at a time, a 32-byte or 64-byte run per segment and instruction.
+__global__ void __launch_bounds__(32) k_synthesise_segments(DecodeParams p)
+{
+    __shared__ __align__(16) SegSmem sm;
+    const uint32_t ch = p.channels;
+    const int lane = lane_id();
+    const uint32_t entry = p.seg_index[(size_t)blockIdx.x * 32 + lane];
+    const unsigned starts = __ballot_sync(kFull, entry != kNoSegment);
+    if (!(starts & 1u))
+        return; // beyond the last warp of the plan
+    const int start = 31 - __clz(starts & (0xffffffffu >> (31 - lane))); // the last segment start at or below
+    const uint32_t sub = __shfl_sync(kFull, entry, start);
+    const int seg = __popc(starts & ((1u << start) - 1u)); // segment ordinal
+    const int n_seg = __popc(starts);
+    const int k = lane - start;
+    const uint32_t frame = sub / ch, pos = sub % ch;
+    const selab200_subframe_desc *fd = p.descs + (size_t)frame * ch;
+    const int n = subframe_width(p, sub);
+    const bool exists = k < n; // lanes past the last segment hold zero taps and store nothing
+
+    // ---- validation of the whole frame (every lane of the segment redundantly) ----
     bool frame_ok = exists;
     unsigned seen = 0, type_mask = 0;
     selab200_subframe_desc mine;
     memset(&mine, 0, sizeof mine);
     if (exists) {
-        const selab200_subframe_desc *fd = p.descs + (size_t)frame * ch;
         for (uint32_t i = 0; i < ch; i++) {
             const selab200_subframe_desc d = fd[i];
             const bool ok = desc_ok(d, ch, p.n_words) && !((seen >> d.channel) & 1);
@@ -955,58 +1009,79 @@ __global__ void __launch_bounds__(32) k_synthesise_quad(DecodeParams p)
             if (d.subframe_type == 1 && ((type_mask >> d.parent_channel) & 1))
                 frame_ok = false; // a parent must be an independent subframe
         }
-        if (!frame_ok && hl == 0)
+        if (!frame_ok && k == 0)
             raise_status(p.status, SELAB200_ERR_BITSTREAM);
     }
     const bool general = exists && frame_ok && frame_needs_general(ch, type_mask);
     const bool proc = exists && frame_ok && !general;
+    const bool diff = proc && mine.subframe_type == 1;
     const int order = proc ? mine.lpc_order : 0;
-
-    // ---- predictors of the four subframes (warp-wide routines, one subframe at a time) ----
-    for (int h = 0; h < 4; h++) {
-        const int order_h = __shfl_sync(kFull, order, 8 * h);
-        const uint32_t sub_h = __shfl_sync(kFull, sub, 8 * h);
-        CoefSmem &cf = sm.cf[h];
-        for (int i = lane; i < 104; i += 32)
-            cf.q[i] = i < order_h ? p.ws_q[(size_t)sub_h * 128 + i] : 0;
-        __syncwarp();
-        warp_coefficients(cf, sm.t, order_h); // order 0 behaves like a zero predictor
-        warp_iir_prepare(cf, sm.ii[h], order_h);
+    int16_t *out = p.pcm_out + (size_t)frame * kFrame * ch;
+    int32_t *row = p.ws_res + (size_t)sub * kFrame;
+    if (k == 0) {
+        sm.row_res[seg] = row;
+        // a difference signal goes back into its (already consumed) residue row; k_diff_fixup turns it into
+        // parent - difference once the parent is complete
+        sm.row_out[seg] = diff ? static_cast<void *>(row) : static_cast<void *>(out + mine.channel);
+        sm.row_mode[seg] = !proc ? 0 : diff ? 2 : 1;
     }
+    __syncwarp();
+
+    // residues of block B -> in[B & 1]: eight rows per instruction, four 16-byte pieces per row
+    auto fetch = [&](int B) {
+        for (int i = lane >> 2; i < n_seg; i += 8) {
+            const int32_t *src = sm.row_res[i] + kSegBlock * B + 4 * (lane & 3);
+            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&sm.in[B & 1][i * kSegRow + 4 * (lane & 3)]);
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    fetch(0);
+    fetch(1);
+
+    // ---- predictors: every segment steps its own order up at once ----
+    for (int i = k; i < order; i += n)
+        sm.q[kTapsPerLane * start + i] = p.ws_q[(size_t)sub * 128 + i];
+    __syncwarp();
     int order_max = order;
-    order_max = max(order_max, __shfl_xor_sync(kFull, order_max, 8));
-    order_max = max(order_max, __shfl_xor_sync(kFull, order_max, 16));
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+        order_max = max(order_max, __shfl_xor_sync(kFull, order_max, o));
+    SegState st;
+    segment_coefficients(sm, start, k, n, order, order_max, st.cl, st.ch);
+    segment_state(st, k, n);
+    st.sp = 0;
 
     // ---- recurrence + output ----
-    QuadIo io;
-    io.res = p.ws_res + (size_t)(exists ? sub : 0) * kFrame;
-    io.stage = sm.stage + quad_stage_offset(q);
-    const bool diff = proc && mine.subframe_type == 1;
-    const uint32_t channel = mine.channel;
-    int16_t *out = p.pcm_out + (size_t)frame * kFrame * ch;
-    int32_t *row = p.ws_res + (size_t)(exists ? sub : 0) * kFrame;
-    auto emit = [&](int B, int kx, int ky) {
-        if (!proc)
-            return;
-        const size_t t = 16 * B + 2 * hl;
-        if (diff) {
-            // a difference signal goes back into its (already consumed) residue row;
-            // k_diff_fixup turns it into parent - difference once the parent is complete
-            *reinterpret_cast<int2 *>(row + t) = make_int2(kx, ky);
-        } else {
-            out[t * ch + channel] = (int16_t)(uint16_t)kx;
-            out[(t + 1) * ch + channel] = (int16_t)(uint16_t)ky;
+    const bool top = k == n - 1, first = k == 0 && exists;
+    int32_t *out_row = sm.out + seg * kSegRow;
+    for (int B = 0; B < kFrame / kSegBlock; B++) {
+        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        __syncwarp();
+        const int32_t *in_row = sm.in[B & 1] + seg * kSegRow;
+        if (B == 0)
+            segment_block<true>(st, in_row, out_row, start, top, first);
+        else
+            segment_block<false>(st, in_row, out_row, start, top, first);
+        __syncwarp();
+        for (int i = lane >> 4; i < n_seg; i += 2) {
+            const int mode = sm.row_mode[i];
+            const int e = lane & 15, t = kSegBlock * B + e;
+            const int v = sm.out[i * kSegRow + e];
+            if (mode == 1)
+                static_cast<int16_t *>(sm.row_out[i])[(size_t)t * ch] = (int16_t)(uint16_t)v;
+            else if (mode == 2)
+                static_cast<int32_t *>(sm.row_out[i])[t] = v;
         }
-    };
-    switch (order_class(order_max)) {
-    case 0: warp_iir_quad<4>(sm.cf[q], sm.ii[q], order, order_max, io, proc, emit); break;
-    case 1: warp_iir_quad<8>(sm.cf[q], sm.ii[q], order, order_max, io, proc, emit); break;
-    default: warp_iir_quad<16>(sm.cf[q], sm.ii[q], order, order_max, io, proc, emit); break;
+        if (B + 2 < kFrame / kSegBlock)
+            fetch(B + 2);
+        else
+            asm volatile("cp.async.commit_group;" ::: "memory");
     }
 
     if (exists && !frame_ok) { // malformed frame: silence
-        for (int t = hl; t < kFrame; t += 8)
-            out[(size_t)t * ch + (pos < ch ? pos : 0)] = 0;
+        for (int t = k; t < kFrame; t += n)
+            out[(size_t)t * ch + pos] = 0;
     }
 }
 

@@ -645,97 +645,142 @@ __device__ void warp_iir_synthesis_pair(const CoefSmem &cf, const IirSmem &ii, i
 }
 
 // ---------------------------------------------------------------------------
-// K6, batch form: FOUR subframes per warp (quarter q = lane>>3 owns one), eight lanes x
-// TPL taps each (TPL*7 >= order, so a quarter's last lane only ever holds zero
-// coefficients and shfl_down past the quarter's edge returns its own, zero, value).
-// No shared-memory sample planes: residues arrive from global memory 16 at a time per
-// quarter (one coalesced 64-byte load, one block ahead) and are handed to lane 0 of the
-// quarter by shuffle; finished samples are parked in a 64-byte staging row per quarter
-// and leave 16 at a time.  Per 16 outputs a quarter therefore touches shared memory
-// 16 + 1 times and global memory twice.
-struct QuadIo {
-    const int32_t *res;   // this quarter's residues (global), 2048 ints, 16-byte aligned
-    int32_t *stage;       // this quarter's staging rows in shared memory: [2][16]
-};
+// K6, batch form: a warp runs as many subframes as fit, each on a SEGMENT of consecutive lanes.  A subframe of
+// order o owns n = max(1, ceil(o / kTapsPerLane)) lanes; lane k of the segment owns taps kTapsPerLane*k + 1 ..
+// kTapsPerLane*(k+1) (zero beyond o).  Every segment runs the transposed recurrence of warp_iir_pair at once:
+// the segment's top lane takes 0 where the others take the accumulator of the lane above, and the finished
+// sample reaches the segment from its first lane.  Taps per lane are fixed, so the multiplies a warp issues
+// follow the orders it holds instead of the largest order of a class.
+constexpr int kTapsPerLane = 8;
+constexpr int kMaxWidth = (kMaxOrder + kTapsPerLane - 1) / kTapsPerLane; // 13 lanes for order 100
+constexpr int kSegBlock = 16; // samples per staging block
+constexpr int kSegRow = 20;   // words per staging row: the rows of eight segments sit on eight distinct 4-bank groups
+static_assert(kSegBlock % kTapsPerLane == 0, "the register of slot 0 must be static inside a block");
 
-template <int TPL>
-struct QuadState {
-    uint32_t cl[TPL];
-    int32_t ch[TPL];
-    unsigned long long alo[TPL];
-    uint32_t ahi[TPL];
-    uint32_t sp;
-};
-
-// One block of 16 outputs t = 16*B + e.  WARM: bias term from the prefix table (t <= order).
-template <int TPL, bool WARM>
-__device__ __forceinline__ void quad_block(QuadState<TPL> &st, const IirSmem &ii, int order, unsigned long long steady,
-                                           int B, int2 rcur, int32_t *stage_row, bool writer)
+__device__ __forceinline__ int segment_width(int order)
 {
-#pragma unroll
-    for (int e = 0; e < 16; e++) {
-        const int t = 16 * B + e;
-        const int rt = __shfl_sync(kFull, (e & 1) ? rcur.y : rcur.x, e >> 1, 8);
-        int vnext;
-        if (WARM && e == 0 && B == 0) { // uniform branch, only compiled into the warm-up variant
-            vnext = rt; // s[0] = r[0]
-        } else {
-            const int u = (e + 16 * TPL - 1) % TPL; // == (t - 1) % TPL, static
-#pragma unroll
-            for (int m = 0; m < TPL; m++) {
-                st.alo[(m + u) % TPL] = mad_wide_u32(st.cl[m], st.sp, st.alo[(m + u) % TPL]);
-                st.ahi[(m + u) % TPL] += (uint32_t)st.ch[m] * st.sp;
-            }
-            const unsigned long long full0 = st.alo[u] + ((unsigned long long)st.ahi[u] << 32);
-            const unsigned long long incoming = __shfl_down_sync(kFull, full0, 1, 8);
-            const unsigned long long base = WARM ? ii.pre[t < order ? t : order] : steady;
-            const unsigned long long tt = base - full0;
-            vnext = rt - (int32_t)((long long)tt >> kQ);
-            vnext = __shfl_sync(kFull, vnext, 0, 8);
-            st.alo[u] = incoming;
-            st.ahi[u] = 0;
-        }
-        if (writer)
-            stage_row[e] = vnext;
-        st.sp = synth_biased(vnext);
-    }
+    return order <= kTapsPerLane ? 1 : (order + kTapsPerLane - 1) / kTapsPerLane;
 }
 
-// Runs the recurrence for the quarter's subframe; after every block calls
-// emit(B, kx, ky) with this lane's two finished samples s[16B + 2*hl], s[16B + 2*hl + 1].
-template <int TPL, typename Emit>
-__device__ void warp_iir_quad(const CoefSmem &cf, const IirSmem &ii, int order, int order_max, const QuadIo io, bool has_res, Emit emit)
+struct SegSmem {
+    int32_t q[32 * kTapsPerLane]; // the segment at lanes S.. : q[kTapsPerLane*S + i]
+    union {
+        double t[32 * kTapsPerLane];  // step-up rows, indexed like q (a segment of n lanes has room for 8n >= order)
+        int32_t out[32 * kSegRow];    // finished samples of the current block, row = segment ordinal
+    };
+    int32_t in[2][32 * kSegRow];      // residues of the next two blocks, row = segment ordinal
+    const int32_t *row_res[32];       // per segment ordinal: its residue row
+    void *row_out[32];                //   where its samples go (int16 PCM of its channel, or its residue row)
+    int row_mode[32];                 //   0: nothing, 1: PCM, 2: residue row (difference subframe)
+};
+
+// warp_coefficients for every segment at once: each segment steps its own order up with its own n lanes
+// (k = lane - start), the loop runs to the largest order in the warp.  Same operations in the same order per
+// element as warp_coefficients.  Returns this lane's taps kTapsPerLane*k + 1 .. as Q35 words.
+__device__ __forceinline__ void segment_coefficients(SegSmem &sm, int start, int k, int n, int order, int order_max,
+                                                     uint32_t (&cl)[kTapsPerLane], int32_t (&ch)[kTapsPerLane])
 {
-    const int hl = lane_id() & 7;
-    QuadState<TPL> st;
+    double *t = sm.t + kTapsPerLane * start;
+    const int32_t *q = sm.q + kTapsPerLane * start;
+    const bool live = order > 1 && k < n; // order <= 1: a single zero reflection coefficient -> c[1] = 0
+    for (int i = 0; i < order_max; i++) {
+        if (live && i < order) {
+            const double ki = dequantise(i, q[i]);
+            const int half = i >> 1;
+            for (int j = k; j < half; j += n) {
+                double a = t[j];
+                double b = t[i - 1 - j];
+                t[j] = dadd(a, dmul(ki, b));
+                t[i - 1 - j] = dadd(b, dmul(ki, a));
+            }
+            if (k == 0) {
+                if (i & 1) {
+                    double mid = t[half];
+                    t[half] = dadd(mid, dmul(mid, ki));
+                }
+                t[i] = ki;
+            }
+        }
+        __syncwarp();
+    }
+    const double scale = 34359738368.0; // 2^35
 #pragma unroll
-    for (int m = 0; m < TPL; m++) {
-        const int j = TPL * hl + m; // tap j+1
-        st.cl[m] = j < 112 ? cf.clo[j] : 0u;
-        st.ch[m] = j < 112 ? cf.chi[j] : 0;
-        st.alo[m] = 0;
+    for (int m = 0; m < kTapsPerLane; m++) {
+        const int j = kTapsPerLane * k + m; // tap j + 1
+        const long long v = (live && j < order) ? __double2ll_rz(dmul(scale, -t[j])) : 0;
+        cl[m] = (uint32_t)v;
+        ch[m] = (int32_t)(v >> 32);
+    }
+    __syncwarp(); // t is dead: its bytes become the output rows
+}
+
+struct SegState {
+    uint32_t cl[kTapsPerLane];
+    int32_t ch[kTapsPerLane];
+    unsigned long long alo[kTapsPerLane];
+    uint32_t ahi[kTapsPerLane];
+    uint32_t sp;
+    unsigned long long steady; // 2^34 + 2^31 * sum_j c[j]: the rounding constant and the sample bias, at the first lane
+};
+
+// Accumulators before the first product: slot m of lane k is output j = kTapsPerLane*k + m + 1, and it starts with
+// what the samples before the subframe contribute in biased form, 2^31 * sum_{j < j' <= order} c[j'] (s[<0] = 0 is
+// s' = 2^31).  Every output then carries the bias of every tap, and one constant removes it from each of them --
+// the same sum mod 2^64 as the warm-up table of warp_iir_pair.
+__device__ __forceinline__ void segment_state(SegState &st, int k, int n)
+{
+    unsigned long long tot = 0, loc[kTapsPerLane];
+#pragma unroll
+    for (int m = kTapsPerLane - 1; m >= 0; m--) {
+        loc[m] = tot; // taps above m in this lane
+        tot += (unsigned long long)(((unsigned long long)(uint32_t)st.ch[m] << 32) | st.cl[m]);
+    }
+    unsigned long long incl = tot; // sum over lanes k.. of the segment
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long x = __shfl_down_sync(kFull, incl, o);
+        if (k + o < n)
+            incl += x;
+    }
+    const unsigned long long above = incl - tot;
+#pragma unroll
+    for (int m = 0; m < kTapsPerLane; m++) {
+        st.alo[m] = (above + loc[m]) << 31;
         st.ahi[m] = 0;
     }
-    st.sp = 0;
-    const unsigned long long steady = ii.pre[order];
-    const bool writer = hl == 0;
-    const int2 *r2 = reinterpret_cast<const int2 *>(io.res);
-    // plain loads: a difference subframe writes its result back into this row behind the reads
-    int2 rcur = has_res ? r2[hl] : make_int2(0, 0);
-    int2 rnext = has_res ? r2[8 + hl] : make_int2(0, 0);
-    const int warm_blocks = order_max / 16 + 1; // blocks that contain some t <= order
-    for (int B = 0; B < kFrame / 16; B++) {
-        int32_t *row = io.stage + (B & 1) * 16;
-        if (B < warm_blocks)
-            quad_block<TPL, true>(st, ii, order, steady, B, rcur, row, writer);
-        else
-            quad_block<TPL, false>(st, ii, order, steady, B, rcur, row, writer);
-        rcur = rnext;
-        if (B + 2 < kFrame / 16 && has_res)
-            rnext = r2[(B + 2) * 8 + hl];
-        __syncwarp();
-        const int2 kept = *reinterpret_cast<const int2 *>(row + 2 * hl);
-        emit(B, kept.x, kept.y);
+    st.steady = (1ull << (kQ - 1)) + (incl << 31);
+}
+
+// One block of kSegBlock outputs.  in_row / out_row: this segment's staging rows; src: its first lane.
+// FIRST: block 0, whose output 0 is s[0] = r[0].
+template <bool FIRST>
+__device__ __forceinline__ void segment_block(SegState &st, const int32_t *in_row, int32_t *out_row, int src, bool top,
+                                              bool first)
+{
+#pragma unroll
+    for (int e = 0; e < kSegBlock; e++) {
+        const int r = in_row[e];
+        int v;
+        if (FIRST && e == 0) {
+            v = r;
+        } else {
+            const int u = (e + kTapsPerLane - 1) % kTapsPerLane; // == (t - 1) % kTapsPerLane, static
+#pragma unroll
+            for (int m = 0; m < kTapsPerLane; m++) {
+                st.alo[(m + u) % kTapsPerLane] = mad_wide_u32(st.cl[m], st.sp, st.alo[(m + u) % kTapsPerLane]);
+                st.ahi[(m + u) % kTapsPerLane] += (uint32_t)st.ch[m] * st.sp;
+            }
+            const unsigned long long full0 = st.alo[u] + ((unsigned long long)st.ahi[u] << 32);
+            const unsigned long long incoming = __shfl_down_sync(kFull, full0, 1);
+            const unsigned long long tt = st.steady - full0;
+            v = r - (int32_t)((long long)tt >> kQ);
+            v = __shfl_sync(kFull, v, src);
+            st.alo[u] = top ? 0ull : incoming;
+            st.ahi[u] = 0;
+        }
+        if (first)
+            out_row[e] = v;
+        st.sp = synth_biased(v);
     }
 }
 
