@@ -77,7 +77,7 @@ typedef struct selab200_subframe_desc {
 int  selab200_init(int device);
 /* Several devices of one box (SURVEY.md 8b: selagpu_init(device_count, device_ids)): every device gets a
  * context of its own (streams, events, pools).  The host-buffer batch calls (selab200_encode_frames,
- * selab200_decode_frames, selab200_encode_container, selab200_container_decode) then cut the frames into one contiguous block per device
+ * selab200_decode_frames, selab200_encode_container, selab200_container_decode and their verify forms) then cut the frames into one contiguous block per device
  * -- n/D frames each, the last device takes the rest, the way sela::Encoder::processFrames cuts them for its
  * threads (src/sela/encoder.cpp:58-73) -- and run the blocks concurrently, reading and writing disjoint ranges
  * of the caller's buffers; results are byte-identical to a single device's.  devices[0] is the primary: it
@@ -218,6 +218,57 @@ int  selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_
                              selab200_container_info *info);
 int  selab200_container_decode(selab200_container *handle, int16_t *pcm_out);
 void selab200_container_close(selab200_container *handle);
+
+/* ------------------------------------------------------------- verify -- */
+
+/* The format is not lossless for every input: encoder and decoder round the Q35 prediction differently
+ * when it lands exactly on a half (DESIGN.md 7), and from that sample on the decoded channel drifts away
+ * from its source.  Verifying coded frames against PCM means decoding them exactly as
+ * selab200_decode_frames does (which equals the reference decoder) and comparing with the PCM sample for
+ * sample.  The report holds one entry per decoded output (frame, channel) that differs, in (frame,
+ * channel) order; a wrong parent makes its difference-coded sibling wrong as well, and both appear. */
+typedef struct selab200_verify_entry {   /* 16 bytes */
+    uint32_t frame;          /* frame index in the batch / file                               */
+    uint16_t channel;
+    uint16_t first_sample;   /* 0..2047, within the frame                                      */
+    uint32_t n_differing;    /* 1..2048 (0 only in the device-resident per-pair array)         */
+    int32_t  first_delta;    /* decoded - source at first_sample                               */
+} selab200_verify_entry;
+
+/* Device-resident core: decode (d_descs, d_words) as selab200_decode_frames_device does and compare with
+ * d_pcm_ref.  d_entries: n_frames*channels records, one per (frame, channel) in frame order, channel order;
+ * a differing pair's record is filled in, every other one is zeroed (n_differing == 0).  *d_n_differing
+ * (uint64, device) receives the number of differing pairs.  Stream-ordered, no synchronisation; d_status
+ * as for decode (the records are all zero after a decode error).  Alignment rules as for the other *_device
+ * forms; d_pcm_ref must also be 16-byte aligned (it is read as 16-byte vectors). */
+size_t selab200_verify_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_verify_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
+                                  const uint32_t *d_words, size_t n_words, const int16_t *d_pcm_ref,
+                                  selab200_verify_entry *d_entries, uint64_t *d_n_differing, int32_t *d_status,
+                                  void *d_workspace, size_t workspace_bytes, void *stream);
+
+/* Host-buffer forms.  A report with differences is SELAB200_OK; malformed streams fail as decode does
+ * (SELAB200_ERR_BITSTREAM).  *n_entries always receives the number of differing pairs, of which the first
+ * `capacity` are written to entries.  With several devices the frames are split as for the other batch
+ * calls; frame indices in the report are those of the whole batch. */
+
+/* selab200_decode_frames + compare with pcm (n_frames*2048*channels interleaved samples), pipelined. */
+int selab200_verify_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
+                           const uint32_t *words, size_t n_words, const int16_t *pcm,
+                           selab200_verify_entry *entries, size_t capacity, size_t *n_entries);
+
+/* selab200_encode_container, and a check that the bytes it returns decode back to pcm (`flac --verify`).
+ * The container bytes are identical to selab200_encode_container's.  Each chunk's byte image is unpacked
+ * on the device, decoded and compared with the PCM the chunk already holds in device memory, on the
+ * chunk's compute lane while the next chunk encodes: neither PCM nor bytes cross PCIe a second time. */
+int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                       uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                       size_t capacity, size_t *bytes_used, selab200_verify_entry *entries,
+                                       size_t entries_capacity, size_t *n_entries);
+
+/* Instead of selab200_container_decode on an open container: compare its info.n_frames frames with pcm. */
+int selab200_container_verify(selab200_container *handle, const int16_t *pcm, selab200_verify_entry *entries,
+                              size_t capacity, size_t *n_entries);
 
 /* ------------------------------------------ stage level (host buffers) -- */
 

@@ -4,6 +4,6 @@ CUDA kernels (sm_90a) behind the C ABI of include/sela_b200.h; this package hold
 the kernels (csrc/), the C++ mirror of the reference interface (host/) and a thin
 Python mirror used by the tests and bench.py.  No CPU fallback.
 """
-from .codec import (DESC_DTYPE, FRAME, SelaB200Error, container_info, decode_container,  # noqa: F401
-                    decode_frames, encode_container, encode_frames, init, lpc_residues, lpc_samples,
-                    rice_decode, rice_encode)
+from .codec import (DESC_DTYPE, FRAME, VERIFY_DTYPE, SelaB200Error, container_info, decode_container,  # noqa: F401
+                    decode_frames, encode_container, encode_container_verified, encode_frames, init,
+                    lpc_residues, lpc_samples, rice_decode, rice_encode, verify_container, verify_frames)

@@ -39,6 +39,12 @@ TRACE_DTYPE = np.dtype([
 ], align=True)
 assert TRACE_DTYPE.itemsize == 2832
 
+# mirrors selab200_verify_entry, 16 bytes
+VERIFY_DTYPE = np.dtype([
+    ("frame", "<u4"), ("channel", "<u2"), ("first_sample", "<u2"), ("n_differing", "<u4"), ("first_delta", "<i4"),
+], align=True)
+assert VERIFY_DTYPE.itemsize == 16
+
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
 
@@ -79,6 +85,11 @@ _SIGNATURES = {
     "selab200_container_open": (_I, [_V, _SZ, _V, _V]),
     "selab200_container_decode": (_I, [_V, _V]),
     "selab200_container_close": (None, [_V]),
+    "selab200_verify_workspace_bytes": (_SZ, [_U32, _U32]),
+    "selab200_verify_frames_device": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _V, _V, _V, _SZ, _V]),
+    "selab200_verify_frames": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _SZ, _V]),
+    "selab200_encode_container_verified": (_I, [_V, _U32, _U32, _U32, C.c_uint16, _V, _SZ, _V, _V, _SZ, _V]),
+    "selab200_container_verify": (_I, [_V, _V, _V, _SZ, _V]),
     "selab200_lpc_residues": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_lpc_samples": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_rice_encode": (_I, [_V, _V, _U32, _U32, _V, _V, _V, _U32]),

@@ -11,6 +11,10 @@ error behaviour as in include/sela_b200.h):
                                     sela::Encoder::process + file::SelaFile::writeToFile, and
                                     file::SelaFile::readFromFile + sela::Decoder::processFrames,
                                     on the byte-packed .sela stream
+    verify_frames / encode_container_verified / verify_container
+                                    not in the reference: decode coded frames and compare them with
+                                    their source PCM, reporting every (frame, channel) that differs
+                                    (the format is not lossless for every input, DESIGN.md 7)
     encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
     / fir_probe                     order threshold and quantiser on chosen values, and its FIR residual
                                     on chosen signals and predictors
@@ -24,7 +28,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import DESC_DTYPE, FRAME, INFO_DTYPE, MAX_ORDER, TRACE_DTYPE, SelaB200Error, check, init, lib  # noqa: F401
+from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, MAX_ORDER, TRACE_DTYPE, VERIFY_DTYPE, SelaB200Error,  # noqa: F401
+                   check, init, lib)
 
 
 def _c(a, dtype):
@@ -219,3 +224,70 @@ def decode_container(container, device=0):
     finally:
         L.selab200_container_close(handle)
     return {k: int(info[0][k]) for k in INFO_DTYPE.names if k != "reserved"}, pcm
+
+
+def _whole_frames(pcm, channels):
+    pcm = _c(pcm, np.int16).reshape(-1)
+    n_frames = pcm.size // (FRAME * channels)
+    if n_frames * FRAME * channels != pcm.size:
+        raise ValueError("pcm must hold whole 2048-sample frames")
+    return pcm, n_frames
+
+
+def verify_frames(descs, words, channels, pcm, device=0):
+    """Decode (descs, words) as decode_frames does and compare with pcm (int16, interleaved, the same frames)
+    -> VERIFY_DTYPE array: one entry per (frame, channel) whose decoded samples differ, in that order."""
+    init(device)
+    descs = _c(descs, DESC_DTYPE)
+    words = _c(words, np.uint32)
+    n_frames = descs.size // channels
+    if n_frames * channels != descs.size:
+        raise ValueError("descs must hold `channels` subframes per frame")
+    pcm, n_pcm = _whole_frames(pcm, channels)
+    if n_pcm != n_frames:
+        raise ValueError("pcm holds %d frames, descs %d" % (n_pcm, n_frames))
+    report = np.zeros(max(descs.size, 1), VERIFY_DTYPE)
+    n = C.c_size_t(0)
+    check(lib().selab200_verify_frames(descs.ctypes.data, n_frames, channels, words.ctypes.data, words.size,
+                                       pcm.ctypes.data, report.ctypes.data, report.size, C.addressof(n)))
+    return report[:n.value].copy()
+
+
+def encode_container_verified(pcm, channels, sample_rate, bits_per_sample=16, capacity=None, device=0):
+    """encode_container, plus a check that the returned bytes decode back to pcm -> (bytes, report), the
+    report as verify_frames returns it.  The bytes are those encode_container returns."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used = C.c_size_t(0)
+    report = np.zeros(max(n_frames * channels, 1), VERIFY_DTYPE)
+    n = C.c_size_t(0)
+    check(L.selab200_encode_container_verified(pcm.ctypes.data, n_frames, channels, sample_rate, bits_per_sample,
+                                               out.ctypes.data, cap, C.addressof(used), report.ctypes.data,
+                                               report.size, C.addressof(n)))
+    return out[:used.value], report[:n.value].copy()
+
+
+def verify_container(container, pcm, device=0):
+    """.sela byte stream and the PCM it should decode to (int16 interleaved, info['n_frames'] frames)
+    -> (info dict, report as verify_frames returns it)."""
+    init(device)
+    buf = _c(np.frombuffer(container, np.uint8) if isinstance(container, (bytes, bytearray)) else container, np.uint8)
+    L = lib()
+    info = np.zeros(1, INFO_DTYPE)
+    handle = C.c_void_p(0)
+    check(L.selab200_container_open(buf.ctypes.data, buf.size, C.addressof(handle), info.ctypes.data))
+    try:
+        n_frames, channels = int(info[0]["n_frames"]), int(info[0]["channels"])
+        pcm = _c(pcm, np.int16).reshape(-1)
+        if pcm.size != n_frames * channels * FRAME:
+            raise ValueError("pcm holds %d samples, the container %d frames of %d channels"
+                             % (pcm.size, n_frames, channels))
+        report = np.zeros(max(n_frames * channels, 1), VERIFY_DTYPE)
+        n = C.c_size_t(0)
+        check(L.selab200_container_verify(handle, pcm.ctypes.data, report.ctypes.data, report.size, C.addressof(n)))
+    finally:
+        L.selab200_container_close(handle)
+    return {k: int(info[0][k]) for k in INFO_DTYPE.names if k != "reserved"}, report[:n.value].copy()

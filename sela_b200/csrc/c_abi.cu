@@ -13,7 +13,7 @@
 #include <thread>
 #include <vector>
 
-#include "kernels.cuh"
+#include "verify.cuh"
 
 using namespace selab200;
 
@@ -79,7 +79,8 @@ struct Context {
     cudaEvent_t ev_h2d[kMaxChunks], ev_done[kMaxChunks], ev_scan[kMaxChunks], ev_reset;
     bool events = false;
     DeviceBuffer in, descs, words, work, lane_work[kLanes], aux, small;
-    int32_t *h_small = nullptr;                    // pinned: [0] status, [2..3] words_used
+    DeviceBuffer verify;                           // verify paths: count, status, per-pair records (VerifyArea)
+    int32_t *h_small = nullptr;                    // pinned: [0] status, [2..3] words_used, [12..14] verify count + status
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
     cudaStream_t last_rice_stream = nullptr;
@@ -526,6 +527,104 @@ int read_status(cudaStream_t stream, const int32_t *d_status)
     return 0;
 }
 
+// Decode as decode_device does into the PCM scratch behind the decode workspace, then compare with d_ref.
+// `fresh`: reset status, count and the per-pair records first (a stand-alone batch); the pipelined host
+// paths reset once and point every chunk at its slice of the records.  Frames in the records are numbered
+// from frame_base.
+int verify_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels, const uint32_t *d_words,
+                  size_t n_words, const int16_t *d_ref, selab200_verify_entry *d_entries, unsigned long long *d_count,
+                  int32_t *d_status, void *d_ws, size_t ws_bytes, cudaStream_t stream, bool fresh = true,
+                  uint32_t frame_base = 0)
+{
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (ws_bytes < selab200_verify_workspace_bytes(n_frames, channels))
+        return fail(SELAB200_ERR_ARGUMENT, "verify workspace too small");
+    if ((reinterpret_cast<uintptr_t>(d_ref) & 15) != 0)
+        return fail(SELAB200_ERR_ARGUMENT, "source PCM must be 16-byte aligned on the device");
+    const size_t n_sub = (size_t)n_frames * channels;
+    if (fresh) {
+        CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), stream));
+        CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), stream));
+        if (n_sub)
+            CUDA_TRY(cudaMemsetAsync(d_entries, 0, n_sub * sizeof(selab200_verify_entry), stream));
+    }
+    if (n_frames == 0)
+        return 0;
+    const size_t dec_bytes = align256(selab200_decode_workspace_bytes(n_frames, channels));
+    int16_t *d_decoded = reinterpret_cast<int16_t *>(static_cast<char *>(d_ws) + dec_bytes);
+    if (int rc = decode_device(d_descs, n_frames, channels, d_words, n_words, d_decoded, d_status, d_ws, dec_bytes,
+                               stream, false))
+        return rc;
+    k_verify_compare<<<n_frames, kVerifyThreads, 0, stream>>>(d_decoded, d_ref, channels, frame_base, d_status,
+                                                              d_entries, d_count);
+    return launch_check("k_verify_compare");
+}
+
+// What the host-buffer verify paths keep on the device (g.verify): the count of differing pairs and a
+// status word, the per-pair records of the whole batch, and -- for encode_container_verified only -- the
+// guarded descriptors and the word arena the container image is unpacked into (file-order offsets, as
+// the encoder assigned them, so every chunk lands in its own range).
+struct VerifyArea {
+    unsigned long long *count = nullptr;
+    int32_t *status = nullptr;
+    selab200_verify_entry *entries = nullptr;
+    selab200_subframe_desc *descs = nullptr;
+    uint32_t *arena = nullptr;
+};
+
+// Sizes g.verify for n_sub pairs (and arena_words unpacked words, if any) and resets count, status and records
+// on `stream`.
+int verify_area(size_t n_sub, size_t arena_words, cudaStream_t stream, VerifyArea &v)
+{
+    const size_t e_bytes = align256(n_sub * sizeof(selab200_verify_entry));
+    const size_t d_bytes = arena_words ? align256(n_sub * sizeof(selab200_subframe_desc)) : 0;
+    if (int rc = g.verify.ensure(256 + e_bytes + d_bytes + (arena_words ? arena_words * 4 + 64 : 0)))
+        return rc;
+    char *b = static_cast<char *>(g.verify.ptr);
+    v.count = reinterpret_cast<unsigned long long *>(b);
+    v.status = reinterpret_cast<int32_t *>(b + 8);
+    v.entries = reinterpret_cast<selab200_verify_entry *>(b + 256);
+    v.descs = arena_words ? reinterpret_cast<selab200_subframe_desc *>(b + 256 + e_bytes) : nullptr;
+    v.arena = arena_words ? reinterpret_cast<uint32_t *>(b + 256 + e_bytes + d_bytes) : nullptr;
+    CUDA_TRY(cudaMemsetAsync(b, 0, 256 + n_sub * sizeof(selab200_verify_entry), stream));
+    return 0;
+}
+
+// Once every chunk has been compared (the caller has synchronised the lanes): the decode status, and the
+// differing pairs in order.  The per-pair records come down only when the count is not zero.
+int collect_report(const VerifyArea &v, size_t n_sub, cudaStream_t stream, std::vector<selab200_verify_entry> &out)
+{
+    out.clear();
+    CUDA_TRY(cudaMemcpyAsync(g.h_small + 12, v.count, 16, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    unsigned long long n;
+    memcpy(&n, g.h_small + 12, 8);
+    const int32_t st = g.h_small[14];
+    if (st != 0)
+        return fail(st, "%s", status_text(st));
+    if (n == 0)
+        return 0;
+    std::vector<selab200_verify_entry> all(n_sub);
+    CUDA_TRY(cudaMemcpyAsync(all.data(), v.entries, n_sub * sizeof(selab200_verify_entry), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    out.reserve((size_t)n);
+    for (const selab200_verify_entry &e : all)
+        if (e.n_differing)
+            out.push_back(e);
+    return 0;
+}
+
+// The report of a host-buffer call: *n_entries = all of it, at most `capacity` entries written.
+int deliver_report(const std::vector<selab200_verify_entry> &report, selab200_verify_entry *entries, size_t capacity,
+                   size_t *n_entries)
+{
+    *n_entries = report.size();
+    if (capacity && !report.empty())
+        memcpy(entries, report.data(), std::min(capacity, report.size()) * sizeof(selab200_verify_entry));
+    return 0;
+}
+
 } // namespace
 
 extern "C" {
@@ -584,6 +683,7 @@ static void shutdown_slot()
     for (int i = 0; i < kLanes; i++)
         g.lane_work[i].release();
     g.aux.release();
+    g.verify.release();
     g.small.release();
     if (g.h_small)
         cudaFreeHost(g.h_small);
@@ -721,6 +821,12 @@ size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
            align256(n_sub * 64) + 256;
 }
 
+size_t selab200_verify_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    // the decode workspace, then the decoded PCM
+    return align256(selab200_decode_workspace_bytes(n_frames, channels)) + align256((size_t)n_frames * channels * kFrame * 2);
+}
+
 int selab200_encode_frames_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
                                   selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
                                   uint64_t *d_words_used, int32_t *d_status, void *d_workspace,
@@ -746,6 +852,21 @@ int selab200_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
     return decode_device(d_descs, n_frames, channels, d_words, n_words, d_pcm_out, d_status, d_workspace,
                          workspace_bytes, (cudaStream_t)stream);
+}
+
+int selab200_verify_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
+                                  const uint32_t *d_words, size_t n_words, const int16_t *d_pcm_ref,
+                                  selab200_verify_entry *d_entries, uint64_t *d_n_differing, int32_t *d_status,
+                                  void *d_workspace, size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_descs ? require_ready_for(d_descs) : require_ready())
+        return rc;
+    if (!d_descs || !d_words || !d_pcm_ref || !d_entries || !d_n_differing || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    return verify_device(d_descs, n_frames, channels, d_words, n_words, d_pcm_ref, d_entries,
+                         reinterpret_cast<unsigned long long *>(d_n_differing), d_status, d_workspace, workspace_bytes,
+                         (cudaStream_t)stream);
 }
 
 // Host-buffer batch calls.  Pipelined in chunks of frames over three engines:
@@ -832,11 +953,16 @@ static unsigned long long container_frame_byte(unsigned long long f, uint32_t ch
 // `defer`: leave the word arena / container body on the device (g.words) instead of copying it out chunk by
 // chunk -- the multi-device driver places every device's block once the sizes of the blocks before it are known.
 // With `defer`, `container` is only a flag (any non-null value selects the byte-packed form).
+// `report` (container form only): also verify the container image, chunk by chunk on the device, and return
+// the differing (frame, channel) pairs, frames numbered from frame_base.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
                        uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
-                       bool defer = false)
+                       bool defer = false, std::vector<selab200_verify_entry> *report = nullptr,
+                       uint32_t frame_base = 0)
 {
     *words_used = 0;
+    if (report)
+        report->clear();
     if (n_frames == 0)
         return 0;
     PipelineDrain drain;
@@ -844,6 +970,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const uint32_t n_chunks = plan.chunks();
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
+    const bool verify = report && container;
     const size_t ws_bytes = selab200_encode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
@@ -851,11 +978,21 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     constexpr int kEncLanes = 2;
     for (int i = 0; i < kEncLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
+    // verify: chunk c is checked on lane kEncLanes + c % kVerifyLanes once its gather is done, so that the check
+    // (a decode: latency-bound Rice kernels) overlaps the encode of the chunks after it instead of queueing in front
+    constexpr int kVerifyLanes = kLanes - kEncLanes;
+    for (int i = 0; verify && i < kVerifyLanes && (uint32_t)i < n_chunks; i++)
+        if (int rc = g.lane_work[kEncLanes + i].ensure(selab200_verify_workspace_bytes(plan.max_frames, channels))) return rc;
     int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
     uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
     uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
+    // every offset the encoder hands out while its status is clean lies below both of these
+    const size_t arena_words = std::min(words_capacity, selab200_encode_words_bound(n_frames, channels));
+    VerifyArea va;
+    if (verify)
+        if (int rc = verify_area(n_sub, arena_words, g.s_compute[0], va)) return rc;
 
     CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
@@ -876,6 +1013,29 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                    (unsigned long long)f0 * channels))
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
+        if (verify) {
+            // The bytes just gathered, read back the way a reader does: the word arrays unpacked from the image,
+            // decoded, and compared with the PCM this chunk already holds.  The guard hands the unpack empty
+            // descriptors once the encoder has failed (offsets past the arena), and the call fails anyway.
+            const size_t chunk_sub = (size_t)nf * channels;
+            selab200_subframe_desc *vd = va.descs + (size_t)f0 * channels;
+            cudaStream_t vs = g.s_compute[kEncLanes + c % kVerifyLanes];
+            DeviceBuffer &vws = g.lane_work[kEncLanes + c % kVerifyLanes];
+            CUDA_TRY(cudaStreamWaitEvent(vs, g.ev_done[c], 0));
+            k_verify_guard_descs<<<(unsigned)((chunk_sub + 255) / 256), 256, 0, vs>>>(d_descs + (size_t)f0 * channels,
+                                                                                   (uint32_t)chunk_sub, d_status, vd);
+            if (int rc = launch_check("k_verify_guard_descs"))
+                return rc;
+            k_container_unpack<<<(unsigned)((chunk_sub + 7) / 8), 256, 0, vs>>>(static_cast<const uint8_t *>(g.words.ptr), vd,
+                                                                               (uint32_t)chunk_sub, channels,
+                                                                               (unsigned long long)f0 * channels, va.arena);
+            if (int rc = launch_check("k_container_unpack"))
+                return rc;
+            if (int rc = verify_device(vd, nf, channels, va.arena, arena_words, d_pcm + (size_t)f0 * channels * kFrame,
+                                       va.entries + (size_t)f0 * channels, va.count, va.status, vws.ptr, vws.bytes, vs,
+                                       false, frame_base + f0))
+                return rc;
+        }
     }
     g.h_totals[0] = 0;
     for (uint32_t c = 0; c < n_chunks; c++) {
@@ -903,7 +1063,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                  g.s_d2h));
         CUDA_TRY(cudaMemcpyAsync(words + lo, d_words + lo, (hi - lo) * 4, cudaMemcpyDeviceToHost, g.s_d2h));
     }
-    for (int i = 0; i < kEncLanes; i++)
+    for (int i = 0; i < (verify ? kLanes : kEncLanes); i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
     CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.s_d2h));
     CUDA_TRY(cudaStreamSynchronize(g.s_d2h));
@@ -912,7 +1072,25 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     *words_used = (size_t)used; // for CAPACITY: the size the caller needs
     if (g.h_small[0] != 0)
         return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    return 0;
+    return verify ? collect_report(va, n_sub, g.s_d2h, *report) : 0;
+}
+
+// The words n descriptors reference, [lo, hi) (descriptors need not be in arena order); hi <= lo if none.
+static void words_referenced(const selab200_subframe_desc *dc, size_t n, size_t n_words, unsigned long long &lo,
+                             unsigned long long &hi)
+{
+    lo = ~0ull;
+    hi = 0;
+    for (size_t i = 0; i < n; i++) {
+        const unsigned long long a0 = dc[i].refl_offset, a1 = a0 + dc[i].refl_words;
+        const unsigned long long b0 = dc[i].res_offset, b1 = b0 + dc[i].res_words;
+        if (a1 <= n_words && b1 <= n_words) { // out-of-range descriptors are rejected on the device
+            lo = a0 < lo ? a0 : lo;
+            lo = b0 < lo ? b0 : lo;
+            hi = a1 > hi ? a1 : hi;
+            hi = b1 > hi ? b1 : hi;
+        }
+    }
 }
 
 static int decode_host(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -945,19 +1123,9 @@ static int decode_host(const selab200_subframe_desc *descs, uint32_t n_frames, u
         CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
     for (uint32_t c = 0; c < n_chunks; c++) {
         const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
-        // the words this chunk's descriptors reference (descriptors need not be in arena order)
-        unsigned long long lo = ~0ull, hi = 0;
         const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
-        for (size_t i = 0; i < (size_t)nf * channels; i++) {
-            const unsigned long long a0 = dc[i].refl_offset, a1 = a0 + dc[i].refl_words;
-            const unsigned long long b0 = dc[i].res_offset, b1 = b0 + dc[i].res_words;
-            if (a1 <= n_words && b1 <= n_words) { // out-of-range descriptors are rejected on the device
-                lo = a0 < lo ? a0 : lo;
-                lo = b0 < lo ? b0 : lo;
-                hi = a1 > hi ? a1 : hi;
-                hi = b1 > hi ? b1 : hi;
-            }
-        }
+        unsigned long long lo, hi;
+        words_referenced(dc, (size_t)nf * channels, n_words, lo, hi);
         CUDA_TRY(cudaMemcpyAsync(d_descs + (size_t)f0 * channels, dc, (size_t)nf * channels * sizeof(*dc),
                                  cudaMemcpyHostToDevice, g.s_h2d));
         if (hi > lo)
@@ -977,6 +1145,59 @@ static int decode_host(const selab200_subframe_desc *descs, uint32_t n_frames, u
     return read_status(g.s_d2h, d_status);
 }
 
+// decode_host with a compare instead of the download: the source PCM goes up with the coded chunk, each lane
+// decodes into its own scratch and compares there (verify_device), and only the count -- and the per-pair
+// records when it is not zero -- come back.  Frames in the report are numbered from frame_base.
+static int verify_host(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels, const uint32_t *words,
+                       size_t n_words, const int16_t *pcm, uint32_t frame_base, std::vector<selab200_verify_entry> &report)
+{
+    report.clear();
+    if (n_frames == 0)
+        return 0;
+    PipelineDrain drain;
+    const ChunkPlan plan = plan_chunks(n_frames);
+    const uint32_t n_chunks = plan.chunks();
+    const size_t n_sub = (size_t)n_frames * channels;
+    const size_t frame_bytes = (size_t)channels * kFrame * 2;
+    const size_t ws_bytes = selab200_verify_workspace_bytes(plan.max_frames, channels);
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
+    for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
+        if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
+    int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
+    selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
+    uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
+    VerifyArea va;
+    if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
+    CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
+    for (int i = 1; i < kLanes; i++)
+        CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
+    for (uint32_t c = 0; c < n_chunks; c++) {
+        const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
+        const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
+        unsigned long long lo, hi;
+        words_referenced(dc, (size_t)nf * channels, n_words, lo, hi);
+        CUDA_TRY(cudaMemcpyAsync(d_descs + (size_t)f0 * channels, dc, (size_t)nf * channels * sizeof(*dc),
+                                 cudaMemcpyHostToDevice, g.s_h2d));
+        if (hi > lo)
+            CUDA_TRY(cudaMemcpyAsync(d_words + lo, words + lo, (hi - lo) * 4, cudaMemcpyHostToDevice, g.s_h2d));
+        CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)f0 * channels * kFrame,
+                                 nf * frame_bytes, cudaMemcpyHostToDevice, g.s_h2d));
+        CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
+        cudaStream_t cs = g.s_compute[c % kLanes];
+        DeviceBuffer &ws = g.lane_work[c % kLanes];
+        CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[c], 0));
+        if (int rc = verify_device(d_descs + (size_t)f0 * channels, nf, channels, d_words, n_words,
+                                   d_pcm + (size_t)f0 * channels * kFrame, va.entries + (size_t)f0 * channels, va.count,
+                                   va.status, ws.ptr, ws.bytes, cs, false, frame_base + f0))
+            return rc;
+    }
+    for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
+        CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
+    return collect_report(va, n_sub, g.s_d2h, report);
+}
+
 // ---- every initialised device at once ----------------------------------------------------------
 //
 // Frames are independent (src/sela/encoder.cpp:40-92 hands contiguous ranges of them to its threads); with more
@@ -992,7 +1213,17 @@ struct DevicePart {
     int rc = 0;
     size_t used = 0;
     char err[sizeof g_error] = "";
+    std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
 };
+
+// The blocks' reports one after the other: blocks are contiguous and in frame order, so this is in order too.
+static std::vector<selab200_verify_entry> joined_reports(const std::vector<DevicePart> &parts)
+{
+    std::vector<selab200_verify_entry> all;
+    for (const DevicePart &p : parts)
+        all.insert(all.end(), p.report.begin(), p.report.end());
+    return all;
+}
 
 static std::vector<DevicePart> device_parts(uint32_t n_frames)
 {
@@ -1037,14 +1268,18 @@ static int run_on_devices(std::vector<DevicePart> &parts, F work)
 }
 
 static int encode_all_devices(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
-                              uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container)
+                              uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
+                              std::vector<selab200_verify_entry> *report = nullptr)
 {
     std::vector<DevicePart> parts = device_parts(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
     const int rc = run_on_devices(parts, [&](DevicePart &p) {
         return encode_host(pcm + p.f0 * per_frame, p.nf, channels, descs ? descs + (size_t)p.f0 * channels : nullptr, nullptr,
-                           selab200_encode_words_bound(p.nf, channels), &p.used, container, true);
+                           selab200_encode_words_bound(p.nf, channels), &p.used, container, true,
+                           report ? &p.report : nullptr, p.f0);
     });
+    if (report)
+        *report = joined_reports(parts);
     size_t total = 0;
     for (const DevicePart &p : parts)
         total += p.used;
@@ -1103,6 +1338,20 @@ static int decode_all_devices(const selab200_subframe_desc *descs, uint32_t n_fr
     });
 }
 
+static int verify_all_devices(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
+                              const uint32_t *words, size_t n_words, const int16_t *pcm,
+                              std::vector<selab200_verify_entry> &report)
+{
+    std::vector<DevicePart> parts = device_parts(n_frames);
+    const size_t per_frame = (size_t)channels * kFrame;
+    const int rc = run_on_devices(parts, [&](DevicePart &p) {
+        return verify_host(descs + (size_t)p.f0 * channels, p.nf, channels, words, n_words, pcm + p.f0 * per_frame, p.f0,
+                           p.report);
+    });
+    report = joined_reports(parts);
+    return rc;
+}
+
 extern "C" {
 
 int selab200_encode_frames(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
@@ -1126,10 +1375,13 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
 }
 
-int selab200_encode_container(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
-                              uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used)
+} // extern "C"
+
+// selab200_encode_container, and with `report` its verified form (g_mutex held by the caller).
+static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                                 uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
+                                 std::vector<selab200_verify_entry> *report)
 {
-    std::lock_guard<std::mutex> lock(g_mutex);
     if (int rc = require_ready())
         return rc;
     if ((!pcm && n_frames) || !container || !bytes_used)
@@ -1148,10 +1400,40 @@ int selab200_encode_container(const int16_t *pcm, uint32_t n_frames, uint32_t ch
     memcpy(container, header, sizeof header);
     size_t words_used = 0;
     const int rc = use_all_devices(n_frames)
-                       ? encode_all_devices(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used, container)
-                       : encode_host(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used, container);
+                       ? encode_all_devices(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
+                                            container, report)
+                       : encode_host(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
+                                     container, false, report);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
     return rc;
+}
+
+extern "C" {
+
+int selab200_encode_container(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                              uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
+                                 nullptr);
+}
+
+int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                                       uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
+                                       selab200_verify_entry *entries, size_t entries_capacity, size_t *n_entries)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!n_entries || (!entries && entries_capacity)) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    *n_entries = 0;
+    std::vector<selab200_verify_entry> report;
+    if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                       bytes_used, &report))
+        return rc;
+    return deliver_report(report, entries, entries_capacity, n_entries);
 }
 
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -1167,6 +1449,26 @@ int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frame
     if (use_all_devices(n_frames))
         return decode_all_devices(descs, n_frames, channels, words, n_words, pcm_out);
     return decode_host(descs, n_frames, channels, words, n_words, pcm_out);
+}
+
+int selab200_verify_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
+                           const uint32_t *words, size_t n_words, const int16_t *pcm, selab200_verify_entry *entries,
+                           size_t capacity, size_t *n_entries)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (((!descs || !pcm) && n_frames) || (!words && n_words) || (!entries && capacity) || !n_entries)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    *n_entries = 0;
+    std::vector<selab200_verify_entry> report;
+    const int rc = use_all_devices(n_frames) ? verify_all_devices(descs, n_frames, channels, words, n_words, pcm, report)
+                                             : verify_host(descs, n_frames, channels, words, n_words, pcm, 0, report);
+    if (rc)
+        return rc;
+    return deliver_report(report, entries, capacity, n_entries);
 }
 
 // ---- .sela container, decode side ----------------------------------------------------------
@@ -1387,8 +1689,13 @@ int selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_c
 // whole byte image (uploaded by selab200_container_open, in pieces with events); any other device uploads just
 // the bytes of its block.  The word arena keeps the descriptors' file-order offsets: it is addressed through a
 // pointer shifted back by the block's first word, so nothing is re-based.
-static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t NF, int16_t *pcm_out, bool primary)
+// With `report` the block is verified instead of downloaded: pcm (the whole file's source PCM) goes up chunk by
+// chunk on the chunk's lane, every lane decodes into its own scratch and compares (verify_device).
+static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t NF, int16_t *pcm_out, bool primary,
+                                  const int16_t *pcm = nullptr, std::vector<selab200_verify_entry> *report = nullptr)
 {
+    if (report)
+        report->clear();
     if (NF == 0)
         return 0;
     const uint32_t channels = h->info.channels;
@@ -1398,7 +1705,8 @@ static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t N
     const uint32_t n_chunks = plan.chunks();
     const size_t n_sub = (size_t)NF * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const size_t ws_bytes = selab200_decode_workspace_bytes(plan.max_frames, channels);
+    const size_t ws_bytes = report ? selab200_verify_workspace_bytes(plan.max_frames, channels)
+                                   : selab200_decode_workspace_bytes(plan.max_frames, channels);
     const size_t n_words = (size_t)h->info.n_words;
     const unsigned long long w_lo = hd[(size_t)F0 * channels].refl_offset;
     const selab200_subframe_desc &tail = hd[(size_t)(F0 + NF) * channels - 1];
@@ -1424,6 +1732,9 @@ static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t N
         CUDA_TRY(cudaEventRecord(g.ev_h2d[0], g.s_h2d));
         d_bytes = static_cast<const uint8_t *>(g.aux.ptr) - b0;
     }
+    VerifyArea va;
+    if (report)
+        if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
 
     CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
@@ -1454,6 +1765,15 @@ static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t N
                                                                            (unsigned long long)(F0 + f0) * channels, d_arena);
         if (int rc = launch_check("k_container_unpack"))
             return rc;
+        if (report) {
+            CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)(F0 + f0) * channels * kFrame,
+                                     nf * frame_bytes, cudaMemcpyHostToDevice, cs));
+            if (int rc = verify_device(d_descs + (size_t)f0 * channels, nf, channels, d_arena, n_words,
+                                       d_pcm + (size_t)f0 * channels * kFrame, va.entries + (size_t)f0 * channels,
+                                       va.count, va.status, ws.ptr, ws.bytes, cs, false, F0 + f0))
+                return rc;
+            continue;
+        }
         if (int rc = decode_device(d_descs + (size_t)f0 * channels, nf, channels, d_arena, n_words,
                                    d_pcm + (size_t)f0 * channels * kFrame, d_status, ws.ptr, ws.bytes, cs, false))
             return rc;
@@ -1461,6 +1781,11 @@ static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t N
         CUDA_TRY(cudaStreamWaitEvent(g.s_d2h, g.ev_done[c], 0));
         CUDA_TRY(cudaMemcpyAsync(pcm_out + (size_t)(F0 + f0) * channels * kFrame, d_pcm + (size_t)f0 * channels * kFrame,
                                  nf * frame_bytes, cudaMemcpyDeviceToHost, g.s_d2h));
+    }
+    if (report) {
+        for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
+            CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
+        return collect_report(va, n_sub, g.s_d2h, *report);
     }
     return read_status(g.s_d2h, d_status);
 }
@@ -1486,6 +1811,38 @@ int selab200_container_decode(selab200_container *h, int16_t *pcm_out)
     // one block of frames per device; the primary (which holds the whole image) takes the first
     std::vector<DevicePart> parts = device_parts(n_frames);
     return run_on_devices(parts, [&](DevicePart &p) { return container_decode_block(h, p.f0, p.nf, pcm_out, tl_ctx == &g_slots[0]); });
+}
+
+int selab200_container_verify(selab200_container *h, const int16_t *pcm, selab200_verify_entry *entries, size_t capacity,
+                              size_t *n_entries)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!h || !n_entries || (!entries && capacity))
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    *n_entries = 0;
+    const uint32_t n_frames = h->info.n_frames, channels = h->info.channels;
+    if (n_frames == 0)
+        return 0;
+    if (!pcm)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    std::vector<selab200_verify_entry> report;
+    int rc;
+    if (!use_all_devices(n_frames)) {
+        rc = container_decode_block(h, 0, n_frames, nullptr, true, pcm, &report);
+    } else {
+        std::vector<DevicePart> parts = device_parts(n_frames);
+        rc = run_on_devices(parts, [&](DevicePart &p) {
+            return container_decode_block(h, p.f0, p.nf, nullptr, tl_ctx == &g_slots[0], pcm, &p.report);
+        });
+        report = joined_reports(parts);
+    }
+    if (rc)
+        return rc;
+    return deliver_report(report, entries, capacity, n_entries);
 }
 
 int selab200_selftest(uint32_t *mismatches)

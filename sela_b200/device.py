@@ -49,6 +49,38 @@ class DeviceCodec:
             pcm_out.data_ptr(), self.status.data_ptr() + 4, self.dec_ws.data_ptr(), self.dec_ws_bytes,
             C.c_void_p(stream)))
 
+    def verify(self, pcm_ref, n_words):
+        """Decode self.descs / self.words[:n_words] and compare with pcm_ref (int16 cuda tensor, 16-byte aligned):
+        per-pair records and the count of differing pairs stay on the device.  Asynchronous; verify_report()
+        collects the result.  The verify buffers are allocated on first use."""
+        assert pcm_ref.dtype == torch.int16 and pcm_ref.is_cuda and pcm_ref.numel() == self.n_sub * FRAME
+        L = lib()
+        if not hasattr(self, "ver_ws"):
+            self.ver_ws_bytes = L.selab200_verify_workspace_bytes(self.n_frames, self.channels)
+            self.ver_ws = torch.zeros(self.ver_ws_bytes, dtype=torch.uint8, device=self.device)
+            self.ver_entries = torch.zeros(max(self.n_sub, 1) * 16, dtype=torch.uint8, device=self.device)
+            self.ver_count = torch.zeros(1, dtype=torch.int64, device=self.device)
+            self.ver_status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_verify_frames_device(
+            self.descs.data_ptr(), self.n_frames, self.channels, self.words.data_ptr(), int(n_words),
+            pcm_ref.data_ptr(), self.ver_entries.data_ptr(), self.ver_count.data_ptr(), self.ver_status.data_ptr(),
+            self.ver_ws.data_ptr(), self.ver_ws_bytes, C.c_void_p(stream)))
+
+    def verify_report(self):
+        """Synchronises; raises if the last verify's decode reported an error, else returns its report: a
+        VERIFY_DTYPE array of the differing (frame, channel) pairs in order (per-pair records copied only
+        when there are any)."""
+        import numpy as np
+        from ._lib import SelaB200Error, STATUS_NAMES, VERIFY_DTYPE
+        st = int(self.ver_status.item())
+        if st != 0:
+            raise SelaB200Error(st, "verify reported %s" % STATUS_NAMES.get(st, st))
+        if int(self.ver_count.item()) == 0:
+            return np.zeros(0, VERIFY_DTYPE)
+        rec = self.ver_entries.cpu().numpy().view(VERIFY_DTYPE)[:self.n_sub]
+        return rec[rec["n_differing"] != 0].copy()
+
     def check_status(self):
         """Synchronises; raises if either the last encode or decode reported an error."""
         from ._lib import SelaB200Error, STATUS_NAMES

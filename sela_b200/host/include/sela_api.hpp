@@ -99,9 +99,21 @@ public:
 } // namespace file
 
 namespace sela {
+// Not in the reference: one decoded (frame, channel) that differs from its source (selab200_verify_entry).
+// The format is not lossless for every input: encoder and decoder round the prediction differently when it
+// lands exactly on a half, and the decoded channel drifts away from the source from that sample on.
+struct VerifyEntry {
+    uint32_t frame;
+    uint16_t channel;
+    uint16_t firstSample;      // first differing sample, within the frame
+    uint32_t differingSamples; // how many of the frame's 2048 samples differ
+    int32_t firstDelta;        // decoded - source at firstSample
+};
+
 class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
+    void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -112,6 +124,10 @@ public:
     // The WAV data chunk goes to the device as it lies in the file and the .sela byte stream comes
     // back ready to write (selab200_encode_container): no per-frame value structs on the host.
     void processTo(std::ofstream &outputFile);
+    // Not in the reference: processTo() that also proves what it wrote (`flac --verify`): the bytes are decoded
+    // on the device and compared with the WAV's whole frames.  Same bytes as processTo(); `report` receives
+    // every (frame, channel) that does not decode back to its source, in order (empty: lossless).
+    void processTo(std::ofstream &outputFile, std::vector<VerifyEntry> &report);
 };
 class Decoder {
     void readFrames();
@@ -125,6 +141,11 @@ public:
     // Not in the reference: process() + WavFile::writeToFile() in one step, byte-identical output
     // (selab200_container_open / _decode: the .sela bytes go to the device as they lie in the file).
     void processTo(std::ofstream &outputFile);
+    // Not in the reference: decode this .sela stream on the device and compare it with the whole frames of the
+    // WAV file `wavInput` (its partial final frame is ignored, as the encoder ignores it).  Returns every
+    // (frame, channel) that differs, in order.  Throws data::Exception if the WAV's channels, sample rate or
+    // whole-frame count disagree with the .sela header.
+    std::vector<VerifyEntry> verifyAgainst(std::ifstream &wavInput);
 };
 // Not in the reference.  On: the processTo() drivers keep page-locked staging buffers per host thread
 // and reuse them from file to file (a process that codes many files, e.g. `sela -E`); off (default):

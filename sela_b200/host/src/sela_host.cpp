@@ -774,11 +774,28 @@ file::SelaFile Encoder::process()
     return file::SelaFile(fmt.sampleRate, fmt.bitsPerSample, (uint8_t)fmt.numChannels, std::move(frames));
 }
 
+// The library's report in the mirror's terms.
+static std::vector<VerifyEntry> mirror_report(const std::vector<selab200_verify_entry> &raw, size_t n)
+{
+    std::vector<VerifyEntry> out;
+    out.reserve(n);
+    for (size_t i = 0; i < n && i < raw.size(); i++)
+        out.push_back(VerifyEntry{raw[i].frame, raw[i].channel, raw[i].first_sample, raw[i].n_differing, raw[i].first_delta});
+    return out;
+}
+
 // process() + file::SelaFile::writeToFile() without the detour through per-frame value structs:
 // the data chunk is handed to the device where it lies in the file buffer, and what comes back is
 // the .sela byte stream.  Output is byte-identical to the two-step path (tests/test_host_cli.py).
-void Encoder::processTo(std::ofstream &outputFile)
+void Encoder::processTo(std::ofstream &outputFile) { encodeTo(outputFile, nullptr); }
+
+void Encoder::processTo(std::ofstream &outputFile, std::vector<VerifyEntry> &report) { encodeTo(outputFile, &report); }
+
+// processTo(); with `report` through selab200_encode_container_verified (same bytes).
+void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report)
 {
+    if (report)
+        report->clear();
     StagingScope staging;
     DeviceWarmup warmup; // CUDA context creation overlaps the file read
     if (g_batch_mode.load())
@@ -808,7 +825,15 @@ void Encoder::processTo(std::ofstream &outputFile)
     const size_t cap = selab200_container_bound((uint32_t)n_frames, channels);
     uint8_t *out = reinterpret_cast<uint8_t *>(t_output.ensure(cap));
     size_t used = 0;
-    {
+    if (report) {
+        Phase p("encode + verify (device)");
+        std::vector<selab200_verify_entry> raw(n_frames * channels);
+        size_t n = 0;
+        check(selab200_encode_container_verified(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                 (uint32_t)n_frames, channels, w.fmt.sampleRate, w.fmt.bitsPerSample,
+                                                 out, cap, &used, raw.data(), raw.size(), &n));
+        *report = mirror_report(raw, n);
+    } else {
         Phase p("encode (device)");
         check(selab200_encode_container(reinterpret_cast<const int16_t *>(file.data + dat.body), (uint32_t)n_frames,
                                         channels, w.fmt.sampleRate, w.fmt.bitsPerSample, out, cap, &used));
@@ -861,6 +886,67 @@ void Decoder::processTo(std::ofstream &outputFile)
     shell.wavChunk.dataSubChunk.subChunkSize = (uint32_t)payload;
     write_wav_header(outputFile, shell.wavChunk);
     outputFile.write(reinterpret_cast<const char *>(pcm), (std::streamsize)(n_samples * 2));
+}
+
+// The .sela stream against a WAV file: the .sela bytes go to the device as processTo() sends them, the WAV's
+// data chunk goes up chunk by chunk from where it lies in the file buffer, and only the report comes back.
+std::vector<VerifyEntry> Decoder::verifyAgainst(std::ifstream &wavInput)
+{
+    StagingScope staging;
+    DeviceWarmup warmup;
+    if (g_batch_mode.load())
+        warmup.join();
+    RawFile file;
+    char *wav = nullptr;
+    size_t wav_size = 0;
+    {
+        Phase p("read inputs");
+        file = slurp_raw(ifStream);
+        wavInput.seekg(0, std::ios::end);
+        const std::streamoff size = wavInput.tellg();
+        wav_size = size > 0 ? (size_t)size : 0;
+        wav = t_output.ensure(wav_size + 1);
+        wavInput.seekg(0, std::ios::beg);
+        if (wav_size)
+            wavInput.read(wav, (std::streamsize)wav_size);
+    }
+    const WavLayout w = scan_wav(wav, wav_size);
+    const WavSpan &dat = w.spans[w.dataIndex];
+    warmup.join();
+    selab200_container *handle = nullptr;
+    selab200_container_info info;
+    {
+        Phase p("open (upload + walk)");
+        if (selab200_container_open(file.bytes(), file.size, &handle, &info) != SELAB200_OK)
+            raise(selab200_last_error());
+    }
+    struct Closer {
+        selab200_container *h;
+        ~Closer() { selab200_container_close(h); }
+    } closer{handle};
+    const uint32_t channels = w.fmt.numChannels;
+    if (channels != info.channels)
+        raise("the WAV file has " + std::to_string(channels) + " channels, the sela file " + std::to_string(info.channels));
+    if (w.fmt.sampleRate != info.sample_rate)
+        raise("the WAV file's sample rate is " + std::to_string(w.fmt.sampleRate) + " Hz, the sela file's " +
+              std::to_string(info.sample_rate) + " Hz");
+    // file::WavFile::demuxSamples (src/file/wav_file.cpp:181-220): whole frames only
+    const size_t wav_frames = channels ? ((size_t)dat.size * 8 / w.fmt.bitsPerSample) / ((size_t)kFrame * channels) : 0;
+    if (wav_frames != info.header_frames)
+        raise("the WAV file holds " + std::to_string(wav_frames) + " whole frames, the sela header declares " +
+              std::to_string(info.header_frames));
+    if (info.n_frames != info.header_frames)
+        raise("the sela file holds " + std::to_string(info.n_frames) + " of the " + std::to_string(info.header_frames) +
+              " frames its header declares");
+    if (info.n_frames > 0 && (channels == 0 || channels > SELAB200_MAX_CHANNELS))
+        raise("sela_b200: unsupported channel count");
+    std::vector<selab200_verify_entry> raw((size_t)info.n_frames * channels);
+    size_t n = 0;
+    {
+        Phase p("verify (device)");
+        check(selab200_container_verify(handle, reinterpret_cast<const int16_t *>(wav + dat.body), raw.data(), raw.size(), &n));
+    }
+    return mirror_report(raw, n);
 }
 
 // sela::Decoder::processFrames (src/sela/decoder.cpp:41-92)
