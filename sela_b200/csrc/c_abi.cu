@@ -503,19 +503,13 @@ int decode_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint
         return rc;
     if (int rc = launch_rice_residues(p, rice_aux, stream))
         return rc;
-    p.fallback_only = 1;
     k_synthesise_segments<<<(unsigned)n_warps, 32, 0, stream>>>(p);
     if (int rc = launch_check("k_synthesise_segments"))
         return rc;
-    if (channels == 2) { // every stereo frame is handled by the batch kernel + the difference fix-up
-        k_diff_fixup<<<n_frames, 128, 0, stream>>>(p);
-        return launch_check("k_diff_fixup");
-    }
-    const size_t smem = synthesise_smem_bytes(channels);
-    if (int rc = set_smem(k_synthesise, smem))
-        return rc;
-    k_synthesise<<<n_frames, 32 * ((channels + 1) / 2), smem, stream>>>(p);
-    return launch_check("k_synthesise");
+    if (channels == 1) // desc_ok admits no difference subframe: its parent would have to be another channel
+        return 0;
+    k_diff_fixup<<<n_frames, 128, 0, stream>>>(p);
+    return launch_check("k_diff_fixup");
 }
 
 int read_status(cudaStream_t stream, const int32_t *d_status)
@@ -902,7 +896,6 @@ int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, ui
     p.ws_q = nullptr;
     p.ws_res = d_residues;
     p.seg_index = nullptr;
-    p.fallback_only = 0;
     p.rice_flags = nullptr;
     if (int rc = g.aux.ensure((size_t)n_frames * channels * 64 + 256))
         return rc;

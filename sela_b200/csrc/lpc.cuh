@@ -14,12 +14,8 @@ namespace selab200 {
 // Per-warp shared memory.  The predictor (shared by encoder and decoder):
 struct CoefSmem {
     uint32_t clo[112];           // low / high words of the Q35 coefficients c[1..], tap j at index
-    int32_t  chi[112];           //   j-1, zero padded: the FIR / IIR read them in blocks of 8
+    int32_t  chi[112];           //   j-1, zero padded: the FIR reads them in blocks of 8
     int32_t  q[104];             // quantised reflection coefficients
-};
-// Decoder only: warm-up bias table of the IIR, 2^34 + 2^31 * sum_{j<=t} c[j] mod 2^64  (t = 0..order)
-struct IirSmem {
-    unsigned long long pre[104];
 };
 // Analysis scratch (3 KB).  The ring is dead once the autocorrelation is done; the
 // reflection coefficients (kk) and the step-up row (t) then live in its bytes.
@@ -503,154 +499,23 @@ __device__ void warp_fir_residual(const Signal &sig, const CoefSmem &cf, int ord
 //   s[i] = r[i] - (int)((2^34 - sum_{j=1..order} c[j]*s[i-j]) >> 35),  s[<0] = 0
 // Decoded samples can be any int32: they enter the products biased by 2^31 (kSynthBias), so that
 // c*s' needs one IMAD.WIDE.U32 (low word of c) and one IMAD (high word), and the bias is taken
-// out once per output (the prefix table below):
+// out once per output (segment_state):
 //   sum_j c[j]*s[i-j] = sum_j c[j]*s'[i-j] - 2^31 * sum_j c[j].
 // Products and sums wrap mod 2^64, which cancels exactly: the result is the reference's int64
 // sum wherever that sum does not overflow.
-// A true recurrence, evaluated in TRANSPOSED form: lane l owns taps TPL*l+1..TPL*l+TPL
+// A true recurrence, evaluated in TRANSPOSED form: a lane owns kTapsPerLane consecutive taps
 // and the partial sums of the outputs those taps will feed next.  When s[i] becomes
 // known every lane adds c[j]*s'[i] to the accumulator of output i+j; the accumulator
-// of output i+1 (tap 1, lane 0) is then complete, lane 0 finishes the sample and
+// of output i+1 (tap 1, first lane) is then complete, that lane finishes the sample and
 // broadcasts it, and every accumulator moves one tap down (one 64-bit shuffle per
 // lane, register renaming inside a lane).  Critical path per sample: one IMAD, a
 // 64-bit subtract, a shift and ONE shuffle -- instead of a five-level reduction.
-__device__ void warp_iir_prepare(const CoefSmem &cf, IirSmem &ii, int order)
-{
-    // pre[t] = 2^34 + 2^31 * sum_{j=1..t} c[j] (mod 2^64): removes the sample bias for output t
-    // (during warm-up only taps j <= t have seen a real sample)
-    const int lane = lane_id();
-    long long v[4], run = 0;
-#pragma unroll
-    for (int m = 0; m < 4; m++) {
-        const int j = 4 * lane + m + 1;
-        run += (j <= order && j <= 112) ? coef_at(cf, j) : 0;
-        v[m] = run;
-    }
-    unsigned long long incl = (unsigned long long)run;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        unsigned long long tmp = __shfl_up_sync(kFull, incl, o);
-        if (lane >= o)
-            incl += tmp;
-    }
-    const unsigned long long excl = incl - (unsigned long long)run;
-#pragma unroll
-    for (int m = 0; m < 4; m++) {
-        const int j = 4 * lane + m + 1;
-        if (j < 104)
-            ii.pre[j] = (1ull << (kQ - 1)) + ((excl + (unsigned long long)v[m]) << 31);
-    }
-    if (lane == 0)
-        ii.pre[0] = 1ull << (kQ - 1);
-    __syncwarp();
-}
-
-// Two subframes share a warp: lanes 0-15 run subframe A, lanes 16-31 subframe B, each
-// lane owning TPL taps (TPL*15 >= order, so the last lane of a half only ever holds
-// zero coefficients and its accumulators stay zero -- shfl_down past the half's edge
-// returns the lane's own, zero, value: no special case).  Per step the warp issues
-// 2*TPL IMADs + ~14 bookkeeping instructions for TWO samples.
-template <int TPL>
-__device__ void warp_iir_pair(const CoefSmem &cf, const IirSmem &ii, int order, int32_t *buf, bool active, int n, int order_max)
-{
-    const int hl = lane_id() & 15;
-    uint32_t cl[TPL];
-    int32_t ch[TPL];
-#pragma unroll
-    for (int m = 0; m < TPL; m++) {
-        const int j = TPL * hl + m; // tap j+1
-        cl[m] = j < 112 ? cf.clo[j] : 0u;
-        ch[m] = j < 112 ? cf.chi[j] : 0;
-    }
-    // accumulators: 64-bit low-word products + a separate 32-bit column for the high-word
-    // products (one IMAD.WIDE.U32 + one IMAD per tap); combined only when handed on
-    unsigned long long alo[TPL];
-    uint32_t ahi[TPL];
-#pragma unroll
-    for (int m = 0; m < TPL; m++) {
-        alo[m] = 0;
-        ahi[m] = 0;
-    }
-    const unsigned long long steady = ii.pre[order];
-    uint32_t sp = synth_biased(buf[0]); // s[0] = r[0]
-    const bool writer = active && hl == 0;
-    // step(u, i, base): consumes s'[i] in `sp`, produces s[i+1].  Slot m of this step
-    // lives in physical register (m + u) % TPL, so the per-step slot shift is free.
-#define SELAB200_IIR_STEP(u, i, base)                                                            \
-    {                                                                                            \
-        _Pragma("unroll") for (int m = 0; m < TPL; m++)                                          \
-        {                                                                                        \
-            alo[(m + (u)) % TPL] = mad_wide_u32(cl[m], sp, alo[(m + (u)) % TPL]);               \
-            ahi[(m + (u)) % TPL] += (uint32_t)ch[m] * sp;                                        \
-        }                                                                                        \
-        const unsigned long long full0 = alo[(u) % TPL] + ((unsigned long long)ahi[(u) % TPL] << 32); \
-        const unsigned long long incoming = __shfl_down_sync(kFull, full0, 1, 16);               \
-        const unsigned long long tt = (base) - full0;                                            \
-        int vnext = buf[(i) + 1] - (int32_t)((long long)tt >> kQ);                               \
-        vnext = __shfl_sync(kFull, vnext, 0, 16);                                                \
-        if (writer)                                                                              \
-            buf[(i) + 1] = vnext;                                                                \
-        alo[(u) % TPL] = incoming; /* becomes the top slot of the next step */                   \
-        ahi[(u) % TPL] = 0;                                                                      \
-        sp = synth_biased(vnext);                                                                \
-    }
-    int i = 0;
-    const int last = n - 1; // steps i = 0 .. last-1
-    // warm-up: outputs 1..order use the prefix table (the longer of the two orders decides)
-    const int warm = order_max < last ? order_max : last;
-    const int warm_groups = (warm + TPL - 1) / TPL;
-    for (int gq = 0; gq < warm_groups; gq++) {
-#pragma unroll
-        for (int u = 0; u < TPL; u++) {
-            if (i < last) {
-                const int t = i + 1;
-                const unsigned long long base = ii.pre[t < order ? t : order];
-                SELAB200_IIR_STEP(u, i, base);
-                i++;
-            }
-        }
-    }
-    // steady state
-    for (; i + TPL <= last;) {
-#pragma unroll
-        for (int u = 0; u < TPL; u++) {
-            SELAB200_IIR_STEP(u, i, steady);
-            i++;
-        }
-    }
-#pragma unroll
-    for (int u = 0; u < TPL; u++) {
-        if (i < last) {
-            SELAB200_IIR_STEP(u, i, steady);
-            i++;
-        }
-    }
-#undef SELAB200_IIR_STEP
-    __syncwarp();
-}
-
-// Synthesis of two subframes in one warp.  cf/buf/order/active are PER HALF (lanes
-// 0-15: A, lanes 16-31: B); cf.pre must be ready (warp_iir_prepare).  buf: r on entry,
-// s on exit (in place), n samples.  An inactive half computes but never stores.
-__device__ void warp_iir_synthesis_pair(const CoefSmem &cf, const IirSmem &ii, int order, int32_t *buf, bool active, int n)
-{
-    const int other = __shfl_xor_sync(kFull, order, 16);
-    const int order_max = order > other ? order : other;
-    if (order_max <= 30)
-        warp_iir_pair<2>(cf, ii, order, buf, active, n, order_max);
-    else if (order_max <= 60)
-        warp_iir_pair<4>(cf, ii, order, buf, active, n, order_max);
-    else
-        warp_iir_pair<8>(cf, ii, order, buf, active, n, order_max);
-}
-
-// ---------------------------------------------------------------------------
-// K6, batch form: a warp runs as many subframes as fit, each on a SEGMENT of consecutive lanes.  A subframe of
+//
+// A warp runs as many subframes as fit, each on a SEGMENT of consecutive lanes.  A subframe of
 // order o owns n = max(1, ceil(o / kTapsPerLane)) lanes; lane k of the segment owns taps kTapsPerLane*k + 1 ..
-// kTapsPerLane*(k+1) (zero beyond o).  Every segment runs the transposed recurrence of warp_iir_pair at once:
-// the segment's top lane takes 0 where the others take the accumulator of the lane above, and the finished
-// sample reaches the segment from its first lane.  Taps per lane are fixed, so the multiplies a warp issues
-// follow the orders it holds instead of the largest order of a class.
+// kTapsPerLane*(k+1) (zero beyond o).  Every segment runs the recurrence at once: the segment's top lane takes 0
+// where the others take the accumulator of the lane above, and the finished sample reaches the segment from its
+// first lane.  Taps per lane are fixed, so the multiplies a warp issues follow the orders it holds.
 constexpr int kTapsPerLane = 8;
 constexpr int kMaxWidth = (kMaxOrder + kTapsPerLane - 1) / kTapsPerLane; // 13 lanes for order 100
 constexpr int kSegBlock = 16; // samples per staging block
@@ -725,8 +590,7 @@ struct SegState {
 
 // Accumulators before the first product: slot m of lane k is output j = kTapsPerLane*k + m + 1, and it starts with
 // what the samples before the subframe contribute in biased form, 2^31 * sum_{j < j' <= order} c[j'] (s[<0] = 0 is
-// s' = 2^31).  Every output then carries the bias of every tap, and one constant removes it from each of them --
-// the same sum mod 2^64 as the warm-up table of warp_iir_pair.
+// s' = 2^31).  Every output then carries the bias of every tap, and one constant removes it from each of them.
 __device__ __forceinline__ void segment_state(SegState &st, int k, int n)
 {
     unsigned long long tot = 0, loc[kTapsPerLane];
@@ -781,6 +645,69 @@ __device__ __forceinline__ void segment_block(SegState &st, const int32_t *in_ro
         if (first)
             out_row[e] = v;
         st.sp = synth_biased(v);
+    }
+}
+
+// The recurrence of every segment of a warp, called by all 32 lanes once sm.row_res / row_out / row_mode are set for
+// every segment ordinal.  This lane is lane k of segment `seg` (of n_seg), n lanes from lane `start`; order is 0 on
+// lanes past the last segment, q points at the segment's quantised reflection coefficients.  Row modes: 0 nothing,
+// 1 int16 PCM (sample t at row_out + t * stride), 2 int32 row.  Residues arrive kSegBlock at a time per segment
+// through cp.async (whole 64-byte pieces of every row, two blocks ahead); finished samples are parked in a staging
+// row per segment and leave kSegBlock at a time, a 32-byte or 64-byte run per segment and instruction.
+__device__ __forceinline__ void segment_synthesis(SegSmem &sm, int start, int k, int n, int seg, int n_seg, int order,
+                                                  const int32_t *q, uint32_t stride)
+{
+    const int lane = lane_id();
+    // residues of block B -> in[B & 1]: eight rows per instruction, four 16-byte pieces per row
+    auto fetch = [&](int B) {
+        for (int i = lane >> 2; i < n_seg; i += 8) {
+            const int32_t *src = sm.row_res[i] + kSegBlock * B + 4 * (lane & 3);
+            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&sm.in[B & 1][i * kSegRow + 4 * (lane & 3)]);
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    fetch(0);
+    fetch(1);
+
+    // ---- predictors: every segment steps its own order up at once ----
+    for (int i = k; i < order; i += n)
+        sm.q[kTapsPerLane * start + i] = q[i];
+    __syncwarp();
+    int order_max = order;
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+        order_max = max(order_max, __shfl_xor_sync(kFull, order_max, o));
+    SegState st;
+    segment_coefficients(sm, start, k, n, order, order_max, st.cl, st.ch);
+    segment_state(st, k, n);
+    st.sp = 0;
+
+    // ---- recurrence + output ----
+    const bool top = k == n - 1, first = k == 0;
+    int32_t *out_row = sm.out + seg * kSegRow;
+    for (int B = 0; B < kFrame / kSegBlock; B++) {
+        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        __syncwarp();
+        const int32_t *in_row = sm.in[B & 1] + seg * kSegRow;
+        if (B == 0)
+            segment_block<true>(st, in_row, out_row, start, top, first);
+        else
+            segment_block<false>(st, in_row, out_row, start, top, first);
+        __syncwarp();
+        for (int i = lane >> 4; i < n_seg; i += 2) {
+            const int mode = sm.row_mode[i];
+            const int e = lane & 15, t = kSegBlock * B + e;
+            const int v = sm.out[i * kSegRow + e];
+            if (mode == 1)
+                static_cast<int16_t *>(sm.row_out[i])[(size_t)t * stride] = (int16_t)(uint16_t)v;
+            else if (mode == 2)
+                static_cast<int32_t *>(sm.row_out[i])[t] = v;
+        }
+        if (B + 2 < kFrame / kSegBlock)
+            fetch(B + 2);
+        else
+            asm volatile("cp.async.commit_group;" ::: "memory");
     }
 }
 

@@ -121,6 +121,14 @@ def signal(rng, amp, n=FRAME):
     return np.clip(np.round(x), I32_MIN, I32_MAX).astype(np.int64)
 
 
+def edge_q(rng, order):
+    """The only predictors that can take int32-limit samples inside the domain are tiny: q = 26 / 27 are the
+    first-order entries closest to a zero reflection coefficient, higher q = 0 is exactly zero."""
+    q = np.zeros(order, np.int32)
+    q[:2] = rng.choice([26, 27], min(order, 2))
+    return q
+
+
 def edge_spikes(O, rng, base, order, q, n_spikes=16, margin=256):
     """`base` with n_spikes samples placed within `margin` of INT32_MAX or INT32_MIN, further apart than the
     predictor is long.  The side is picked per spike so that the residue s + prediction stays inside int32."""
@@ -146,10 +154,7 @@ def crafted_subframe(O, rng, order, kind, channel=0, sub_type=0, parent=None, tr
     parent = channel if parent is None else parent
     for _ in range(tries):
         if kind == "edge":
-            # the only predictors that can take int32-limit samples inside the domain are tiny: q = 26 / 27 are
-            # the first-order entries closest to a zero reflection coefficient, higher q = 0 is exactly zero
-            q = np.zeros(order, np.int32)
-            q[:2] = rng.choice([26, 27], min(order, 2))
+            q = edge_q(rng, order)
             base = signal(rng, 3000)
             s = edge_spikes(O, rng, base, order, q)
         else:
@@ -168,14 +173,18 @@ def crafted_subframe(O, rng, order, kind, channel=0, sub_type=0, parent=None, tr
     raise AssertionError("no in-domain %s subframe of order %d" % (kind, order))
 
 
-def difference_subframe(O, rng, order, parent, channel, tries=40):
+def difference_subframe(O, rng, order, parent, channel, kind="small", tries=40):
     """A difference-coded subframe (type 1) on `parent` (a Sub with known samples) whose parent - difference
-    stays inside int32: small values, of the parent's sign wherever the parent is large."""
+    stays inside int32: small values, of the parent's sign wherever the parent is large.  kind "edge": within
+    2^8 of INT32_MIN wherever the parent is, so that both operands of parent - difference are near INT32_MIN."""
     big = np.abs(parent.samples.astype(np.int64)) > (1 << 30)
+    low = parent.samples.astype(np.int64) <= I32_MIN + 255
     for _ in range(tries):
-        q = draw_q(rng, order)
+        q = edge_q(rng, order) if kind == "edge" else draw_q(rng, order)
         d = signal(rng, 3000)
         d[big] = np.sign(parent.samples[big]) * np.abs(d[big])
+        if kind == "edge":
+            d[low] = I32_MIN + rng.integers(0, 256, int(low.sum()))
         r = residues_for(O, d, order, q)
         if r is not None:
             return Sub(channel, 1, parent.channel, order, q, r, d.astype(np.int32))

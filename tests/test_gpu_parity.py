@@ -290,7 +290,7 @@ def test_decode_descriptors_in_arbitrary_arena_order(O):
         del os.environ["SELAB200_CHUNK_FRAMES"]
 
 
-def test_difference_coding_outside_stereo_uses_general_kernel(O):
+def test_difference_coding_outside_stereo(O):
     """The reference DEcoder accepts difference-coded subframes at any channel count
     (src/frame/frame_decoder.cpp:40-69) although its encoder only emits them for stereo.  Build a
     3-channel frame whose channel 2 is coded as channel0 - channel2 and check against the oracle."""

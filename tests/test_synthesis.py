@@ -3,10 +3,10 @@ against the reference decoder and the exact integer model of tests/exact_decode.
 
 The encoder only produces 16/17-bit signals and the orders its analysis picks; the decoder must reproduce
 the reference for every stream the descriptors admit.  These batches reach what encoder output does not:
-orders on both sides of every predictor-order class edge, four subframes of different orders in one warp,
-class segments with ragged ends and a class change across the 1024-subframe classify tile, samples beyond
-16 bits, below -2^17 and at the int32 limits, permuted channel fields, difference subframes at every
-position and channel count 1-16 (the general kernel k_synthesise)."""
+orders 0-3 and around 28, 56 and 100 (segments of 1, 4, 7, 8 and 13 lanes), subframes of several segment widths
+side by side, ragged width counts and a width change across the 1024-subframe tile of the packing plan, samples
+beyond 16 bits, below -2^17 and at the int32 limits, permuted channel fields, difference subframes at every
+position and channel count 1-16, with parent and difference both near INT32_MIN (k_diff_fixup)."""
 import numpy as np
 import pytest
 
@@ -19,6 +19,16 @@ pytestmark = pytest.mark.gpu
 FRAME = 2048
 ORDERS = [0, 1, 2, 3, 27, 28, 29, 30, 31, 55, 56, 57, 60, 61, 99, 100]
 KINDS = ["small", "wide", "neg17", "edge"]
+TAPS = 8                                                            # kTapsPerLane (lpc.cuh)
+
+
+def width(order):
+    """Lanes of the synthesis segment of a subframe of this order (segment_width, lpc.cuh)."""
+    return max(1, -(-order // TAPS))
+
+
+# every width 1..13: orders 0, 1, both ends of each width and the largest order
+EDGES = sorted({0, 1, 100} | {o for w in range(1, 13) for o in (TAPS * w, TAPS * w + 1)})
 
 
 @pytest.fixture(scope="module")
@@ -29,21 +39,6 @@ def O():
 @pytest.fixture(scope="module")
 def P():
     return ol.load("port")
-
-
-def order_class(order):
-    return 0 if order <= 28 else 1 if order <= 56 else 2          # kernels.cuh order_class()
-
-
-def warps(orders):
-    """Subframe ids per warp of k_synthesise_quad, as k_decode_classify lays them out for a mono batch: a stable
-    counting sort by order class, widest class first, every class segment padded to a multiple of four
-    (None = an empty slot)."""
-    slots = []
-    for c in (2, 1, 0):
-        ids = [i for i, o in enumerate(orders) if order_class(o) == c]
-        slots += ids + [None] * (-len(ids) % 4)
-    return [slots[i:i + 4] for i in range(0, len(slots), 4)]
 
 
 def check_decode(O, P, subs, channels):
@@ -65,49 +60,45 @@ def content(P, rng, order, i, **kw):
     return CR.crafted_subframe(P, rng, order, "wide" if i % 2 else "small", **kw)
 
 
-# ------------------------------------------------------------------------------- order classes --
+# ------------------------------------------------------------------------------------- orders --
 
 def test_order_classes_alone_and_mixed(O, P):
+    """Every order of ORDERS four times, then groups of four orders of two segment widths each: the plan packs
+    segments of different widths into one warp, each stepping its own order up."""
     rng = np.random.default_rng(100)
-    orders = [o for o in ORDERS for _ in range(4)]                 # every order alone in a warp
+    orders = [o for o in ORDERS for _ in range(4)]
     mixed = [[0, 1, 2, 28], [27, 3, 28, 0], [29, 30, 55, 56], [56, 31, 29, 55], [57, 60, 99, 100], [100, 61, 57, 99]]
     for g in mixed:
+        assert len({width(o) for o in g}) == 2, g
         orders += g
-    # Each class count is a multiple of four here and k_decode_classify keeps file order inside a class, so
-    # every listed group of four lands in one warp of the batch kernel:
-    groups = [tuple(w) for w in warps(orders)]
-    base = 4 * len(ORDERS)
-    for j, g in enumerate(mixed):
-        assert tuple(range(base + 4 * j, base + 4 * j + 4)) in groups, g
     subs = [content(P, rng, o, i) for i, o in enumerate(orders)]
     check_decode(O, P, subs, 1)
 
 
-# -------------------------------------------------------------------------------- class layout --
+# ------------------------------------------------------------------------------- packing plan --
 
 def _mono(P, rng, orders):
     return [CR.crafted_subframe(P, rng, int(o), "small") for o in orders]
 
 
 def test_class_layout_ragged_segments_across_classify_tiles(O, P):
-    """>= 1100 subframes: classify runs two CTAs; every class count is 1, 2 or 3 mod 4, and class membership
-    changes across subframe 1024 (the first subframe of the second classify tile)."""
+    """>= 1100 subframes drawn from three order ranges: the packing plan runs two CTAs, width counts are ragged,
+    and the segment width changes across subframe 1024 (the first subframe of the plan's second CTA)."""
     rng = np.random.default_rng(101)
-    counts = {0: 401, 1: 350, 2: 351}                              # = 1, 2, 3 (mod 4)
+    counts = {0: 401, 1: 350, 2: 351}
     pool = {0: [0, 1, 2, 3, 17, 27, 28], 1: [29, 30, 31, 40, 55, 56], 2: [57, 60, 61, 80, 99, 100]}
     cls = np.concatenate([np.full(n, c) for c, n in counts.items()])
     rng.shuffle(cls)
     j = int(np.flatnonzero(cls != cls[1023])[0])
-    cls[[1024, j]] = cls[[j, 1024]]                                # subframes 1023 and 1024 in different classes
+    cls[[1024, j]] = cls[[j, 1024]]                                # subframes 1023 and 1024 from different ranges
     orders = [int(rng.choice(pool[int(c)])) for c in cls]
-    assert order_class(orders[1023]) != order_class(orders[1024])
-    assert sorted(np.bincount([order_class(o) for o in orders]) % 4) == [1, 2, 3]
+    assert width(orders[1023]) != width(orders[1024])
     check_decode(O, P, _mono(P, rng, orders), 1)
 
 
 @pytest.mark.parametrize("orders", [
-    [0, 5, 28, 17, 1, 2, 3, 28, 11],                               # all class 0
-    [1, 70, 100, 2, 28, 57, 99, 0, 61],                            # class 1 empty
+    [0, 5, 28, 17, 1, 2, 3, 28, 11],                               # all orders <= 28
+    [1, 70, 100, 2, 28, 57, 99, 0, 61],                            # none in 29..56
     [100], [29, 3], [57, 0, 56], [28, 29, 56, 57, 100],            # 1, 2, 3 and 5 subframes
 ], ids=["class0_only", "no_class1", "n1", "n2", "n3", "n5"])
 def test_class_layout_small_batches(O, P, orders):
@@ -116,9 +107,9 @@ def test_class_layout_small_batches(O, P, orders):
 
 # -------------------------------------------------------------------------------- sample range --
 
-def _range_batch(P, kind, seed):
+def _range_batch(P, kind, seed, orders=ORDERS):
     rng = np.random.default_rng(seed)
-    return [CR.crafted_subframe(P, rng, o, kind) for o in ORDERS]
+    return [CR.crafted_subframe(P, rng, o, kind) for o in orders]
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -131,8 +122,9 @@ def test_sample_range_decode(O, P, kind):
 
 @pytest.mark.parametrize("kind", KINDS)
 def test_sample_range_lpc_samples(O, P, kind):
-    """The same subframes through the stage-level entry point (k_lpc_samples: warp_iir_pair, classes 30 / 60)."""
-    subs = _range_batch(P, kind, 200 + KINDS.index(kind))
+    """The same subframes, then every segment width (EDGES), through the stage-level entry point (k_lpc_samples:
+    the decoder's segment recurrence, one subframe per warp)."""
+    subs = _range_batch(P, kind, 200 + KINDS.index(kind), ORDERS + EDGES)
     res = np.stack([s.res for s in subs])
     orders = np.array([s.order for s in subs], np.uint8)
     q = np.zeros((len(subs), 100), np.int32)
@@ -151,13 +143,13 @@ def test_sample_range_lpc_samples(O, P, kind):
 
 def _stereo(P, rng):
     """Difference subframe at position 0 and at position 1, with the channel fields in and out of position
-    order; parent and difference always in different order classes."""
+    order; parent and difference always of different segment widths."""
     subs = []
     layouts = [  # (position 0, position 1): (channel, type) -- parent channel is the other one
         ((0, 0), (1, 1)), ((0, 1), (1, 0)), ((1, 0), (0, 1)), ((1, 1), (0, 0)), ((1, 0), (0, 0)), ((0, 0), (1, 0))]
     pairs = [(2, 57), (100, 28), (29, 0), (56, 99), (1, 61), (30, 3)]
     for f, (lay, (op, od)) in enumerate(zip(layouts, pairs)):
-        assert order_class(op) != order_class(od)
+        assert width(op) != width(od)
         (c0, t0), (c1, t1) = lay
         par = content(P, rng, op, f, channel=c0 if t0 == 0 else c1)
         if t0 or t1:
@@ -177,7 +169,7 @@ def test_stereo_difference_positions_and_classes(O, P):
 def _frames(P, rng, ch, n_frames=2):
     """Frame 0: independent subframes, channel fields a random permutation of the positions.  Further frames
     (ch >= 2): difference subframes.  From 3 channels: two of them share one parent, which sits at a higher
-    channel index than its children; positions permuted as well."""
+    channel index than its children; positions permuted as well.  From 2 channels a last frame: _edge_frame."""
     subs = []
     for f in range(n_frames):
         chans = rng.permutation(ch)
@@ -197,7 +189,22 @@ def _frames(P, rng, ch, n_frames=2):
                 frame[pos_of[c]] = (CR.difference_subframe(P, rng, o, par, channel=c) if c in kids
                                     else content(P, rng, o, c, channel=c))
         subs += frame
+    if ch >= 2:
+        subs += _edge_frame(P, rng, ch)
     return subs
+
+
+def _edge_frame(P, rng, ch):
+    """Channel 0 is the difference to channel ch - 1, and both are within 2^8 of INT32_MIN at the same sample
+    positions: parent - difference is small there, though in int32 arithmetic the int16 output of the parent
+    minus the difference would overflow.  Other channels independent, positions permuted."""
+    par = CR.crafted_subframe(P, rng, int(rng.choice(ORDERS[2:])), "edge", channel=ch - 1)
+    kid = CR.difference_subframe(P, rng, int(rng.choice(ORDERS)), par, channel=0, kind="edge")
+    assert ((par.samples <= CR.I32_MIN + 255) & (kid.samples <= CR.I32_MIN + 255)).any()
+    by_channel = {0: kid, ch - 1: par}
+    for c in range(1, ch - 1):
+        by_channel[c] = content(P, rng, int(rng.choice(ORDERS)), c, channel=c)
+    return [by_channel[int(c)] for c in rng.permutation(ch)]
 
 
 @pytest.mark.parametrize("ch", range(1, 17))
@@ -210,8 +217,8 @@ def test_every_channel_count(O, P, ch):
 
 @pytest.mark.parametrize("ch", [2, 5])
 def test_chunked_decode(O, P, monkeypatch, ch):
-    """The pipelined host call cuts the batch into chunks of SELAB200_CHUNK_FRAMES frames: order classes and the
-    general kernel per chunk must give the same output."""
+    """The pipelined host call cuts the batch into chunks of SELAB200_CHUNK_FRAMES frames: the packing plan and
+    the difference fix-up per chunk must give the same output."""
     rng = np.random.default_rng(500 + ch)
     subs = _stereo(P, rng) if ch == 2 else _frames(P, rng, ch, n_frames=5)
     descs, words, want = check_decode(O, P, subs, ch)

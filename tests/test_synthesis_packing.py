@@ -9,10 +9,9 @@ import numpy as np
 import pytest
 
 import crafted as CR
-from test_synthesis import check_decode
+from test_synthesis import EDGES, check_decode, width
 
 pytestmark = pytest.mark.gpu
-TAPS = 8                                                            # kTapsPerLane (lpc.cuh)
 
 
 @pytest.fixture(scope="module")
@@ -25,14 +24,6 @@ def O():
 def P():
     import oracle_lib as ol
     return ol.load("port")
-
-
-def width(order):
-    return max(1, -(-order // TAPS))
-
-
-# every width 1..13: orders 0, 1, both ends of each width and the largest order
-EDGES = sorted({0, 1, 100} | {o for w in range(1, 13) for o in (TAPS * w, TAPS * w + 1)})
 
 
 def test_every_segment_width():
