@@ -77,7 +77,7 @@ typedef struct selab200_subframe_desc {
 int  selab200_init(int device);
 /* Several devices of one box (SURVEY.md 8b: selagpu_init(device_count, device_ids)): every device gets a
  * context of its own (streams, events, pools).  The host-buffer batch calls (selab200_encode_frames,
- * selab200_decode_frames, selab200_encode_container, selab200_container_decode and their verify forms) then cut the frames into one contiguous block per device
+ * selab200_decode_frames, selab200_encode_container, selab200_container_decode and their verify and lossless forms) then cut the frames into one contiguous block per device
  * -- n/D frames each, the last device takes the rest, the way sela::Encoder::processFrames cuts them for its
  * threads (src/sela/encoder.cpp:58-73) -- and run the blocks concurrently, reading and writing disjoint ranges
  * of the caller's buffers; results are byte-identical to a single device's.  devices[0] is the primary: it
@@ -269,6 +269,52 @@ int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, ui
 /* Instead of selab200_container_decode on an open container: compare its info.n_frames frames with pcm. */
 int selab200_container_verify(selab200_container *handle, const int16_t *pcm, selab200_verify_entry *entries,
                               size_t capacity, size_t *n_entries);
+
+/* ----------------------------------------------------------- lossless -- */
+
+/* Encodes that decode back to their source (DESIGN.md 7.2).  A subframe has a tie when, at some sample, the
+ * encoder's and the decoder's rounding of the prediction differ; it then does not decode back to its source.  The
+ * lossless forms find such subframes while encoding, and in every frame where the reference encoder would emit one,
+ * code each subframe candidate that has a tie with a slightly different predictor: one quantised reflection
+ * coefficient moved by 1, or a lower order, whichever tie-free choice costs the fewest words.  The output is an
+ * ordinary stream that the unmodified reference decoder reads; every other frame keeps the reference encoder's
+ * bytes.  The report holds one entry per emitted (frame, channel) that differs from the reference encoder's, in
+ * (frame, channel) order: the order and words (reflection + residue) of the reference's subframe and of the one
+ * emitted.  Frame indices are those of the whole batch / file. */
+typedef struct selab200_lossless_entry { /* 16 bytes */
+    uint32_t frame;
+    uint16_t channel;
+    uint8_t  ref_order;      /* the reference encoder's subframe                                */
+    uint8_t  order;          /* the emitted subframe                                            */
+    uint32_t ref_words;
+    uint32_t words;          /* 0 only in the device-resident per-pair array, where nothing changed */
+} selab200_lossless_entry;
+
+/* selab200_encode_frames, lossless.  *n_entries receives the number of re-coded subframes, of which the first
+ * `capacity` are written to entries.  Frames are split over devices as for the other batch calls. */
+int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                    selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                    size_t *words_used, selab200_lossless_entry *entries, size_t capacity,
+                                    size_t *n_entries);
+
+/* selab200_encode_container, lossless; report as selab200_encode_frames_lossless. */
+int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                       uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                       size_t capacity, size_t *bytes_used, selab200_lossless_entry *entries,
+                                       size_t entries_capacity, size_t *n_entries);
+
+/* Device-resident form of selab200_encode_frames_lossless: arguments as selab200_encode_frames_device, with
+ * selab200_encode_lossless_workspace_bytes() of workspace.  d_entries: n_frames*channels records, one per
+ * (frame, channel) in frame order, channel order; a re-coded pair's record is filled in, every other one is zeroed
+ * (words == 0).  *d_n_entries (uint64, device) receives the number of re-coded pairs.  Stream-ordered, no
+ * synchronisation: the repair runs on the device whatever it finds. */
+size_t selab200_encode_lossless_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                           selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                           size_t words_capacity, uint64_t *d_words_used,
+                                           selab200_lossless_entry *d_entries, uint64_t *d_n_entries,
+                                           int32_t *d_status, void *d_workspace, size_t workspace_bytes,
+                                           void *stream);
 
 /* ------------------------------------------ stage level (host buffers) -- */
 

@@ -45,6 +45,12 @@ VERIFY_DTYPE = np.dtype([
 ], align=True)
 assert VERIFY_DTYPE.itemsize == 16
 
+# mirrors selab200_lossless_entry, 16 bytes
+LOSSLESS_DTYPE = np.dtype([
+    ("frame", "<u4"), ("channel", "<u2"), ("ref_order", "u1"), ("order", "u1"), ("ref_words", "<u4"), ("words", "<u4"),
+], align=True)
+assert LOSSLESS_DTYPE.itemsize == 16
+
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
 
@@ -90,6 +96,10 @@ _SIGNATURES = {
     "selab200_verify_frames": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _SZ, _V]),
     "selab200_encode_container_verified": (_I, [_V, _U32, _U32, _U32, C.c_uint16, _V, _SZ, _V, _V, _SZ, _V]),
     "selab200_container_verify": (_I, [_V, _V, _V, _SZ, _V]),
+    "selab200_encode_lossless_workspace_bytes": (_SZ, [_U32, _U32]),
+    "selab200_encode_frames_lossless_device": (_I, [_V, _U32, _U32, _V, _V, _SZ, _V, _V, _V, _V, _V, _SZ, _V]),
+    "selab200_encode_frames_lossless": (_I, [_V, _U32, _U32, _V, _V, _SZ, _V, _V, _SZ, _V]),
+    "selab200_encode_container_lossless": (_I, [_V, _U32, _U32, _U32, C.c_uint16, _V, _SZ, _V, _V, _SZ, _V]),
     "selab200_lpc_residues": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_lpc_samples": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_rice_encode": (_I, [_V, _V, _U32, _U32, _V, _V, _V, _U32]),

@@ -15,6 +15,9 @@ error behaviour as in include/sela_b200.h):
                                     not in the reference: decode coded frames and compare them with
                                     their source PCM, reporting every (frame, channel) that differs
                                     (the format is not lossless for every input, DESIGN.md 7)
+    encode_frames_lossless / encode_container_lossless
+                                    not in the reference: encodes that decode back to their source, re-coding
+                                    the few subframes the reference decoder would not reproduce (DESIGN.md 7.2)
     encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
     / fir_probe                     order threshold and quantiser on chosen values, and its FIR residual
                                     on chosen signals and predictors
@@ -28,7 +31,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, MAX_ORDER, TRACE_DTYPE, VERIFY_DTYPE, SelaB200Error,  # noqa: F401
+from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, LOSSLESS_DTYPE, MAX_ORDER, TRACE_DTYPE, VERIFY_DTYPE, SelaB200Error,  # noqa: F401
                    check, init, lib)
 
 
@@ -291,3 +294,36 @@ def verify_container(container, pcm, device=0):
     finally:
         L.selab200_container_close(handle)
     return {k: int(info[0][k]) for k in INFO_DTYPE.names if k != "reserved"}, report[:n.value].copy()
+
+
+def encode_frames_lossless(pcm, channels, words_capacity=None, device=0):
+    """encode_frames, lossless -> (descs, words, report).  report: LOSSLESS_DTYPE array, one entry per re-coded
+    (frame, channel) in that order: the reference encoder's order and words there, and the emitted ones."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used = C.c_size_t(0)
+    report = np.zeros(max(n_frames * channels, 1), LOSSLESS_DTYPE)
+    n = C.c_size_t(0)
+    check(L.selab200_encode_frames_lossless(pcm.ctypes.data, n_frames, channels, descs.ctypes.data, words.ctypes.data,
+                                            cap, C.addressof(used), report.ctypes.data, report.size, C.addressof(n)))
+    return descs, words[:used.value].copy(), report[:n.value].copy()
+
+
+def encode_container_lossless(pcm, channels, sample_rate, bits_per_sample=16, capacity=None, device=0):
+    """encode_container, lossless -> (bytes, report), the report as encode_frames_lossless returns it."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used = C.c_size_t(0)
+    report = np.zeros(max(n_frames * channels, 1), LOSSLESS_DTYPE)
+    n = C.c_size_t(0)
+    check(L.selab200_encode_container_lossless(pcm.ctypes.data, n_frames, channels, sample_rate, bits_per_sample,
+                                               out.ctypes.data, cap, C.addressof(used), report.ctypes.data,
+                                               report.size, C.addressof(n)))
+    return out[:used.value], report[:n.value].copy()

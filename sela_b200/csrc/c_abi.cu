@@ -13,6 +13,7 @@
 #include <thread>
 #include <vector>
 
+#include "lossless.cuh"
 #include "verify.cuh"
 
 using namespace selab200;
@@ -80,6 +81,7 @@ struct Context {
     bool events = false;
     DeviceBuffer in, descs, words, work, lane_work[kLanes], aux, small;
     DeviceBuffer verify;                           // verify paths: count, status, per-pair records (VerifyArea)
+    DeviceBuffer lossless;                         // lossless host paths: count, per-pair records of re-coded subframes
     int32_t *h_small = nullptr;                    // pinned: [0] status, [2..3] words_used, [12..14] verify count + status
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
@@ -295,16 +297,51 @@ int launch_unit_means(const void *src, size_t n_units, uint32_t channels, double
     return launch_check("k_unit_means");
 }
 
-// k_encode_units<STEREO, TRACE>, a warp per analysis unit.
-template <bool STEREO, bool TRACE>
+// k_encode_units<STEREO, TRACE, CHECK>, a warp per analysis unit.
+template <bool STEREO, bool TRACE, bool CHECK = false>
 int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis_trace *d_trace, cudaStream_t stream)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_encode_units<STEREO, TRACE>, smem))
+    if (int rc = set_smem(k_encode_units<STEREO, TRACE, CHECK>, smem))
         return rc;
-    k_encode_units<STEREO, TRACE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace);
+    k_encode_units<STEREO, TRACE, CHECK><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace);
     return launch_check("k_encode_units");
 }
+
+// The lossless repair between k_encode_units<S, false, true> and the scan (lossless.cuh).  Every launch has a grid
+// of a fixed size: nothing here depends on what the check found.  The warp kernels use at most one residue row
+// per unit of the batch.
+template <bool STEREO>
+int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream)
+{
+    constexpr size_t smem = encode_smem_bytes<STEREO>();
+    if (int rc = set_smem(k_lossless_candidates<STEREO>, smem))
+        return rc;
+    if (int rc = set_smem(k_lossless_repack<STEREO>, smem))
+        return rc;
+    k_lossless_select<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, r);
+    if (int rc = launch_check("k_lossless_select"))
+        return rc;
+    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
+    for (int round = 0; round < 2; round++) {
+        k_lossless_candidates<STEREO><<<warps, 32, smem, stream>>>(p, r, round);
+        if (int rc = launch_check("k_lossless_candidates"))
+            return rc;
+    }
+    k_lossless_repack<STEREO><<<warps, 32, smem, stream>>>(p, r);
+    if (int rc = launch_check("k_lossless_repack"))
+        return rc;
+    k_lossless_report<<<(unsigned)std::min((n_frames + 255) / 256, (size_t)g.sms), 256, 0, stream>>>(p, r);
+    return launch_check("k_lossless_report");
+}
+
+// Where a lossless encode reports its re-coded subframes: the batch's per-pair records, their count, and the frame
+// number of the batch's first frame.
+struct LosslessArgs {
+    selab200_lossless_entry *entries;
+    unsigned long long *n_entries;
+    uint32_t frame_base;
+};
 
 // ---- device-resident cores (no synchronisation) --------------------------
 
@@ -316,11 +353,12 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
                   size_t ws_bytes, cudaStream_t stream, bool fresh = true, cudaEvent_t before_scan = nullptr,
                   cudaEvent_t after_scan = nullptr, unsigned long long *h_fill_after = nullptr,
                   uint8_t *d_container = nullptr, unsigned long long sub_base = 0,
-                  selab200_analysis_trace *d_trace = nullptr)
+                  selab200_analysis_trace *d_trace = nullptr, const LosslessArgs *lossless = nullptr)
 {
     if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
         return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    if (ws_bytes < selab200_encode_workspace_bytes(n_frames, channels))
+    if (ws_bytes < (lossless ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
+                             : selab200_encode_workspace_bytes(n_frames, channels)))
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
         return fail(SELAB200_ERR_ARGUMENT, "stereo PCM must be 16-byte aligned on the device");
@@ -349,12 +387,31 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
                         : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
         return rc;
-    const int rc_units = stereo ? (d_trace ? launch_encode_units<true, true>(p, n_units, d_trace, stream)
-                                           : launch_encode_units<true, false>(p, n_units, nullptr, stream))
-                                : (d_trace ? launch_encode_units<false, true>(p, n_units, d_trace, stream)
-                                           : launch_encode_units<false, false>(p, n_units, nullptr, stream));
-    if (rc_units)
-        return rc_units;
+    if (lossless) {
+        RepairParams r;
+        char *b = static_cast<char *>(d_ws) + align256(selab200_encode_workspace_bytes(n_frames, channels));
+        r.count = reinterpret_cast<uint32_t *>(b);
+        r.frames = reinterpret_cast<uint32_t *>(b + 256);
+        r.orig = reinterpret_cast<UnitRecord *>(b + 256 + align256((size_t)n_frames * 4));
+        r.units = reinterpret_cast<RepairUnit *>(reinterpret_cast<char *>(r.orig) + align256(n_units * sizeof(UnitRecord)));
+        r.entries = lossless->entries;
+        r.n_entries = lossless->n_entries;
+        r.frame_base = lossless->frame_base;
+        CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
+        if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
+                            : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
+            return rc;
+        if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream)
+                            : launch_repair<false>(p, r, n_frames, n_units, stream))
+            return rc;
+    } else {
+        const int rc_units = stereo ? (d_trace ? launch_encode_units<true, true>(p, n_units, d_trace, stream)
+                                               : launch_encode_units<true, false>(p, n_units, nullptr, stream))
+                                    : (d_trace ? launch_encode_units<false, true>(p, n_units, d_trace, stream)
+                                               : launch_encode_units<false, false>(p, n_units, nullptr, stream));
+        if (rc_units)
+            return rc_units;
+    }
     const unsigned scan_ctas = (unsigned)((n_sub + kScanTile - 1) / kScanTile);
     k_encode_sizes<<<scan_ctas, kScanTile, 0, stream>>>(p);
     if (int rc = launch_check("k_encode_sizes"))
@@ -678,6 +735,7 @@ static void shutdown_slot()
         g.lane_work[i].release();
     g.aux.release();
     g.verify.release();
+    g.lossless.release();
     g.small.release();
     if (g.h_small)
         cudaFreeHost(g.h_small);
@@ -808,6 +866,11 @@ size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels)
            align256(n_units * sizeof(double)) + n_units * (size_t)kFrame * 4 + 256;
 }
 
+size_t selab200_encode_lossless_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    return align256(selab200_encode_workspace_bytes(n_frames, channels)) + repair_lists_bytes(n_frames, channels);
+}
+
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_sub = (size_t)n_frames * channels;
@@ -833,6 +896,28 @@ int selab200_encode_frames_device(const int16_t *d_pcm, uint32_t n_frames, uint3
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                           selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
+                                           uint64_t *d_words_used, selab200_lossless_entry *d_entries,
+                                           uint64_t *d_n_entries, int32_t *d_status, void *d_workspace,
+                                           size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_entries || !d_n_entries || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    const cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(cudaMemsetAsync(d_n_entries, 0, sizeof(uint64_t), st));
+    if (n_frames)
+        CUDA_TRY(cudaMemsetAsync(d_entries, 0, (size_t)n_frames * channels * sizeof(selab200_lossless_entry), st));
+    const LosslessArgs la{d_entries, reinterpret_cast<unsigned long long *>(d_n_entries), 0};
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, st, true, nullptr, nullptr, nullptr, nullptr, 0, nullptr, &la);
 }
 
 int selab200_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
@@ -933,6 +1018,7 @@ int selab200_rice_decode_flagged(uint32_t *n_flagged)
 } // extern "C"
 
 static_assert(sizeof(selab200_analysis_trace) == 2832, "selab200_analysis_trace layout (include/sela_b200.h)");
+static_assert(sizeof(selab200_lossless_entry) == 16, "selab200_lossless_entry layout (include/sela_b200.h)");
 
 // Bytes of container in front of frame f when `words` Rice words precede it.
 static unsigned long long container_frame_byte(unsigned long long f, uint32_t channels, unsigned long long words)
@@ -948,14 +1034,17 @@ static unsigned long long container_frame_byte(unsigned long long f, uint32_t ch
 // With `defer`, `container` is only a flag (any non-null value selects the byte-packed form).
 // `report` (container form only): also verify the container image, chunk by chunk on the device, and return
 // the differing (frame, channel) pairs, frames numbered from frame_base.
+// `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs, numbered likewise.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
                        uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
                        bool defer = false, std::vector<selab200_verify_entry> *report = nullptr,
-                       uint32_t frame_base = 0)
+                       uint32_t frame_base = 0, std::vector<selab200_lossless_entry> *recoded = nullptr)
 {
     *words_used = 0;
     if (report)
         report->clear();
+    if (recoded)
+        recoded->clear();
     if (n_frames == 0)
         return 0;
     PipelineDrain drain;
@@ -964,10 +1053,17 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
     const bool verify = report && container;
-    const size_t ws_bytes = selab200_encode_workspace_bytes(plan.max_frames, channels);
+    const size_t ws_bytes = recoded ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
+                                    : selab200_encode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(container_frame_byte(n_frames, channels, words_capacity) + 64)) return rc;
+    // lossless: the count of re-coded pairs, then the per-pair records of the whole batch
+    if (recoded)
+        if (int rc = g.lossless.ensure(256 + n_sub * sizeof(selab200_lossless_entry))) return rc;
+    unsigned long long *d_recoded = static_cast<unsigned long long *>(g.lossless.ptr);
+    selab200_lossless_entry *d_rec_entries =
+        recoded ? reinterpret_cast<selab200_lossless_entry *>(static_cast<char *>(g.lossless.ptr) + 256) : nullptr;
     constexpr int kEncLanes = 2;
     for (int i = 0; i < kEncLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
@@ -988,11 +1084,14 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         if (int rc = verify_area(n_sub, arena_words, g.s_compute[0], va)) return rc;
 
     CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
+    if (recoded)
+        CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, 256 + n_sub * sizeof(selab200_lossless_entry), g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
     for (int i = 1; i < kLanes; i++)
         CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
     for (uint32_t c = 0; c < n_chunks; c++) {
         const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
+        const LosslessArgs la{d_rec_entries + (size_t)f0 * channels, d_recoded, frame_base + f0};
         CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)f0 * channels * kFrame,
                                  nf * frame_bytes, cudaMemcpyHostToDevice, g.s_h2d));
         CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
@@ -1003,7 +1102,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                    d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, false,
                                    c ? g.ev_scan[c - 1] : nullptr, g.ev_scan[c], &g.h_totals[c + 1],
                                    container ? static_cast<uint8_t *>(g.words.ptr) : nullptr,
-                                   (unsigned long long)f0 * channels))
+                                   (unsigned long long)f0 * channels, nullptr, recoded ? &la : nullptr))
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
         if (verify) {
@@ -1065,6 +1164,17 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     *words_used = (size_t)used; // for CAPACITY: the size the caller needs
     if (g.h_small[0] != 0)
         return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (recoded) { // the per-pair records come down only when there are any
+        unsigned long long n = 0;
+        CUDA_TRY(cudaMemcpy(&n, d_recoded, 8, cudaMemcpyDeviceToHost));
+        if (n) {
+            std::vector<selab200_lossless_entry> all(n_sub);
+            CUDA_TRY(cudaMemcpy(all.data(), d_rec_entries, n_sub * sizeof(selab200_lossless_entry), cudaMemcpyDeviceToHost));
+            for (const selab200_lossless_entry &e : all)
+                if (e.words)
+                    recoded->push_back(e);
+        }
+    }
     return verify ? collect_report(va, n_sub, g.s_d2h, *report) : 0;
 }
 
@@ -1207,6 +1317,7 @@ struct DevicePart {
     size_t used = 0;
     char err[sizeof g_error] = "";
     std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
+    std::vector<selab200_lossless_entry> recoded; // lossless calls: this block's re-coded pairs, file-global frames
 };
 
 // The blocks' reports one after the other: blocks are contiguous and in frame order, so this is in order too.
@@ -1262,17 +1373,23 @@ static int run_on_devices(std::vector<DevicePart> &parts, F work)
 
 static int encode_all_devices(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
                               uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
-                              std::vector<selab200_verify_entry> *report = nullptr)
+                              std::vector<selab200_verify_entry> *report = nullptr,
+                              std::vector<selab200_lossless_entry> *recoded = nullptr)
 {
     std::vector<DevicePart> parts = device_parts(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
     const int rc = run_on_devices(parts, [&](DevicePart &p) {
         return encode_host(pcm + p.f0 * per_frame, p.nf, channels, descs ? descs + (size_t)p.f0 * channels : nullptr, nullptr,
                            selab200_encode_words_bound(p.nf, channels), &p.used, container, true,
-                           report ? &p.report : nullptr, p.f0);
+                           report ? &p.report : nullptr, p.f0, recoded ? &p.recoded : nullptr);
     });
     if (report)
         *report = joined_reports(parts);
+    if (recoded) {
+        recoded->clear();
+        for (const DevicePart &p : parts)
+            recoded->insert(recoded->end(), p.recoded.begin(), p.recoded.end());
+    }
     size_t total = 0;
     for (const DevicePart &p : parts)
         total += p.used;
@@ -1363,6 +1480,44 @@ int selab200_encode_frames(const int16_t *pcm, uint32_t n_frames, uint32_t chann
     return encode_host(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr);
 }
 
+} // extern "C"
+
+// The report of a lossless host-buffer call: *n_entries = all of it, at most `capacity` entries written.
+static void deliver_recoded(const std::vector<selab200_lossless_entry> &rec, selab200_lossless_entry *entries,
+                            size_t capacity, size_t *n_entries)
+{
+    *n_entries = rec.size();
+    if (capacity && !rec.empty())
+        memcpy(entries, rec.data(), std::min(capacity, rec.size()) * sizeof(selab200_lossless_entry));
+}
+
+extern "C" {
+
+int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                    selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                    size_t *words_used, selab200_lossless_entry *entries, size_t capacity,
+                                    size_t *n_entries)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || (!entries && capacity) || !n_entries)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    *n_entries = 0;
+    std::vector<selab200_lossless_entry> rec;
+    const int rc = use_all_devices(n_frames)
+                       ? encode_all_devices(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr,
+                                            nullptr, &rec)
+                       : encode_host(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr, false,
+                                     nullptr, 0, &rec);
+    if (rc)
+        return rc;
+    deliver_recoded(rec, entries, capacity, n_entries);
+    return 0;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -1373,7 +1528,8 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 // selab200_encode_container, and with `report` its verified form (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
-                                 std::vector<selab200_verify_entry> *report)
+                                 std::vector<selab200_verify_entry> *report,
+                                 std::vector<selab200_lossless_entry> *recoded = nullptr)
 {
     if (int rc = require_ready())
         return rc;
@@ -1394,9 +1550,9 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     size_t words_used = 0;
     const int rc = use_all_devices(n_frames)
                        ? encode_all_devices(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
-                                            container, report)
+                                            container, report, recoded)
                        : encode_host(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
-                                     container, false, report);
+                                     container, false, report, 0, recoded);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
     return rc;
 }
@@ -1427,6 +1583,25 @@ int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, ui
                                        bytes_used, &report))
         return rc;
     return deliver_report(report, entries, entries_capacity, n_entries);
+}
+
+int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                                       uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
+                                       selab200_lossless_entry *entries, size_t entries_capacity, size_t *n_entries)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!n_entries || (!entries && entries_capacity)) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    *n_entries = 0;
+    std::vector<selab200_lossless_entry> rec;
+    if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                       bytes_used, nullptr, &rec))
+        return rc;
+    deliver_recoded(rec, entries, entries_capacity, n_entries);
+    return 0;
 }
 
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,

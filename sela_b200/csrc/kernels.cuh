@@ -1,7 +1,8 @@
 // kernels.cuh -- the __global__ kernels of the SELA hot path (sm_90a).
 //
 //   encode   k_unit_means<KIND> (lane per analysis unit: the mean of its samples)
-//            k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot)
+//            k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot; its
+//            CHECK instantiation also flags ties, and lossless.cuh re-codes flagged units through encode_unit)
 //            k_encode_sizes + k_encode_scan (stereo decision, prefix sum, descriptors)
 //            k_encode_gather / k_encode_gather_container (slot -> word arena / .sela byte stream)
 //   decode   k_container_unpack (.sela bytes -> word arena)
@@ -182,12 +183,66 @@ __host__ __device__ inline uint32_t encode_units(uint32_t n_frames, uint32_t cha
     return channels == 2 ? n_frames * 3u : n_frames * channels;
 }
 
-// TRACE (tests only, selab200_encode_trace): the same kernel, which also copies each unit's analysis
-// intermediates to trace[unit] as they are produced.  Production runs TRACE = false, where none of it exists and
-// `trace` is null.  `trace` is a kernel argument of its own rather than a field of EncodeParams: a longer
-// EncodeParams would move the parameter offsets of the kernels that take arguments after it.
-template <bool STEREO, bool TRACE = false>
-__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_analysis_trace *trace)
+// ---- lossless repair (DESIGN.md 7.2) ----
+// A unit whose FIR has a tie does not decode back to its source.  The repair codes it with a slightly different
+// predictor, chosen from the candidates of a unit of order o >= 2 with quantised coefficients q[0..o):
+//   round 1: q[j] - 1, q[j] + 1 for j = 0, 1, o-1 (increasing j, each once), then order o-1;
+//   round 2: q[j] - 1, q[j] + 1 for every other j (2 .. o-2), then orders o-2, o-3, .. 1.
+// An edit that leaves [-64, 63] is no candidate.  Order 1 has no tie (c[1] = 0), so round 2 always has one.  The
+// winner is the tie-free candidate of the first round that has any with the fewest words, ties to the earlier
+// candidate.  Candidates are numbered 0 .. 3o-2 in this order, round 1 first.
+struct PredictorEdit {
+    int order, j, delta; // code at `order`; q[j] += delta where delta != 0
+};
+__host__ __device__ inline int repair_round1(int o) { return o == 2 ? 5 : 7; }
+__host__ __device__ inline int repair_candidates(int o) { return o < 2 ? 0 : 3 * o - 1; }
+constexpr int kRepairRound2Max = 3 * kMaxOrder - 1 - 7;
+__host__ __device__ inline PredictorEdit repair_edit(int o, int c)
+{
+    PredictorEdit e{o, 0, 0};
+    const int n1 = repair_round1(o);
+    if (c < n1) {
+        if (c == n1 - 1) {
+            e.order = o - 1;
+        } else {
+            e.j = (c >> 1) < 2 ? (c >> 1) : o - 1;
+            e.delta = (c & 1) ? 1 : -1;
+        }
+        return e;
+    }
+    c -= n1;
+    const int n_edits = o > 3 ? 2 * (o - 3) : 0;
+    if (c < n_edits) {
+        e.j = 2 + (c >> 1);
+        e.delta = (c & 1) ? 1 : -1;
+    } else {
+        e.order = o - 2 - (c - n_edits);
+    }
+    return e;
+}
+
+// A unit being repaired: its index in the batch, its order as analysed, and the best candidate so far as the key
+// round << 63 | words << 32 | candidate (all ones: none yet), so that one atomicMin keeps the winner.
+struct RepairUnit {
+    uint32_t unit, order;
+    unsigned long long best;
+};
+constexpr unsigned long long kNoCandidate = ~0ull;
+
+// What encode_unit does with the unit:
+//   kUnitEncode     analyse, FIR, Rice, pack into the unit's slot and write its record (production)
+//   kUnitCheck      kUnitEncode, and bit 1 of the record's flags when the FIR has a tie
+//   kUnitCandidate  analyse, apply candidate `cand`, FIR with the tie check, Rice sizes: a tie-free candidate enters
+//                   ru->best; nothing is packed
+//   kUnitRepack     analyse, apply candidate `cand`, FIR, Rice, pack into the unit's slot and rewrite its record
+enum { kUnitEncode = 0, kUnitCheck = 1, kUnitCandidate = 2, kUnitRepack = 3 };
+
+// The work of one analysis unit by one warp.
+// TRACE (tests only, selab200_encode_trace): also copies the unit's analysis intermediates to trace[unit] as they
+// are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.
+template <bool STEREO, bool TRACE, int MODE>
+__device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_analysis_trace *trace, const uint32_t unit,
+                                            RepairUnit *ru, uint32_t cand)
 {
     constexpr int kRow = kHistoryPad + kFrame;
     constexpr int kLoWords = (kHistoryPad + kFrame) / 32; // parity bits of a difference signal
@@ -203,7 +258,6 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
     CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kCoefAlias);
 
     const int lane = lane_id();
-    const uint32_t unit = blockIdx.x;
     const uint32_t frame = STEREO ? unit / 3 : unit / p.channels;
     const uint32_t role = STEREO ? unit % 3 : unit % p.channels; // stereo: 0 ch0, 1 ch1, 2 ch0-ch1
 
@@ -255,7 +309,8 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
     __syncwarp();
 
     // ---- analysis ----
-    int32_t *res = p.residues + (size_t)unit * kFrame;
+    // the residue row: the unit's own, or in the repair (which runs several candidates of a unit at once) the warp's
+    int32_t *res = p.residues + (size_t)(MODE == kUnitEncode || MODE == kUnitCheck ? unit : blockIdx.x) * kFrame;
     // one lane loads the mean and the warp gets it by shuffle: a warp-wide load of p.means[unit] moves the unit
     // index out of the uniform registers, and the stereo kernel then needs 78 registers instead of 72
     warp_autocorrelation(sig, scratch, shfl_d(lane == 0 ? p.means[unit] : 0.0, 0));
@@ -267,7 +322,23 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
             tr.ac[i] = scratch.ac[i];
     }
     warp_schur(scratch);
-    const int order = warp_order_and_quantise(scratch, cf);
+    int order = warp_order_and_quantise(scratch, cf);
+    if constexpr (MODE == kUnitCandidate || MODE == kUnitRepack) {
+        const PredictorEdit e = repair_edit(order, (int)cand);
+        if (e.delta) {
+            const int v = cf.q[e.j] + e.delta;
+            if (v < -64 || v > 63)
+                return; // no candidate (the whole warp)
+            __syncwarp();
+            if (lane == 0)
+                cf.q[e.j] = v;
+        } else {
+            for (int i = e.order + lane; i < order; i += 32)
+                cf.q[i] = 0;
+        }
+        __syncwarp();
+        order = e.order;
+    }
     warp_coefficients(cf, scratch.t(), order);
     if constexpr (TRACE) { // k[] (ring[0, 100)) is still intact: t[] and the predictor lie behind it
         selab200_analysis_trace &tr = trace[unit];
@@ -283,14 +354,25 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
     // the digit planes of the FIR overlay k[] and the step-up row, dead now (the trace has copied k)
     static_assert(kPlaneBytes <= kCoefAlias, "FIR digit planes");
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
+    constexpr bool kCheck = MODE == kUnitCheck || MODE == kUnitCandidate;
+    bool tie;
     if (STEREO && role == 2)
-        warp_fir_residual<true>(sig, cf, order, planes, res);
+        tie = warp_fir_residual<true, kCheck>(sig, cf, order, planes, res);
     else
-        warp_fir_residual<false>(sig, cf, order, planes, res);
+        tie = warp_fir_residual<false, kCheck>(sig, cf, order, planes, res);
 
     // ---- Rice: parameter search, then pack into this unit's slot ----
     const RiceChoice cq = warp_rice_choose(cf.q, order);
     const RiceChoice cr = warp_rice_choose(res, kFrame);
+    if constexpr (MODE == kUnitCandidate) {
+        __syncwarp();
+        for (int l = lane; l < kFrame * 4 / 128; l += 32)
+            asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
+        const unsigned long long round = cand >= (uint32_t)repair_round1(ru->order) ? 1ull : 0ull;
+        if (lane == 0 && !tie)
+            atomicMin(&ru->best, round << 63 | (unsigned long long)(cq.words + cr.words) << 32 | cand);
+        return;
+    }
     const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
     uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
     if (!too_large) {
@@ -310,10 +392,19 @@ __global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_an
         u.refl_words = cq.words;
         u.res_k = cr.k;
         u.res_words = cr.words;
-        u.flags = too_large ? 1u : 0u;
+        u.flags = (too_large ? 1u : 0u) | (tie ? 2u : 0u); // 2: not lossless (kUnitCheck only)
         u.pad[0] = u.pad[1] = 0;
         p.units[unit] = u;
     }
+}
+
+// k_encode_units: encode_unit for unit blockIdx.x.  CHECK: the kUnitCheck instantiation (lossless encodes).
+// `trace` is a kernel argument of its own rather than a field of EncodeParams: a longer EncodeParams would move
+// the parameter offsets of the kernels that take arguments after it.
+template <bool STEREO, bool TRACE = false, bool CHECK = false>
+__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_analysis_trace *trace)
+{
+    encode_unit<STEREO, TRACE, CHECK ? kUnitCheck : kUnitEncode>(p, trace, blockIdx.x, nullptr, 0);
 }
 
 template <bool STEREO>

@@ -407,9 +407,13 @@ __device__ __forceinline__ unsigned long long mad_wide_s32(int32_t a, int32_t b,
 }
 
 // WIDE: sig is a 17-bit signal (sig.lo != nullptr).  planes: 1088 bytes of scratch (see warp_fir_planes).
-template <bool WIDE>
-__device__ void warp_fir_residual(const Signal &sig, const CoefSmem &cf, int order, uint32_t *planes, int32_t *res)
+// CHECK: also return, to every lane, whether some output is a tie -- a prediction the decoder rounds differently,
+// (int32)((2^34 + P) >> 35) + (int32)((2^34 - P) >> 35) != 0 with 2^34 - P = 2^35 - sum mod 2^64 (DESIGN.md 7.2).
+// The unit then does not decode back to its source under the reference decoder; without one it does.
+template <bool WIDE, bool CHECK = false>
+__device__ bool warp_fir_residual(const Signal &sig, const CoefSmem &cf, int order, uint32_t *planes, int32_t *res)
 {
+    bool tie = false;
     constexpr int NL = WIDE ? 3 : 2; // sample limbs: u8, (u8,) s8
     const int lane = lane_id();
     const int g = lane >> 2, t = lane & 3;
@@ -486,11 +490,16 @@ __device__ void warp_fir_residual(const Signal &sig, const CoefSmem &cf, int ord
                                      ((uint32_t)T[7][r] << 24); // weights 2^32 .. 2^56: only the high word
                 sum += (unsigned long long)top << 32;
                 out[e] = s[e] - (int32_t)((long long)sum >> kQ);
+                if constexpr (CHECK)
+                    tie |= (int32_t)((long long)sum >> kQ) + (int32_t)((long long)((1ull << kQ) - sum) >> kQ) != 0;
             }
             *reinterpret_cast<int2 *>(res + i) = make_int2(out[0], out[1]);
         }
     }
     __syncwarp();
+    if constexpr (CHECK)
+        return __any_sync(kFull, tie);
+    return false;
 }
 
 // ---------------------------------------------------------------------------

@@ -40,6 +40,33 @@ class DeviceCodec:
             self.capacity, self.words_used.data_ptr(), self.status.data_ptr(), self.enc_ws.data_ptr(),
             self.enc_ws_bytes, C.c_void_p(stream)))
 
+    def encode_lossless(self, pcm):
+        """encode, lossless (DESIGN.md 7.2): also fills the per-pair records of re-coded subframes on the device.
+        Asynchronous, and the host never waits for what the check finds; lossless_report() collects the report.
+        The lossless buffers are allocated on first use."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.numel() == self.n_sub * FRAME
+        L = lib()
+        if not hasattr(self, "ll_ws"):
+            self.ll_ws_bytes = L.selab200_encode_lossless_workspace_bytes(self.n_frames, self.channels)
+            self.ll_ws = torch.zeros(self.ll_ws_bytes, dtype=torch.uint8, device=self.device)
+            self.ll_entries = torch.zeros(max(self.n_sub, 1) * 16, dtype=torch.uint8, device=self.device)
+            self.ll_count = torch.zeros(1, dtype=torch.int64, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_encode_frames_lossless_device(
+            pcm.data_ptr(), self.n_frames, self.channels, self.descs.data_ptr(), self.words.data_ptr(),
+            self.capacity, self.words_used.data_ptr(), self.ll_entries.data_ptr(), self.ll_count.data_ptr(),
+            self.status.data_ptr(), self.ll_ws.data_ptr(), self.ll_ws_bytes, C.c_void_p(stream)))
+
+    def lossless_report(self):
+        """Synchronises: the report of the last encode_lossless, a LOSSLESS_DTYPE array of the re-coded
+        (frame, channel) pairs in order."""
+        import numpy as np
+        from ._lib import LOSSLESS_DTYPE
+        if int(self.ll_count.item()) == 0:
+            return np.zeros(0, LOSSLESS_DTYPE)
+        rec = self.ll_entries.cpu().numpy().view(LOSSLESS_DTYPE)[:self.n_sub]
+        return rec[rec["words"] != 0].copy()
+
     def decode(self, pcm_out, n_words):
         """Decode self.descs / self.words[:n_words] into pcm_out (int16 cuda tensor). Asynchronous."""
         assert pcm_out.dtype == torch.int16 and pcm_out.is_cuda and pcm_out.numel() == self.n_sub * FRAME

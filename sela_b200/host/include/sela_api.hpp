@@ -110,10 +110,19 @@ struct VerifyEntry {
     int32_t firstDelta;        // decoded - source at firstSample
 };
 
+// Not in the reference: one subframe a lossless encode emits in place of the reference encoder's
+// (selab200_lossless_entry): that subframe's order and words (reflection + residue), and the emitted one's.
+struct RecodedEntry {
+    uint32_t frame;
+    uint16_t channel;
+    uint8_t refOrder, order;
+    uint32_t refWords, words;
+};
+
 class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
-    void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report);
+    void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -128,6 +137,10 @@ public:
     // on the device and compared with the WAV's whole frames.  Same bytes as processTo(); `report` receives
     // every (frame, channel) that does not decode back to its source, in order (empty: lossless).
     void processTo(std::ofstream &outputFile, std::vector<VerifyEntry> &report);
+    // Not in the reference: processTo() writing a file that decodes back to its source under the unmodified
+    // reference decoder (selab200_encode_container_lossless).  Frames without a tie keep processTo()'s bytes;
+    // `recoded` receives every (frame, channel) coded differently, in order.
+    void processLosslessTo(std::ofstream &outputFile, std::vector<RecodedEntry> &recoded);
 };
 class Decoder {
     void readFrames();

@@ -5,6 +5,8 @@
 // Not in the reference: `-V in.wav out.sela` (encode, then prove the written bytes decode back to the WAV)
 // and `-t in.sela in.wav` (test a coded file against a WAV).  Exit status 0 when every frame decodes to its
 // source, 2 when some do not (one stderr line per (frame, channel), then a summary), 1 on errors.
+// `-L in.wav out.sela`: a lossless encode (a file that decodes back to the WAV under the reference decoder, the same
+// bytes as -e where -e's already do), one line with the number of re-coded subframes.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -94,6 +96,8 @@ int usage(const std::string &prog)
               << "Playing a file:\n" << prog << " -p path/to/input.sela\n\n"
               << "Encoding a file and verifying that it decodes back to the input (H100 build):\n" << prog
               << " -V path/to/input.wav path/to/output.sela\n\n"
+              << "Encoding a file so that it decodes back to the input (H100 build):\n" << prog
+              << " -L path/to/input.wav path/to/output.sela\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -153,6 +157,13 @@ int main(int argc, char **argv)
             std::vector<sela::VerifyEntry> report;
             sela::Encoder(in).processTo(out, report);
             status = print_report(report);
+        } else if (mode == "-L" && argc == 4) {
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Encoding losslessly: " << argv[2] << std::endl;
+            std::vector<sela::RecodedEntry> recoded;
+            sela::Encoder(in).processLosslessTo(out, recoded);
+            std::cout << "Re-coded " << recoded.size() << " subframes" << std::endl;
         } else if (mode == "-t" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ifstream wav(argv[3], std::ios::binary);

@@ -787,15 +787,23 @@ static std::vector<VerifyEntry> mirror_report(const std::vector<selab200_verify_
 // process() + file::SelaFile::writeToFile() without the detour through per-frame value structs:
 // the data chunk is handed to the device where it lies in the file buffer, and what comes back is
 // the .sela byte stream.  Output is byte-identical to the two-step path (tests/test_host_cli.py).
-void Encoder::processTo(std::ofstream &outputFile) { encodeTo(outputFile, nullptr); }
+void Encoder::processTo(std::ofstream &outputFile) { encodeTo(outputFile, nullptr, nullptr); }
 
-void Encoder::processTo(std::ofstream &outputFile, std::vector<VerifyEntry> &report) { encodeTo(outputFile, &report); }
+void Encoder::processTo(std::ofstream &outputFile, std::vector<VerifyEntry> &report) { encodeTo(outputFile, &report, nullptr); }
 
-// processTo(); with `report` through selab200_encode_container_verified (same bytes).
-void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report)
+void Encoder::processLosslessTo(std::ofstream &outputFile, std::vector<RecodedEntry> &recoded)
+{
+    encodeTo(outputFile, nullptr, &recoded);
+}
+
+// processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
+// selab200_encode_container_lossless.
+void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded)
 {
     if (report)
         report->clear();
+    if (recoded)
+        recoded->clear();
     StagingScope staging;
     DeviceWarmup warmup; // CUDA context creation overlaps the file read
     if (g_batch_mode.load())
@@ -833,6 +841,16 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
                                                  (uint32_t)n_frames, channels, w.fmt.sampleRate, w.fmt.bitsPerSample,
                                                  out, cap, &used, raw.data(), raw.size(), &n));
         *report = mirror_report(raw, n);
+    } else if (recoded) {
+        Phase p("lossless encode (device)");
+        std::vector<selab200_lossless_entry> raw(n_frames * channels);
+        size_t n = 0;
+        check(selab200_encode_container_lossless(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                 (uint32_t)n_frames, channels, w.fmt.sampleRate, w.fmt.bitsPerSample,
+                                                 out, cap, &used, raw.data(), raw.size(), &n));
+        for (size_t i = 0; i < n && i < raw.size(); i++)
+            recoded->push_back(RecodedEntry{raw[i].frame, raw[i].channel, raw[i].ref_order, raw[i].order,
+                                            raw[i].ref_words, raw[i].words});
     } else {
         Phase p("encode (device)");
         check(selab200_encode_container(reinterpret_cast<const int16_t *>(file.data + dat.body), (uint32_t)n_frames,
