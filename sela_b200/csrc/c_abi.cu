@@ -76,7 +76,7 @@ struct Context {
     int sms = 0;                                   // streaming multiprocessors of `device`
     cudaStream_t stream = nullptr;                 // stage-level calls
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr; // pipelined batch calls: copy engines ...
-    cudaStream_t s_compute[kLanes] = {};           // ... and alternating compute lanes
+    cudaStream_t s_compute[kLanes] = {};           // ... and compute lanes
     cudaEvent_t ev_h2d[kMaxChunks], ev_done[kMaxChunks], ev_scan[kMaxChunks], ev_reset;
     bool events = false;
     DeviceBuffer in, descs, words, work, lane_work[kLanes], aux, small;
@@ -148,7 +148,7 @@ struct PipelineDrain {
     }
 };
 
-// Chunking of the pipelined host-buffer calls (encode_host, decode_host, container_decode_block): about
+// Chunking of the pipelined host-buffer calls (encode_host, decode_pipeline): about
 // eight chunks, enough to overlap PCIe with compute, each still several waves of warps, workspace bounded
 // for huge batches.  SELAB200_CHUNK_FRAMES forces the chunk size (tools/e2e_chunk_sweep.py sweeps it on the
 // BASELINE batch; tests use it to get many chunks).
@@ -252,6 +252,13 @@ int require_ready_for(const void *device_ptr)
                                        "(selab200_init / selab200_init_devices)", attr.device);
 }
 
+int check_channels(uint32_t channels)
+{
+    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
+        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    return 0;
+}
+
 size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // Raises a kernel's dynamic shared-memory limit; remembered per (kernel, device): the attribute call is a
@@ -345,24 +352,32 @@ struct LosslessArgs {
 
 // ---- device-resident cores (no synchronisation) --------------------------
 
-// `fresh`: reset status and the arena fill level first (a stand-alone batch); the pipelined
-// host path resets once and then chains chunks through *d_used.  `before_scan`: optional event
-// the scan must wait for (the previous chunk's scan, when chunks alternate between streams).
+// How encode_device chains into a pipelined call, and what it produces besides the word arena.  The defaults are
+// a stand-alone batch.
+struct EncodeOptions {
+    bool fresh = true;                          // reset status and the arena fill level first; the pipelined host
+                                                // path resets once and then chains chunks through *d_used
+    cudaEvent_t before_scan = nullptr;          // the scan waits for it (the previous chunk's scan on another lane)
+    cudaEvent_t after_scan = nullptr;           // recorded once this batch's fill level has been taken
+    unsigned long long *h_fill_after = nullptr; // pinned: receives the fill level this batch leaves behind
+    uint8_t *d_container = nullptr;             // gather into this byte-packed .sela image instead of the arena ...
+    unsigned long long sub_base = 0;            // ... where the batch's first subframe is subframe sub_base
+    selab200_analysis_trace *d_trace = nullptr; // the tracing unit kernel writes every unit's analysis here
+    const LosslessArgs *lossless = nullptr;     // encode lossless (DESIGN.md 7.2) and report the re-coded pairs
+};
+
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
                   uint32_t *d_words, size_t capacity, uint64_t *d_used, int32_t *d_status, void *d_ws,
-                  size_t ws_bytes, cudaStream_t stream, bool fresh = true, cudaEvent_t before_scan = nullptr,
-                  cudaEvent_t after_scan = nullptr, unsigned long long *h_fill_after = nullptr,
-                  uint8_t *d_container = nullptr, unsigned long long sub_base = 0,
-                  selab200_analysis_trace *d_trace = nullptr, const LosslessArgs *lossless = nullptr)
+                  size_t ws_bytes, cudaStream_t stream, const EncodeOptions &o = EncodeOptions())
 {
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    if (ws_bytes < (lossless ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
-                             : selab200_encode_workspace_bytes(n_frames, channels)))
+    if (int rc = check_channels(channels))
+        return rc;
+    if (ws_bytes < (o.lossless ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
+                               : selab200_encode_workspace_bytes(n_frames, channels)))
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
         return fail(SELAB200_ERR_ARGUMENT, "stereo PCM must be 16-byte aligned on the device");
-    if (fresh) {
+    if (o.fresh) {
         CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), stream));
         CUDA_TRY(cudaMemsetAsync(d_used, 0, sizeof(uint64_t), stream));
     }
@@ -387,16 +402,16 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
                         : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
         return rc;
-    if (lossless) {
+    if (o.lossless) {
         RepairParams r;
         char *b = static_cast<char *>(d_ws) + align256(selab200_encode_workspace_bytes(n_frames, channels));
         r.count = reinterpret_cast<uint32_t *>(b);
         r.frames = reinterpret_cast<uint32_t *>(b + 256);
         r.orig = reinterpret_cast<UnitRecord *>(b + 256 + align256((size_t)n_frames * 4));
         r.units = reinterpret_cast<RepairUnit *>(reinterpret_cast<char *>(r.orig) + align256(n_units * sizeof(UnitRecord)));
-        r.entries = lossless->entries;
-        r.n_entries = lossless->n_entries;
-        r.frame_base = lossless->frame_base;
+        r.entries = o.lossless->entries;
+        r.n_entries = o.lossless->n_entries;
+        r.frame_base = o.lossless->frame_base;
         CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
         if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
                             : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
@@ -405,10 +420,10 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
                             : launch_repair<false>(p, r, n_frames, n_units, stream))
             return rc;
     } else {
-        const int rc_units = stereo ? (d_trace ? launch_encode_units<true, true>(p, n_units, d_trace, stream)
-                                               : launch_encode_units<true, false>(p, n_units, nullptr, stream))
-                                    : (d_trace ? launch_encode_units<false, true>(p, n_units, d_trace, stream)
-                                               : launch_encode_units<false, false>(p, n_units, nullptr, stream));
+        const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
+                                                 : launch_encode_units<true, false>(p, n_units, nullptr, stream))
+                                    : (o.d_trace ? launch_encode_units<false, true>(p, n_units, o.d_trace, stream)
+                                                 : launch_encode_units<false, false>(p, n_units, nullptr, stream));
         if (rc_units)
             return rc_units;
     }
@@ -416,20 +431,20 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     k_encode_sizes<<<scan_ctas, kScanTile, 0, stream>>>(p);
     if (int rc = launch_check("k_encode_sizes"))
         return rc;
-    if (before_scan)
-        CUDA_TRY(cudaStreamWaitEvent(stream, before_scan, 0));
+    if (o.before_scan)
+        CUDA_TRY(cudaStreamWaitEvent(stream, o.before_scan, 0));
     k_encode_scan<<<scan_ctas, kScanTile, 0, stream>>>(p);
     if (int rc = launch_check("k_encode_scan"))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(d_used, p.residues, 8, cudaMemcpyDeviceToDevice, stream)); // the new fill level (see k_encode_scan)
     // The fill level this chunk leaves behind must be captured BEFORE the next chunk's scan (on the
     // other compute lane) may overwrite *d_used: copy it out now and only then release the event.
-    if (h_fill_after)
-        CUDA_TRY(cudaMemcpyAsync(h_fill_after, d_used, 8, cudaMemcpyDeviceToHost, stream));
-    if (after_scan)
-        CUDA_TRY(cudaEventRecord(after_scan, stream));
-    if (d_container) { // byte-packed .sela stream instead of the word arena
-        k_encode_gather_container<<<(unsigned)((n_sub + 7) / 8), 256, 0, stream>>>(p, d_container, sub_base);
+    if (o.h_fill_after)
+        CUDA_TRY(cudaMemcpyAsync(o.h_fill_after, d_used, 8, cudaMemcpyDeviceToHost, stream));
+    if (o.after_scan)
+        CUDA_TRY(cudaEventRecord(o.after_scan, stream));
+    if (o.d_container) { // byte-packed .sela stream instead of the word arena
+        k_encode_gather_container<<<(unsigned)((n_sub + 7) / 8), 256, 0, stream>>>(p, o.d_container, o.sub_base);
         return launch_check("k_encode_gather_container");
     }
     k_encode_gather<<<(unsigned)((n_sub + 7) / 8), 256, 0, stream>>>(p);
@@ -525,8 +540,8 @@ int decode_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint
                   const uint32_t *d_words, size_t n_words, int16_t *d_pcm, int32_t *d_status, void *d_ws,
                   size_t ws_bytes, cudaStream_t stream, bool fresh = true)
 {
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     if (ws_bytes < selab200_decode_workspace_bytes(n_frames, channels))
         return fail(SELAB200_ERR_ARGUMENT, "decode workspace too small");
     if (fresh)
@@ -587,8 +602,8 @@ int verify_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint
                   int32_t *d_status, void *d_ws, size_t ws_bytes, cudaStream_t stream, bool fresh = true,
                   uint32_t frame_base = 0)
 {
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     if (ws_bytes < selab200_verify_workspace_bytes(n_frames, channels))
         return fail(SELAB200_ERR_ARGUMENT, "verify workspace too small");
     if ((reinterpret_cast<uintptr_t>(d_ref) & 15) != 0)
@@ -642,37 +657,46 @@ int verify_area(size_t n_sub, size_t arena_words, cudaStream_t stream, VerifyAre
     return 0;
 }
 
-// Once every chunk has been compared (the caller has synchronised the lanes): the decode status, and the
-// differing pairs in order.  The per-pair records come down only when the count is not zero.
-int collect_report(const VerifyArea &v, size_t n_sub, cudaStream_t stream, std::vector<selab200_verify_entry> &out)
+// A per-pair record that says something: a verify record with differing samples, a lossless record of a re-coded
+// subframe.  Every other record is all zeros.
+bool record_set(const selab200_verify_entry &e) { return e.n_differing != 0; }
+bool record_set(const selab200_lossless_entry &e) { return e.words != 0; }
+
+// Once the records are complete (the caller has synchronised the lanes that write them): the set ones of the
+// n records at d_records, in order.  The records come down only when the count at d_count is not zero.  A
+// non-null d_status is a decode status that lies right behind the count (VerifyArea): it comes down in the same
+// copy, and a non-zero status fails the call.
+template <typename T>
+int collect_records(const unsigned long long *d_count, const int32_t *d_status, const T *d_records, size_t n,
+                    cudaStream_t stream, std::vector<T> &out)
 {
     out.clear();
-    CUDA_TRY(cudaMemcpyAsync(g.h_small + 12, v.count, 16, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small + 12, d_count, d_status ? 16 : 8, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
-    unsigned long long n;
-    memcpy(&n, g.h_small + 12, 8);
-    const int32_t st = g.h_small[14];
+    unsigned long long count;
+    memcpy(&count, g.h_small + 12, 8);
+    const int32_t st = d_status ? g.h_small[14] : 0;
     if (st != 0)
         return fail(st, "%s", status_text(st));
-    if (n == 0)
+    if (count == 0)
         return 0;
-    std::vector<selab200_verify_entry> all(n_sub);
-    CUDA_TRY(cudaMemcpyAsync(all.data(), v.entries, n_sub * sizeof(selab200_verify_entry), cudaMemcpyDeviceToHost, stream));
+    std::vector<T> all(n);
+    CUDA_TRY(cudaMemcpyAsync(all.data(), d_records, n * sizeof(T), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
-    out.reserve((size_t)n);
-    for (const selab200_verify_entry &e : all)
-        if (e.n_differing)
+    out.reserve((size_t)count);
+    for (const T &e : all)
+        if (record_set(e))
             out.push_back(e);
     return 0;
 }
 
-// The report of a host-buffer call: *n_entries = all of it, at most `capacity` entries written.
-int deliver_report(const std::vector<selab200_verify_entry> &report, selab200_verify_entry *entries, size_t capacity,
-                   size_t *n_entries)
+// The records of a host-buffer call: *n_entries = all of them, at most `capacity` entries written.
+template <typename T>
+int deliver_records(const std::vector<T> &records, T *entries, size_t capacity, size_t *n_entries)
 {
-    *n_entries = report.size();
-    if (capacity && !report.empty())
-        memcpy(entries, report.data(), std::min(capacity, report.size()) * sizeof(selab200_verify_entry));
+    *n_entries = records.size();
+    if (capacity && !records.empty())
+        memcpy(entries, records.data(), std::min(capacity, records.size()) * sizeof(T));
     return 0;
 }
 
@@ -909,15 +933,17 @@ int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_fram
         return rc;
     if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_entries || !d_n_entries || !d_status || !d_workspace)
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     const cudaStream_t st = (cudaStream_t)stream;
     CUDA_TRY(cudaMemsetAsync(d_n_entries, 0, sizeof(uint64_t), st));
     if (n_frames)
         CUDA_TRY(cudaMemsetAsync(d_entries, 0, (size_t)n_frames * channels * sizeof(selab200_lossless_entry), st));
     const LosslessArgs la{d_entries, reinterpret_cast<unsigned long long *>(d_n_entries), 0};
+    EncodeOptions o;
+    o.lossless = &la;
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
-                         d_workspace, workspace_bytes, st, true, nullptr, nullptr, nullptr, nullptr, 0, nullptr, &la);
+                         d_workspace, workspace_bytes, st, o);
 }
 
 int selab200_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
@@ -948,14 +974,6 @@ int selab200_verify_frames_device(const selab200_subframe_desc *d_descs, uint32_
                          (cudaStream_t)stream);
 }
 
-// Host-buffer batch calls.  Pipelined in chunks of frames over three engines:
-//   s_h2d      PCM (encode) / descriptors + words (decode) of chunk c+1 .. go up
-//   s_compute  two alternating lanes run the kernels of chunk c (tails of one chunk overlap the
-//              head of the next; the encoder's scans are chained by events because each needs
-//              the arena fill level its predecessor left in *d_used)
-//   s_d2h      results of chunk c-1 come down
-// With pinned host buffers (selab200_host_alloc) the three overlap; pageable memory works
-// but serialises inside the driver.
 int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
                                        const uint32_t *d_words, size_t n_words, int32_t *d_residues,
                                        int32_t *d_status, void *stream)
@@ -965,8 +983,8 @@ int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, ui
         return rc;
     if (!d_descs || !d_words || !d_residues || !d_status)
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), (cudaStream_t)stream));
     if (n_frames == 0)
         return 0;
@@ -1026,20 +1044,39 @@ static unsigned long long container_frame_byte(unsigned long long f, uint32_t ch
     return kContainerHeaderBytes + 4 * f + (unsigned long long)kSubframeHeaderBytes * f * channels + 4 * words;
 }
 
-// The pipelined encoder over host buffers.  Two output forms: descriptors + word arena
-// (descs/words), or the byte-packed container (`container`, descs == words == nullptr) whose
-// device image lives in g.words.
-// `defer`: leave the word arena / container body on the device (g.words) instead of copying it out chunk by
-// chunk -- the multi-device driver places every device's block once the sizes of the blocks before it are known.
-// With `defer`, `container` is only a flag (any non-null value selects the byte-packed form).
+// Host-buffer batch calls.  Pipelined in chunks of frames (plan_chunks) over three engines:
+//   s_h2d      PCM (encode) / descriptors + words (decode) of chunk c+1 .. go up
+//   s_compute  compute lanes run the kernels of chunk c, so that the tails of one chunk overlap the head of the
+//              next.  Encode alternates two lanes (its scans are chained by events because each needs the arena
+//              fill level its predecessor left in *d_used) and verifies, if asked, on the others; decode gives
+//              every chunk a lane of its own, up to kLanes.
+//   s_d2h      results of chunk c-1 come down
+// With pinned host buffers (selab200_host_alloc) the three overlap; pageable memory works
+// but serialises inside the driver.
+
+// Where the pipelined encoder puts its output.
+enum class EncodeForm { arena, container };
+struct EncodeTarget {
+    EncodeForm form;
+    // Leave the word arena / container body on the device (g.words) instead of copying it out chunk by chunk:
+    // with several devices, every device's block is placed once the sizes of the blocks before it are known.
+    bool defer;
+    selab200_subframe_desc *descs; // arena: one descriptor per subframe (written even with `defer`)
+    uint32_t *words;               // arena: the Rice words (unused with `defer`)
+    uint8_t *container;            // container: the whole .sela stream, header written by the caller (unused with `defer`)
+    size_t words_capacity;         // Rice words the output holds
+};
+
+// The pipelined encoder over host buffers, frames numbered from frame_base in what it reports.
 // `report` (container form only): also verify the container image, chunk by chunk on the device, and return
-// the differing (frame, channel) pairs, frames numbered from frame_base.
-// `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs, numbered likewise.
-static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
-                       uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
-                       bool defer = false, std::vector<selab200_verify_entry> *report = nullptr,
-                       uint32_t frame_base = 0, std::vector<selab200_lossless_entry> *recoded = nullptr)
+// the differing (frame, channel) pairs.
+// `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs.
+static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
+                       size_t *words_used, uint32_t frame_base, std::vector<selab200_verify_entry> *report,
+                       std::vector<selab200_lossless_entry> *recoded)
 {
+    const size_t words_capacity = t.words_capacity;
+    const bool to_container = t.form == EncodeForm::container;
     *words_used = 0;
     if (report)
         report->clear();
@@ -1052,7 +1089,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const uint32_t n_chunks = plan.chunks();
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const bool verify = report && container;
+    const bool verify = report && to_container;
     const size_t ws_bytes = recoded ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
                                     : selab200_encode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
@@ -1098,11 +1135,16 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         cudaStream_t cs = g.s_compute[c % kEncLanes];
         DeviceBuffer &ws = g.lane_work[c % kEncLanes];
         CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[c], 0));
+        EncodeOptions o;
+        o.fresh = false;
+        o.before_scan = c ? g.ev_scan[c - 1] : nullptr;
+        o.after_scan = g.ev_scan[c];
+        o.h_fill_after = &g.h_totals[c + 1];
+        o.d_container = to_container ? static_cast<uint8_t *>(g.words.ptr) : nullptr;
+        o.sub_base = (unsigned long long)f0 * channels;
+        o.lossless = recoded ? &la : nullptr;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
-                                   d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, false,
-                                   c ? g.ev_scan[c - 1] : nullptr, g.ev_scan[c], &g.h_totals[c + 1],
-                                   container ? static_cast<uint8_t *>(g.words.ptr) : nullptr,
-                                   (unsigned long long)f0 * channels, nullptr, recoded ? &la : nullptr))
+                                   d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, o))
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
         if (verify) {
@@ -1136,24 +1178,24 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         const unsigned long long lo = g.h_totals[c], hi = g.h_totals[c + 1];
         if (hi > words_capacity || hi < lo)
             break; // capacity exceeded: reported through the status word below
-        if (defer) {
-            if (!container)
-                CUDA_TRY(cudaMemcpyAsync(descs + (size_t)f0 * channels, d_descs + (size_t)f0 * channels,
+        if (t.defer) {
+            if (!to_container)
+                CUDA_TRY(cudaMemcpyAsync(t.descs + (size_t)f0 * channels, d_descs + (size_t)f0 * channels,
                                          (size_t)nf * channels * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost,
                                          g.s_d2h));
             continue;
         }
-        if (container) {
+        if (to_container) {
             const unsigned long long b0 = container_frame_byte(f0, channels, lo);
             const unsigned long long b1 = container_frame_byte(f0 + nf, channels, hi);
-            CUDA_TRY(cudaMemcpyAsync(container + b0, static_cast<uint8_t *>(g.words.ptr) + b0, b1 - b0,
+            CUDA_TRY(cudaMemcpyAsync(t.container + b0, static_cast<uint8_t *>(g.words.ptr) + b0, b1 - b0,
                                      cudaMemcpyDeviceToHost, g.s_d2h));
             continue;
         }
-        CUDA_TRY(cudaMemcpyAsync(descs + (size_t)f0 * channels, d_descs + (size_t)f0 * channels,
+        CUDA_TRY(cudaMemcpyAsync(t.descs + (size_t)f0 * channels, d_descs + (size_t)f0 * channels,
                                  (size_t)nf * channels * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost,
                                  g.s_d2h));
-        CUDA_TRY(cudaMemcpyAsync(words + lo, d_words + lo, (hi - lo) * 4, cudaMemcpyDeviceToHost, g.s_d2h));
+        CUDA_TRY(cudaMemcpyAsync(t.words + lo, d_words + lo, (hi - lo) * 4, cudaMemcpyDeviceToHost, g.s_d2h));
     }
     for (int i = 0; i < (verify ? kLanes : kEncLanes); i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
@@ -1164,18 +1206,10 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     *words_used = (size_t)used; // for CAPACITY: the size the caller needs
     if (g.h_small[0] != 0)
         return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (recoded) { // the per-pair records come down only when there are any
-        unsigned long long n = 0;
-        CUDA_TRY(cudaMemcpy(&n, d_recoded, 8, cudaMemcpyDeviceToHost));
-        if (n) {
-            std::vector<selab200_lossless_entry> all(n_sub);
-            CUDA_TRY(cudaMemcpy(all.data(), d_rec_entries, n_sub * sizeof(selab200_lossless_entry), cudaMemcpyDeviceToHost));
-            for (const selab200_lossless_entry &e : all)
-                if (e.words)
-                    recoded->push_back(e);
-        }
-    }
-    return verify ? collect_report(va, n_sub, g.s_d2h, *report) : 0;
+    if (recoded)
+        if (int rc = collect_records(d_recoded, nullptr, d_rec_entries, n_sub, g.s_d2h, *recoded))
+            return rc;
+    return verify ? collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, *report) : 0;
 }
 
 // The words n descriptors reference, [lo, hi) (descriptors need not be in arena order); hi <= lo if none.
@@ -1196,109 +1230,171 @@ static void words_referenced(const selab200_subframe_desc *dc, size_t n, size_t 
     }
 }
 
-static int decode_host(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
-                       const uint32_t *words, size_t n_words, int16_t *pcm_out)
+struct selab200_container {
+    const uint8_t *bytes = nullptr;
+    size_t n_bytes = 0;
+    selab200_container_info info{};
+    ContainerBuffers buf;
+    size_t piece_bytes = 0;
+    int n_pieces = 0;
+};
+
+// One host-to-device copy.
+struct Upload {
+    void *dst = nullptr;
+    const void *src = nullptr;
+    size_t bytes = 0;
+};
+
+// Where the decode-side pipeline's coded input comes from, frames numbered file-globally in both cases: the caller's
+// descriptor and word arrays (h == nullptr), or an open container whose byte image is unpacked into the word arena on
+// the device.  start() sizes the arena for the block of frames [F0, F0 + NF) and uploads what the block needs as a
+// whole; chunk() puts one chunk's descriptors and words on the device, then `also` on the stream that carried the
+// descriptors, and makes the chunk's lane wait for all of it.
+struct CodedInput {
+    const selab200_subframe_desc *descs; // the whole file's descriptors, in host memory
+    const uint32_t *words;               // caller arrays: the words the descriptors reference
+    size_t n_words;
+    const selab200_container *h;         // or an open container
+    // set by start()
+    uint32_t channels = 0;
+    uint32_t *arena = nullptr;           // the decoder's word array, addressed by the descriptors' offsets
+    const uint8_t *d_bytes = nullptr;    // container: the byte image on this device, addressed by file offset
+    bool primary = true;
+
+    int start(uint32_t F0, uint32_t NF, uint32_t ch)
+    {
+        channels = ch;
+        if (!h) {
+            if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
+            arena = static_cast<uint32_t *>(g.words.ptr);
+            return 0;
+        }
+        // The arena keeps the descriptors' file-order offsets: it is addressed through a pointer shifted back by the
+        // block's first word, so nothing is re-based.
+        const unsigned long long w_lo = descs[(size_t)F0 * ch].refl_offset;
+        const selab200_subframe_desc &tail = descs[(size_t)(F0 + NF) * ch - 1];
+        const unsigned long long w_hi = tail.res_offset + tail.res_words;
+        if (int rc = g.words.ensure((size_t)(w_hi - w_lo) * 4 + 96)) return rc;
+        // 16 bytes of slack in front (the Rice decoder reads whole 16-byte vectors), the 16-byte phase of file order kept
+        arena = reinterpret_cast<uint32_t *>(static_cast<char *>(g.words.ptr) + 16 + ((w_lo * 4) & 15)) - w_lo;
+        // The primary device holds the whole byte image (uploaded by selab200_container_open, in pieces with events);
+        // any other device uploads just the bytes of its block.
+        primary = tl_ctx == &g_slots[0];
+        d_bytes = static_cast<const uint8_t *>(h->buf.d_bytes);
+        if (!primary) {
+            const unsigned long long b0 = container_frame_byte(F0, ch, w_lo) & ~3ull; // the unpack kernel reads aligned 32-bit words
+            const size_t end = std::min<size_t>(h->n_bytes, (size_t)container_frame_byte(F0 + NF, ch, w_hi) + 4);
+            if (int rc = g.aux.ensure(end - (size_t)b0 + 64)) return rc;
+            CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, h->bytes + b0, end - (size_t)b0, cudaMemcpyHostToDevice, g.s_h2d));
+            CUDA_TRY(cudaEventRecord(g.ev_h2d[0], g.s_h2d));
+            d_bytes = static_cast<const uint8_t *>(g.aux.ptr) - b0;
+        }
+        return 0;
+    }
+
+    // Chunk c, frames [f0, f0 + nf): its descriptors to d_descs and its words to the arena, for `lane` to decode.
+    int chunk(uint32_t c, uint32_t f0, uint32_t nf, selab200_subframe_desc *d_descs, cudaStream_t lane, const Upload &also)
+    {
+        const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
+        const size_t n = (size_t)nf * channels;
+        // a container's descriptors go up on the chunk's own lane: s_h2d is still busy with the container bytes
+        const cudaStream_t carrier = h ? lane : g.s_h2d;
+        CUDA_TRY(cudaMemcpyAsync(d_descs, dc, n * sizeof(*dc), cudaMemcpyHostToDevice, carrier));
+        if (!h) {
+            unsigned long long lo, hi;
+            words_referenced(dc, n, n_words, lo, hi);
+            if (hi > lo)
+                CUDA_TRY(cudaMemcpyAsync(arena + lo, words + lo, (hi - lo) * 4, cudaMemcpyHostToDevice, g.s_h2d));
+        } else {
+            cudaEvent_t uploaded = g.ev_h2d[0];
+            if (primary) { // the container bytes this chunk reads end with its last subframe (+3 bytes of slack)
+                const selab200_subframe_desc &last = dc[n - 1];
+                const unsigned long long end_byte =
+                    container_frame_byte(f0 + nf, channels, last.res_offset + last.res_words) + 3;
+                uploaded = h->buf.ev_piece[std::min(h->n_pieces - 1, (int)(end_byte / h->piece_bytes))];
+            }
+            CUDA_TRY(cudaStreamWaitEvent(lane, uploaded, 0));
+            k_container_unpack<<<(unsigned)((n + 7) / 8), 256, 0, lane>>>(d_bytes, d_descs, (uint32_t)n, channels,
+                                                                           (unsigned long long)f0 * channels, arena);
+            if (int rc = launch_check("k_container_unpack"))
+                return rc;
+        }
+        if (also.bytes)
+            CUDA_TRY(cudaMemcpyAsync(also.dst, also.src, also.bytes, cudaMemcpyHostToDevice, carrier));
+        if (!h) {
+            CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
+            CUDA_TRY(cudaStreamWaitEvent(lane, g.ev_h2d[c], 0));
+        }
+        return 0;
+    }
+};
+
+// Frames [F0, F0 + NF) of `in` through the chunk pipeline on the device of the current context.  Without `report`
+// the decoded samples come down into pcm_out; with it, each lane compares them on the device with `source`
+// (verify_device) and only the differing pairs come back.  pcm_out, source and the report's frames are file-global.
+static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t channels, int16_t *pcm_out,
+                           const int16_t *source, std::vector<selab200_verify_entry> *report)
 {
-    if (n_frames == 0)
+    if (report)
+        report->clear();
+    if (NF == 0)
         return 0;
     PipelineDrain drain;
     // Every chunk gets its own compute lane (up to kLanes): the Rice kernel is one lane per stream
     // and latency-bound (a fixed time however small the chunk), so the chunks' Rice kernels must
     // overlap each other and the synthesis kernels of earlier chunks rather than queue up.
-    const ChunkPlan plan = plan_chunks(n_frames);
+    const ChunkPlan plan = plan_chunks(NF);
     const uint32_t n_chunks = plan.chunks();
-    const size_t n_sub = (size_t)n_frames * channels;
+    const size_t n_sub = (size_t)NF * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const size_t ws_bytes = selab200_decode_workspace_bytes(plan.max_frames, channels);
+    const size_t ws_bytes = report ? selab200_verify_workspace_bytes(plan.max_frames, channels)
+                                   : selab200_decode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
     for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
+    if (int rc = in.start(F0, NF, channels)) return rc;
     int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
-    uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
-
-    CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
+    VerifyArea va;
+    if (report) {
+        if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
+    } else {
+        CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
+    }
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
     for (int i = 1; i < kLanes; i++)
         CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
     for (uint32_t c = 0; c < n_chunks; c++) {
-        const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
-        const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
-        unsigned long long lo, hi;
-        words_referenced(dc, (size_t)nf * channels, n_words, lo, hi);
-        CUDA_TRY(cudaMemcpyAsync(d_descs + (size_t)f0 * channels, dc, (size_t)nf * channels * sizeof(*dc),
-                                 cudaMemcpyHostToDevice, g.s_h2d));
-        if (hi > lo)
-            CUDA_TRY(cudaMemcpyAsync(d_words + lo, words + lo, (hi - lo) * 4, cudaMemcpyHostToDevice, g.s_h2d));
-        CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
+        const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0; // within the block
+        const size_t at = (size_t)f0 * channels, file_at = (size_t)(F0 + f0) * channels; // the chunk's first subframe
         cudaStream_t cs = g.s_compute[c % kLanes];
         DeviceBuffer &ws = g.lane_work[c % kLanes];
-        CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[c], 0));
-        if (int rc = decode_device(d_descs + (size_t)f0 * channels, nf, channels, d_words, n_words,
-                                   d_pcm + (size_t)f0 * channels * kFrame, d_status, ws.ptr, ws.bytes, cs, false))
+        // verify: the chunk's source PCM goes up with its coded input
+        const Upload src = report ? Upload{d_pcm + at * kFrame, source + file_at * kFrame, nf * frame_bytes} : Upload{};
+        if (int rc = in.chunk(c, F0 + f0, nf, d_descs + at, cs, src))
+            return rc;
+        if (report) {
+            if (int rc = verify_device(d_descs + at, nf, channels, in.arena, in.n_words, d_pcm + at * kFrame,
+                                       va.entries + at, va.count, va.status, ws.ptr, ws.bytes, cs, false, F0 + f0))
+                return rc;
+            continue;
+        }
+        if (int rc = decode_device(d_descs + at, nf, channels, in.arena, in.n_words, d_pcm + at * kFrame, d_status,
+                                   ws.ptr, ws.bytes, cs, false))
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
         CUDA_TRY(cudaStreamWaitEvent(g.s_d2h, g.ev_done[c], 0));
-        CUDA_TRY(cudaMemcpyAsync(pcm_out + (size_t)f0 * channels * kFrame, d_pcm + (size_t)f0 * channels * kFrame,
-                                 nf * frame_bytes, cudaMemcpyDeviceToHost, g.s_d2h));
+        CUDA_TRY(cudaMemcpyAsync(pcm_out + file_at * kFrame, d_pcm + at * kFrame, nf * frame_bytes,
+                                 cudaMemcpyDeviceToHost, g.s_d2h));
     }
-    return read_status(g.s_d2h, d_status);
-}
-
-// decode_host with a compare instead of the download: the source PCM goes up with the coded chunk, each lane
-// decodes into its own scratch and compares there (verify_device), and only the count -- and the per-pair
-// records when it is not zero -- come back.  Frames in the report are numbered from frame_base.
-static int verify_host(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels, const uint32_t *words,
-                       size_t n_words, const int16_t *pcm, uint32_t frame_base, std::vector<selab200_verify_entry> &report)
-{
-    report.clear();
-    if (n_frames == 0)
-        return 0;
-    PipelineDrain drain;
-    const ChunkPlan plan = plan_chunks(n_frames);
-    const uint32_t n_chunks = plan.chunks();
-    const size_t n_sub = (size_t)n_frames * channels;
-    const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const size_t ws_bytes = selab200_verify_workspace_bytes(plan.max_frames, channels);
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
-    for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
-        if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
-    int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
-    selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
-    uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
-    VerifyArea va;
-    if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
-    CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
-    for (int i = 1; i < kLanes; i++)
-        CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
-    for (uint32_t c = 0; c < n_chunks; c++) {
-        const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
-        const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
-        unsigned long long lo, hi;
-        words_referenced(dc, (size_t)nf * channels, n_words, lo, hi);
-        CUDA_TRY(cudaMemcpyAsync(d_descs + (size_t)f0 * channels, dc, (size_t)nf * channels * sizeof(*dc),
-                                 cudaMemcpyHostToDevice, g.s_h2d));
-        if (hi > lo)
-            CUDA_TRY(cudaMemcpyAsync(d_words + lo, words + lo, (hi - lo) * 4, cudaMemcpyHostToDevice, g.s_h2d));
-        CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)f0 * channels * kFrame,
-                                 nf * frame_bytes, cudaMemcpyHostToDevice, g.s_h2d));
-        CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
-        cudaStream_t cs = g.s_compute[c % kLanes];
-        DeviceBuffer &ws = g.lane_work[c % kLanes];
-        CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[c], 0));
-        if (int rc = verify_device(d_descs + (size_t)f0 * channels, nf, channels, d_words, n_words,
-                                   d_pcm + (size_t)f0 * channels * kFrame, va.entries + (size_t)f0 * channels, va.count,
-                                   va.status, ws.ptr, ws.bytes, cs, false, frame_base + f0))
-            return rc;
-    }
+    if (!report)
+        return read_status(g.s_d2h, d_status);
     for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
-    return collect_report(va, n_sub, g.s_d2h, report);
+    return collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, *report);
 }
 
 // ---- every initialised device at once ----------------------------------------------------------
@@ -1319,15 +1415,6 @@ struct DevicePart {
     std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
     std::vector<selab200_lossless_entry> recoded; // lossless calls: this block's re-coded pairs, file-global frames
 };
-
-// The blocks' reports one after the other: blocks are contiguous and in frame order, so this is in order too.
-static std::vector<selab200_verify_entry> joined_reports(const std::vector<DevicePart> &parts)
-{
-    std::vector<selab200_verify_entry> all;
-    for (const DevicePart &p : parts)
-        all.insert(all.end(), p.report.begin(), p.report.end());
-    return all;
-}
 
 static std::vector<DevicePart> device_parts(uint32_t n_frames)
 {
@@ -1371,56 +1458,66 @@ static int run_on_devices(std::vector<DevicePart> &parts, F work)
     return 0;
 }
 
-static int encode_all_devices(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
-                              uint32_t *words, size_t words_capacity, size_t *words_used, uint8_t *container,
-                              std::vector<selab200_verify_entry> *report = nullptr,
-                              std::vector<selab200_lossless_entry> *recoded = nullptr)
+// What run_blocks did: its blocks, and the blocks' reports and re-coded lists one after the other.  Blocks are
+// contiguous and in frame order, so the joined lists are in order too.
+struct Blocks {
+    int rc = 0;
+    std::vector<DevicePart> parts;
+    std::vector<selab200_verify_entry> report;
+    std::vector<selab200_lossless_entry> recoded;
+};
+
+// Runs work(block) over frames [0, n_frames) of a host-buffer call: as one block on the primary context, or, with
+// enough frames for several devices (use_all_devices), as one block per device, each on its own worker thread.
+template <typename F>
+static Blocks run_blocks(uint32_t n_frames, F work)
 {
-    std::vector<DevicePart> parts = device_parts(n_frames);
-    const size_t per_frame = (size_t)channels * kFrame;
-    const int rc = run_on_devices(parts, [&](DevicePart &p) {
-        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, descs ? descs + (size_t)p.f0 * channels : nullptr, nullptr,
-                           selab200_encode_words_bound(p.nf, channels), &p.used, container, true,
-                           report ? &p.report : nullptr, p.f0, recoded ? &p.recoded : nullptr);
-    });
-    if (report)
-        *report = joined_reports(parts);
-    if (recoded) {
-        recoded->clear();
-        for (const DevicePart &p : parts)
-            recoded->insert(recoded->end(), p.recoded.begin(), p.recoded.end());
+    Blocks b;
+    if (use_all_devices(n_frames)) {
+        b.parts = device_parts(n_frames);
+        b.rc = run_on_devices(b.parts, work);
+    } else {
+        b.parts.resize(1);
+        b.parts[0].nf = n_frames;
+        b.rc = work(b.parts[0]);
     }
-    size_t total = 0;
-    for (const DevicePart &p : parts)
-        total += p.used;
-    *words_used = total;
-    if (rc)
-        return rc;
-    if (total > words_capacity)
+    for (const DevicePart &p : b.parts) {
+        b.report.insert(b.report.end(), p.report.begin(), p.report.end());
+        b.recoded.insert(b.recoded.end(), p.recoded.begin(), p.recoded.end());
+    }
+    return b;
+}
+
+// The encoder's second step with several devices: every device's block (left on the device, EncodeTarget::defer)
+// goes out once the sizes of all blocks are known, and the descriptors' offsets are re-based to file order.
+static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels, const EncodeTarget &t, size_t total)
+{
+    if (total > t.words_capacity)
         return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    const bool to_container = t.form == EncodeForm::container;
     size_t base = 0;
     for (int d = 0; d < g_n_ctx; d++) { // every device's block goes out at once, each over its own link
         tl_ctx = &g_slots[d];
         const DevicePart &p = parts[d];
         CUDA_TRY(cudaSetDevice(g.device));
-        if (container) {
+        if (to_container) {
             const size_t body = (size_t)container_frame_byte(p.nf, channels, p.used) - kContainerHeaderBytes;
             const size_t at = (size_t)container_frame_byte(p.f0, channels, base);
             if (body)
-                CUDA_TRY(cudaMemcpyAsync(container + at, static_cast<uint8_t *>(g.words.ptr) + kContainerHeaderBytes, body,
+                CUDA_TRY(cudaMemcpyAsync(t.container + at, static_cast<uint8_t *>(g.words.ptr) + kContainerHeaderBytes, body,
                                          cudaMemcpyDeviceToHost, g.s_d2h));
         } else if (p.used) {
-            CUDA_TRY(cudaMemcpyAsync(words + base, g.words.ptr, p.used * 4, cudaMemcpyDeviceToHost, g.s_d2h));
+            CUDA_TRY(cudaMemcpyAsync(t.words + base, g.words.ptr, p.used * 4, cudaMemcpyDeviceToHost, g.s_d2h));
         }
         base += p.used;
     }
-    if (!container) { // meanwhile: descriptor offsets from block-local to file order
+    if (!to_container) { // meanwhile: descriptor offsets from block-local to file order
         size_t b = 0;
         for (const DevicePart &p : parts) {
             if (b)
                 for (size_t i = (size_t)p.f0 * channels; i < (size_t)(p.f0 + p.nf) * channels; i++) {
-                    descs[i].refl_offset += b;
-                    descs[i].res_offset += b;
+                    t.descs[i].refl_offset += b;
+                    t.descs[i].res_offset += b;
                 }
             b += p.used;
         }
@@ -1438,28 +1535,32 @@ static int encode_all_devices(const int16_t *pcm, uint32_t n_frames, uint32_t ch
     return rc2;
 }
 
-static int decode_all_devices(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
-                              const uint32_t *words, size_t n_words, int16_t *pcm_out)
+// Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.
+static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
+                         size_t *words_used, std::vector<selab200_verify_entry> *report,
+                         std::vector<selab200_lossless_entry> *recoded)
 {
-    std::vector<DevicePart> parts = device_parts(n_frames);
+    const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
-    return run_on_devices(parts, [&](DevicePart &p) {
-        return decode_host(descs + (size_t)p.f0 * channels, p.nf, channels, words, n_words, pcm_out + p.f0 * per_frame);
+    Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
+        EncodeTarget block = t;
+        if (split) // the block stays on its device; its words are counted from its own start
+            block = EncodeTarget{t.form, true, t.descs ? t.descs + (size_t)p.f0 * channels : nullptr, nullptr, nullptr,
+                                 selab200_encode_words_bound(p.nf, channels)};
+        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, &p.used, p.f0, report ? &p.report : nullptr,
+                           recoded ? &p.recoded : nullptr);
     });
-}
-
-static int verify_all_devices(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
-                              const uint32_t *words, size_t n_words, const int16_t *pcm,
-                              std::vector<selab200_verify_entry> &report)
-{
-    std::vector<DevicePart> parts = device_parts(n_frames);
-    const size_t per_frame = (size_t)channels * kFrame;
-    const int rc = run_on_devices(parts, [&](DevicePart &p) {
-        return verify_host(descs + (size_t)p.f0 * channels, p.nf, channels, words, n_words, pcm + p.f0 * per_frame, p.f0,
-                           p.report);
-    });
-    report = joined_reports(parts);
-    return rc;
+    if (report)
+        *report = std::move(b.report);
+    if (recoded)
+        *recoded = std::move(b.recoded);
+    size_t total = 0;
+    for (const DevicePart &p : b.parts)
+        total += p.used;
+    *words_used = total;
+    if (b.rc || !split)
+        return b.rc;
+    return place_blocks(b.parts, channels, t, total);
 }
 
 extern "C" {
@@ -1473,25 +1574,11 @@ int selab200_encode_frames(const int16_t *pcm, uint32_t n_frames, uint32_t chann
         return rc;
     if (!pcm || !descs || !words || !words_used)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    if (use_all_devices(n_frames))
-        return encode_all_devices(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr);
-    return encode_host(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr);
+    if (int rc = check_channels(channels))
+        return rc;
+    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
+    return encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr);
 }
-
-} // extern "C"
-
-// The report of a lossless host-buffer call: *n_entries = all of it, at most `capacity` entries written.
-static void deliver_recoded(const std::vector<selab200_lossless_entry> &rec, selab200_lossless_entry *entries,
-                            size_t capacity, size_t *n_entries)
-{
-    *n_entries = rec.size();
-    if (capacity && !rec.empty())
-        memcpy(entries, rec.data(), std::min(capacity, rec.size()) * sizeof(selab200_lossless_entry));
-}
-
-extern "C" {
 
 int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                     selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
@@ -1503,19 +1590,14 @@ int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint3
         return rc;
     if (!pcm || !descs || !words || !words_used || (!entries && capacity) || !n_entries)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     *n_entries = 0;
     std::vector<selab200_lossless_entry> rec;
-    const int rc = use_all_devices(n_frames)
-                       ? encode_all_devices(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr,
-                                            nullptr, &rec)
-                       : encode_host(pcm, n_frames, channels, descs, words, words_capacity, words_used, nullptr, false,
-                                     nullptr, 0, &rec);
-    if (rc)
+    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
+    if (int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, &rec))
         return rc;
-    deliver_recoded(rec, entries, capacity, n_entries);
-    return 0;
+    return deliver_records(rec, entries, capacity, n_entries);
 }
 
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
@@ -1525,18 +1607,19 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 
 } // extern "C"
 
-// selab200_encode_container, and with `report` its verified form (g_mutex held by the caller).
+// selab200_encode_container, and with `report` its verified form, with `recoded` its lossless form (g_mutex held
+// by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
                                  std::vector<selab200_verify_entry> *report,
-                                 std::vector<selab200_lossless_entry> *recoded = nullptr)
+                                 std::vector<selab200_lossless_entry> *recoded)
 {
     if (int rc = require_ready())
         return rc;
     if ((!pcm && n_frames) || !container || !bytes_used)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     const unsigned long long fixed = container_frame_byte(n_frames, channels, 0);
     *bytes_used = (size_t)fixed;
     if (capacity < fixed)
@@ -1548,11 +1631,8 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
                                 (uint8_t)n_frames, (uint8_t)(n_frames >> 8), (uint8_t)(n_frames >> 16), (uint8_t)(n_frames >> 24)};
     memcpy(container, header, sizeof header);
     size_t words_used = 0;
-    const int rc = use_all_devices(n_frames)
-                       ? encode_all_devices(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
-                                            container, report, recoded)
-                       : encode_host(pcm, n_frames, channels, nullptr, nullptr, (size_t)((capacity - fixed) / 4), &words_used,
-                                     container, false, report, 0, recoded);
+    const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4)};
+    const int rc = encode_blocks(pcm, n_frames, channels, t, &words_used, report, recoded);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
     return rc;
 }
@@ -1564,7 +1644,7 @@ int selab200_encode_container(const int16_t *pcm, uint32_t n_frames, uint32_t ch
 {
     std::lock_guard<std::mutex> lock(g_mutex);
     return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
-                                 nullptr);
+                                 nullptr, nullptr);
 }
 
 int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -1580,9 +1660,9 @@ int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, ui
     *n_entries = 0;
     std::vector<selab200_verify_entry> report;
     if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
-                                       bytes_used, &report))
+                                       bytes_used, &report, nullptr))
         return rc;
-    return deliver_report(report, entries, entries_capacity, n_entries);
+    return deliver_records(report, entries, entries_capacity, n_entries);
 }
 
 int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -1600,8 +1680,7 @@ int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, ui
     if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
                                        bytes_used, nullptr, &rec))
         return rc;
-    deliver_recoded(rec, entries, entries_capacity, n_entries);
-    return 0;
+    return deliver_records(rec, entries, entries_capacity, n_entries);
 }
 
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -1612,11 +1691,12 @@ int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frame
         return rc;
     if (!descs || !pcm_out || (!words && n_words))
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    if (use_all_devices(n_frames))
-        return decode_all_devices(descs, n_frames, channels, words, n_words, pcm_out);
-    return decode_host(descs, n_frames, channels, words, n_words, pcm_out);
+    if (int rc = check_channels(channels))
+        return rc;
+    const CodedInput in{descs, words, n_words, nullptr};
+    return run_blocks(n_frames, [&](DevicePart &p) {
+        return decode_pipeline(in, p.f0, p.nf, channels, pcm_out, nullptr, nullptr);
+    }).rc;
 }
 
 int selab200_verify_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -1628,29 +1708,21 @@ int selab200_verify_frames(const selab200_subframe_desc *descs, uint32_t n_frame
         return rc;
     if (((!descs || !pcm) && n_frames) || (!words && n_words) || (!entries && capacity) || !n_entries)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    *n_entries = 0;
-    std::vector<selab200_verify_entry> report;
-    const int rc = use_all_devices(n_frames) ? verify_all_devices(descs, n_frames, channels, words, n_words, pcm, report)
-                                             : verify_host(descs, n_frames, channels, words, n_words, pcm, 0, report);
-    if (rc)
+    if (int rc = check_channels(channels))
         return rc;
-    return deliver_report(report, entries, capacity, n_entries);
+    *n_entries = 0;
+    const CodedInput in{descs, words, n_words, nullptr};
+    const Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
+        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.report);
+    });
+    if (b.rc)
+        return b.rc;
+    return deliver_records(b.report, entries, capacity, n_entries);
 }
 
 // ---- .sela container, decode side ----------------------------------------------------------
 
 } // extern "C"
-
-struct selab200_container {
-    const uint8_t *bytes = nullptr;
-    size_t n_bytes = 0;
-    selab200_container_info info{};
-    ContainerBuffers buf;
-    size_t piece_bytes = 0;
-    int n_pieces = 0;
-};
 
 namespace {
 
@@ -1851,115 +1923,6 @@ int selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_c
     return 0;
 }
 
-} // extern "C"
-
-// Frames [F0, F0 + NF) of an open container on the device of the current context.  The primary device holds the
-// whole byte image (uploaded by selab200_container_open, in pieces with events); any other device uploads just
-// the bytes of its block.  The word arena keeps the descriptors' file-order offsets: it is addressed through a
-// pointer shifted back by the block's first word, so nothing is re-based.
-// With `report` the block is verified instead of downloaded: pcm (the whole file's source PCM) goes up chunk by
-// chunk on the chunk's lane, every lane decodes into its own scratch and compares (verify_device).
-static int container_decode_block(selab200_container *h, uint32_t F0, uint32_t NF, int16_t *pcm_out, bool primary,
-                                  const int16_t *pcm = nullptr, std::vector<selab200_verify_entry> *report = nullptr)
-{
-    if (report)
-        report->clear();
-    if (NF == 0)
-        return 0;
-    const uint32_t channels = h->info.channels;
-    const selab200_subframe_desc *hd = h->buf.h_descs;
-    PipelineDrain drain;
-    const ChunkPlan plan = plan_chunks(NF);
-    const uint32_t n_chunks = plan.chunks();
-    const size_t n_sub = (size_t)NF * channels;
-    const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const size_t ws_bytes = report ? selab200_verify_workspace_bytes(plan.max_frames, channels)
-                                   : selab200_decode_workspace_bytes(plan.max_frames, channels);
-    const size_t n_words = (size_t)h->info.n_words;
-    const unsigned long long w_lo = hd[(size_t)F0 * channels].refl_offset;
-    const selab200_subframe_desc &tail = hd[(size_t)(F0 + NF) * channels - 1];
-    const unsigned long long w_hi = tail.res_offset + tail.res_words;
-    const unsigned long long b_lo = container_frame_byte(F0, channels, w_lo);
-    const unsigned long long b_hi = container_frame_byte(F0 + NF, channels, w_hi);
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure((size_t)(w_hi - w_lo) * 4 + 96)) return rc;
-    for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
-        if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
-    selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
-    // 16 bytes of slack in front (the Rice decoder reads whole 16-byte vectors), the 16-byte phase of file order kept
-    uint32_t *d_arena = reinterpret_cast<uint32_t *>(static_cast<char *>(g.words.ptr) + 16 + ((w_lo * 4) & 15)) - w_lo;
-    const uint8_t *d_bytes = static_cast<const uint8_t *>(h->buf.d_bytes);
-    if (!primary) {
-        const unsigned long long b0 = b_lo & ~3ull; // the unpack kernel reads aligned 32-bit words of the byte image
-        const size_t end = std::min<size_t>(h->n_bytes, (size_t)b_hi + 4);
-        if (int rc = g.aux.ensure(end - (size_t)b0 + 64)) return rc;
-        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, h->bytes + b0, end - (size_t)b0, cudaMemcpyHostToDevice, g.s_h2d));
-        CUDA_TRY(cudaEventRecord(g.ev_h2d[0], g.s_h2d));
-        d_bytes = static_cast<const uint8_t *>(g.aux.ptr) - b0;
-    }
-    VerifyArea va;
-    if (report)
-        if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
-
-    CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
-    CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
-    for (int i = 1; i < kLanes; i++)
-        CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
-    for (uint32_t c = 0; c < n_chunks; c++) {
-        const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0; // within the block
-        const selab200_subframe_desc *dc = hd + (size_t)(F0 + f0) * channels;
-        const size_t chunk_sub = (size_t)nf * channels;
-        cudaStream_t cs = g.s_compute[c % kLanes];
-        DeviceBuffer &ws = g.lane_work[c % kLanes];
-        // descriptors go up on the chunk's own lane: s_h2d is still busy with the container bytes
-        CUDA_TRY(cudaMemcpyAsync(d_descs + (size_t)f0 * channels, dc, chunk_sub * sizeof(*dc), cudaMemcpyHostToDevice, cs));
-        if (primary) {
-            // the container bytes this chunk reads end with its last subframe (+3 bytes of slack)
-            const selab200_subframe_desc &last = dc[chunk_sub - 1];
-            const unsigned long long end_byte =
-                container_frame_byte(F0 + f0 + nf, channels, last.res_offset + last.res_words) + 3;
-            int piece = (int)(end_byte / h->piece_bytes);
-            if (piece >= h->n_pieces)
-                piece = h->n_pieces - 1;
-            CUDA_TRY(cudaStreamWaitEvent(cs, h->buf.ev_piece[piece], 0));
-        } else {
-            CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[0], 0));
-        }
-        k_container_unpack<<<(unsigned)((chunk_sub + 7) / 8), 256, 0, cs>>>(d_bytes, d_descs + (size_t)f0 * channels,
-                                                                           (uint32_t)chunk_sub, channels,
-                                                                           (unsigned long long)(F0 + f0) * channels, d_arena);
-        if (int rc = launch_check("k_container_unpack"))
-            return rc;
-        if (report) {
-            CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)(F0 + f0) * channels * kFrame,
-                                     nf * frame_bytes, cudaMemcpyHostToDevice, cs));
-            if (int rc = verify_device(d_descs + (size_t)f0 * channels, nf, channels, d_arena, n_words,
-                                       d_pcm + (size_t)f0 * channels * kFrame, va.entries + (size_t)f0 * channels,
-                                       va.count, va.status, ws.ptr, ws.bytes, cs, false, F0 + f0))
-                return rc;
-            continue;
-        }
-        if (int rc = decode_device(d_descs + (size_t)f0 * channels, nf, channels, d_arena, n_words,
-                                   d_pcm + (size_t)f0 * channels * kFrame, d_status, ws.ptr, ws.bytes, cs, false))
-            return rc;
-        CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
-        CUDA_TRY(cudaStreamWaitEvent(g.s_d2h, g.ev_done[c], 0));
-        CUDA_TRY(cudaMemcpyAsync(pcm_out + (size_t)(F0 + f0) * channels * kFrame, d_pcm + (size_t)f0 * channels * kFrame,
-                                 nf * frame_bytes, cudaMemcpyDeviceToHost, g.s_d2h));
-    }
-    if (report) {
-        for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
-            CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
-        return collect_report(va, n_sub, g.s_d2h, *report);
-    }
-    return read_status(g.s_d2h, d_status);
-}
-
-extern "C" {
-
 int selab200_container_decode(selab200_container *h, int16_t *pcm_out)
 {
     std::lock_guard<std::mutex> lock(g_mutex);
@@ -1972,13 +1935,13 @@ int selab200_container_decode(selab200_container *h, int16_t *pcm_out)
         return 0;
     if (!pcm_out)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    if (!use_all_devices(n_frames))
-        return container_decode_block(h, 0, n_frames, pcm_out, true);
-    // one block of frames per device; the primary (which holds the whole image) takes the first
-    std::vector<DevicePart> parts = device_parts(n_frames);
-    return run_on_devices(parts, [&](DevicePart &p) { return container_decode_block(h, p.f0, p.nf, pcm_out, tl_ctx == &g_slots[0]); });
+    if (int rc = check_channels(channels))
+        return rc;
+    // with several devices the primary (which holds the whole image) takes the first block
+    const CodedInput in{h->buf.h_descs, nullptr, (size_t)h->info.n_words, h};
+    return run_blocks(n_frames, [&](DevicePart &p) {
+        return decode_pipeline(in, p.f0, p.nf, channels, pcm_out, nullptr, nullptr);
+    }).rc;
 }
 
 int selab200_container_verify(selab200_container *h, const int16_t *pcm, selab200_verify_entry *entries, size_t capacity,
@@ -1995,22 +1958,15 @@ int selab200_container_verify(selab200_container *h, const int16_t *pcm, selab20
         return 0;
     if (!pcm)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
-    std::vector<selab200_verify_entry> report;
-    int rc;
-    if (!use_all_devices(n_frames)) {
-        rc = container_decode_block(h, 0, n_frames, nullptr, true, pcm, &report);
-    } else {
-        std::vector<DevicePart> parts = device_parts(n_frames);
-        rc = run_on_devices(parts, [&](DevicePart &p) {
-            return container_decode_block(h, p.f0, p.nf, nullptr, tl_ctx == &g_slots[0], pcm, &p.report);
-        });
-        report = joined_reports(parts);
-    }
-    if (rc)
+    if (int rc = check_channels(channels))
         return rc;
-    return deliver_report(report, entries, capacity, n_entries);
+    const CodedInput in{h->buf.h_descs, nullptr, (size_t)h->info.n_words, h};
+    const Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
+        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.report);
+    });
+    if (b.rc)
+        return b.rc;
+    return deliver_records(b.report, entries, capacity, n_entries);
 }
 
 int selab200_selftest(uint32_t *mismatches)
@@ -2040,8 +1996,8 @@ int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channe
         return rc;
     if (!pcm || !descs || !words || !words_used || !trace)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (channels == 0 || channels > SELAB200_MAX_CHANNELS)
-        return fail(SELAB200_ERR_ARGUMENT, "channels must be in [1, %d]", SELAB200_MAX_CHANNELS);
+    if (int rc = check_channels(channels))
+        return rc;
     *words_used = 0;
     if (n_frames == 0)
         return 0;
@@ -2057,10 +2013,11 @@ int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channe
     selab200_analysis_trace *d_trace = static_cast<selab200_analysis_trace *>(g.aux.ptr);
     CUDA_TRY(cudaMemsetAsync(d_trace, 0, n_units * sizeof(selab200_analysis_trace), g.stream));
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    EncodeOptions o;
+    o.d_trace = d_trace;
     if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
                                static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
-                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, true, nullptr,
-                               nullptr, nullptr, nullptr, 0, d_trace))
+                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaMemcpyAsync(trace, d_trace, n_units * sizeof(selab200_analysis_trace), cudaMemcpyDeviceToHost, g.stream));
