@@ -1221,7 +1221,8 @@ static void words_referenced(const selab200_subframe_desc *dc, size_t n, size_t 
     for (size_t i = 0; i < n; i++) {
         const unsigned long long a0 = dc[i].refl_offset, a1 = a0 + dc[i].refl_words;
         const unsigned long long b0 = dc[i].res_offset, b1 = b0 + dc[i].res_words;
-        if (a1 <= n_words && b1 <= n_words) { // out-of-range descriptors are rejected on the device
+        // out-of-range descriptors are rejected on the device (desc_ok), by the same wrap-free test
+        if (words_in_arena(a0, dc[i].refl_words, n_words) && words_in_arena(b0, dc[i].res_words, n_words)) {
             lo = a0 < lo ? a0 : lo;
             lo = b0 < lo ? b0 : lo;
             hi = a1 > hi ? a1 : hi;

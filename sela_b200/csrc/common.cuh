@@ -114,6 +114,27 @@ __device__ __forceinline__ void stage_17bit_row(const int32_t *src, int16_t *row
     }
 }
 
+// A stream of `words` words at word `offset` lies inside an arena of n_words words.  Written without a sum:
+// offset + words <= n_words wraps in 64 bits for offset = 2^64 - w and would accept a stream that starts in
+// front of the arena.
+__host__ __device__ __forceinline__ bool words_in_arena(unsigned long long offset, unsigned long long words,
+                                                        unsigned long long n_words)
+{
+    return words <= n_words && offset <= n_words - words;
+}
+
+// The decoder's acceptance of one subframe descriptor (frame_check in kernels.cuh adds the rules that span a
+// frame).  The host uses the same range test to decide which words a batch references.
+__host__ __device__ __forceinline__ bool desc_ok(const selab200_subframe_desc &d, uint32_t channels,
+                                                 unsigned long long n_words)
+{
+    return d.channel < channels && d.parent_channel < channels && d.subframe_type <= 1 &&
+           d.lpc_order <= kMaxOrder && d.refl_rice_param < 32 && d.res_rice_param < 32 &&
+           d.samples == kFrame && words_in_arena(d.refl_offset, d.refl_words, n_words) &&
+           words_in_arena(d.res_offset, d.res_words, n_words) &&
+           !(d.subframe_type == 1 && d.parent_channel == d.channel);
+}
+
 // Device-side status: first error wins (codes are negative, so take the min).
 __device__ __forceinline__ void raise_status(int32_t *status, int code)
 {

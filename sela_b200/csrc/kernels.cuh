@@ -736,17 +736,7 @@ __global__ void __launch_bounds__(256) k_container_unpack(const uint8_t *contain
 
 // ------------------------------------------------------------------ decode --
 
-__device__ __forceinline__ bool desc_ok(const selab200_subframe_desc &d, uint32_t channels,
-                                        unsigned long long n_words)
-{
-    return d.channel < channels && d.parent_channel < channels && d.subframe_type <= 1 &&
-           d.lpc_order <= kMaxOrder && d.refl_rice_param < 32 && d.res_rice_param < 32 &&
-           d.samples == kFrame && d.refl_offset + d.refl_words <= n_words &&
-           d.res_offset + d.res_words <= n_words &&
-           !(d.subframe_type == 1 && d.parent_channel == d.channel);
-}
-
-// Acceptance of a whole frame (its ch descriptors fd[0..ch)): every subframe passes desc_ok, the channel fields form
+// Acceptance of a whole frame (its ch descriptors fd[0..ch)): every subframe passes desc_ok (common.cuh), the channel fields form
 // a permutation and every parent is an independent subframe.
 __device__ __forceinline__ bool frame_check(const selab200_subframe_desc *fd, uint32_t ch, unsigned long long n_words)
 {

@@ -51,14 +51,6 @@ struct RiceVsParams {
     int32_t *status;
 };
 
-__device__ __forceinline__ bool rice_desc_ok(const selab200_subframe_desc &d, uint32_t channels, unsigned long long n_words)
-{
-    return d.channel < channels && d.parent_channel < channels && d.subframe_type <= 1 && d.lpc_order <= kMaxOrder &&
-           d.refl_rice_param < 32 && d.res_rice_param < 32 && d.samples == kFrame &&
-           d.refl_offset + d.refl_words <= n_words && d.res_offset + d.res_words <= n_words &&
-           !(d.subframe_type == 1 && d.parent_channel == d.channel);
-}
-
 // Position of the highest set bit, 0xffffffff for zero: the raw FLO, without the 31 - x of __clz.
 __device__ __forceinline__ uint32_t bfind_u32(uint32_t x)
 {
@@ -460,7 +452,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_split_index(RiceVsParams
     if (exists)
         d = p.descs[st];
     // splittable: well-formed and every lane gets at least four words
-    const bool ok = exists && rice_desc_ok(d, p.channels, p.n_words) && d.res_words >= 4u * S;
+    const bool ok = exists && desc_ok(d, p.channels, p.n_words) && d.res_words >= 4u * S;
     const uintptr_t addr = reinterpret_cast<uintptr_t>(p.words + (ok ? d.res_offset : 0));
     const uint32_t skip = (uint32_t)(addr >> 2) & 3u;
     const uint32_t total = ok ? (uint32_t)d.res_words + skip : 0u; // words from the aligned base
@@ -761,7 +753,7 @@ __global__ void __launch_bounds__(32 * kVsWarps) k_rice_decode_vc(RiceVsParams p
     memset(&d, 0, sizeof d);
     if (exists)
         d = p.descs[st];
-    bool ok = exists && rice_desc_ok(d, p.channels, p.n_words);
+    bool ok = exists && desc_ok(d, p.channels, p.n_words);
     if (exists && !ok && l == 0)
         raise_status(p.status, SELAB200_ERR_BITSTREAM);
     const bool store_row = ok; // rows of flagged streams may hold garbage: the general kernel rewrites them

@@ -75,6 +75,8 @@ class Oracle:
         L.sela_oracle_time_encode.restype = C.c_double
         L.sela_oracle_time_decode.restype = C.c_double
         L.sela_oracle_rice_encode.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]
+        # (without argtypes ctypes passes a Python int as a C int: a pointer above 2^32 would be truncated)
+        L.sela_oracle_rice_size.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         L.sela_oracle_rice_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p]
         L.sela_oracle_lpc_analyse.argtypes = [C.c_void_p, C.c_size_t] + [C.c_void_p] * 6
         L.sela_oracle_lpc_synthesise.argtypes = [C.c_void_p, C.c_size_t, C.c_uint8, C.c_void_p, C.c_void_p]

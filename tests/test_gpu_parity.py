@@ -196,23 +196,107 @@ def test_frames_edge_signals_stereo(O):
     assert np.array_equal(sela_b200.decode_frames(d, w, 2), pcm.reshape(-1))
 
 
+def _malformed_base(O):
+    """Two stereo frames whose fields sit at the limits the decoder accepts: an order-100 subframe, a difference
+    subframe, an order-0 subframe with a k = 31 residue stream of random bits and an order-1 subframe with a k = 31
+    reflection stream."""
+    import crafted as CR
+    import rice_families as RF
+    P = ol.load("port")
+    rng = np.random.default_rng(12)
+    a = CR.crafted_subframe(P, rng, 100, "small", channel=1)
+    b = CR.difference_subframe(P, rng, 2, a, channel=0)
+    d = CR.crafted_subframe(P, rng, 1, "small", channel=1)
+    refl = lambda s, k: (k, CR.pack_stream(CR.zigzag(s.q), k))
+    k31 = next(s for s in RF.family("random") if s[0] == 31)
+    subs = [dict(channel=1, order=100, refl=refl(a, 6), res=CR.rice_code(P, a.res)),
+            dict(channel=0, type=1, parent=1, order=2, refl=refl(b, 3), res=CR.rice_code(P, b.res)),
+            dict(channel=0, order=0, refl=(0, np.zeros(0, np.uint32)), res=k31),
+            dict(channel=1, order=1, refl=refl(d, 31), res=CR.rice_code(P, d.res))]
+    return RF.layout(subs, 2)
+
+
+def _to_end(descs, words, i, name, cut=0):
+    """Stream `name` of subframe i moved to the end of the arena (offset + words == n_words), minus `cut` words."""
+    d, w = descs.copy(), words
+    at, n = int(d[name + "_offset"][i]), int(d[name + "_words"][i])
+    w = np.concatenate([w, np.full(2, 0xFFFFFFFF, np.uint32), w[at:at + n]])
+    d[name + "_offset"][i] = w.size - n
+    return d, w[:w.size - cut]
+
+
+def _edit(**fields):
+    def f(d, w):
+        d = d.copy()
+        for key, (i, v) in fields.items():
+            d[key][i] = v
+        return d, w
+    return f
+
+
+MALFORMED = [
+    ("at the limits", _edit()),
+    ("order 101", _edit(lpc_order=(0, 101))),
+    ("residue k 32", _edit(res_rice_param=(2, 32))),
+    ("residue k 40", _edit(res_rice_param=(1, 40))),
+    ("reflection k 32", _edit(refl_rice_param=(3, 32))),
+    ("residue at the arena's end", lambda d, w: _to_end(d, w, 2, "res")),
+    ("residue one word past it", lambda d, w: _to_end(d, w, 2, "res", 1)),
+    ("reflection at the arena's end", lambda d, w: _to_end(d, w, 0, "refl")),
+    ("reflection one word past it", lambda d, w: _to_end(d, w, 0, "refl", 1)),
+    ("channel = channels", _edit(channel=(2, 2))),
+    ("channel 7", _edit(channel=(1, 7))),
+    ("parent = channels", _edit(parent_channel=(1, 2))),
+    ("duplicate channel", _edit(channel=(3, 0))),
+    ("difference of a difference", _edit(subframe_type=(0, 1), parent_channel=(0, 0))),
+    ("difference of itself", _edit(parent_channel=(1, 0))),
+    ("subframe type 2", _edit(subframe_type=(2, 2))),
+    ("samples 2047", _edit(samples=(0, 2047))),
+    ("samples 100", _edit(samples=(1, 100))),
+    ("residue offset 2^40", _edit(res_offset=(1, 1 << 40))),
+    ("residue offset 2^64 - 1", _edit(res_offset=(2, (1 << 64) - 1))),
+    ("residue offset 2^64 - words", lambda d, w: _edit(res_offset=(2, (1 << 64) - int(d["res_words"][2])))(d, w)),
+    ("reflection offset 2^64 - words",
+     lambda d, w: _edit(refl_offset=(0, (1 << 64) - int(d["refl_words"][0])))(d, w)),
+    ("truncated arena", lambda d, w: (d, w[:w.size // 2])),
+]
+
+
 def test_decode_rejects_malformed(O):
-    pcm = synth.sine_noise(44100, 2, n_frames=2, seed=4)
-    d, w = sela_b200.encode_frames(pcm, 2)
-    for field, value in [("lpc_order", 101), ("res_rice_param", 40), ("channel", 7), ("samples", 100),
-                         ("res_offset", 1 << 40)]:
-        bad = d.copy()
-        bad[field][1] = value
+    """Every descriptor rule at its limit and one past it, and offsets that wrap in 64 bits, through decode_frames,
+    verify_frames, decode_frames_device and rice_decode_frames_device: the exact model's acceptance predicate
+    (tests/exact_rice.py) decides between the reference's output and SELAB200_ERR_BITSTREAM."""
+    base = _malformed_base(O)
+    for case, edit in MALFORMED:
+        _check_malformed(O, case, *edit(*base))
+
+
+def _check_malformed(O, case, descs, words):
+    import exact_rice as XR
+    from gpu_calls import decode_frames_device
+    from sela_b200.device import rice_decode_frames
+    if XR.accepts(descs, words, 2):
+        want = O.decode_frames(descs, words, 2)
+        assert np.array_equal(sela_b200.decode_frames(descs, words, 2), want), case
+        assert sela_b200.verify_frames(descs, words, 2, want).size == 0, case
+        assert np.array_equal(decode_frames_device(descs, words, 2), want), case
+    else:
+        assert case != "at the limits"
+        for call in (lambda: sela_b200.decode_frames(descs, words, 2),
+                     lambda: sela_b200.verify_frames(descs, words, 2, np.zeros(descs.size * FRAME, np.int16)),
+                     lambda: decode_frames_device(descs, words, 2)):
+            with pytest.raises(sela_b200.SelaB200Error) as e:
+                call()
+            assert e.value.status == -6, case
+    if XR.accepts(descs, words, 2, frames=False):
+        res, _ = rice_decode_frames(descs, words, 2)
+        want, _ = XR.parse_batch([(int(d["res_rice_param"]), words[int(d["res_offset"]):][:int(d["res_words"])])
+                                  for d in descs], FRAME)
+        assert np.array_equal(res, want), case
+    else:
         with pytest.raises(sela_b200.SelaB200Error) as e:
-            sela_b200.decode_frames(bad, w, 2)
-        assert e.value.status == -6
-    dup = d.copy()
-    dup["channel"][1] = dup["channel"][0]
-    with pytest.raises(sela_b200.SelaB200Error):
-        sela_b200.decode_frames(dup, w, 2)
-    # truncated arena: must not fault, must report
-    with pytest.raises(sela_b200.SelaB200Error):
-        sela_b200.decode_frames(d, w[: w.size // 2], 2)
+            rice_decode_frames(descs, words, 2)
+        assert e.value.status == -6, case
 
 
 def test_encode_capacity_error():

@@ -8,6 +8,7 @@ import pytest
 import oracle_lib as ol
 import sela_b200
 from crafted import pack_stream, zigzag
+from rice_families import synthetic_streams
 from sela_b200 import _lib, synth
 from sela_b200.device import rice_decode_frames
 
@@ -48,36 +49,6 @@ def build_batch(streams, channels=1, gap_words=(0, 1, 2, 3, 5)):
         arena.append(w)
         at += w.size
     return descs, np.concatenate(arena)
-
-
-def synthetic_streams(rng):
-    out = []
-    lap = lambda scale: np.round(rng.laplace(0, scale, FRAME)).astype(np.int64)
-    # the BASELINE regime (k ~ 11) and its neighbours, chosen k around the optimum and away from it
-    for scale, k in [(900, 10), (900, 11), (900, 12), (60, 5), (60, 7), (3, 1), (3, 2), (0.3, 0), (20000, 15), (20000, 13)]:
-        out.append((k, zigzag(lap(scale))))
-    # silence and constants: periodic streams in which a wrong-phase parse may never resynchronise
-    out.append((0, zigzag(np.zeros(FRAME))))
-    out.append((10, zigzag(np.full(FRAME, 1234))))
-    out.append((3, zigzag(np.full(FRAME, -5))))
-    out.append((6, zigzag(np.tile([37, -37], FRAME // 2))))
-    out.append((11, zigzag(np.tile([1000, 1001, -999], FRAME // 3 + 1)[:FRAME])))
-    # outliers: a few symbols longer than one 32-bit window, and very long runs
-    v = lap(500); v[[5, 700, 701, 2047]] = [40000, -60000, 90000, -120000]; out.append((9, zigzag(v)))
-    v = lap(30); v[::97] = 5000; out.append((4, zigzag(v)))
-    v = lap(2); v[1000] = 3000; out.append((0, zigzag(v)))
-    v = lap(800); v[256 * np.arange(1, 8)] = 70000; out.append((10, zigzag(v)))   # long symbols AT the part boundaries
-    v = lap(800); v[256 * np.arange(1, 8) - 1] = -70000; out.append((10, zigzag(v)))
-    # loud then quiet: parts with very different bit densities
-    v = np.concatenate([lap(8000)[:300], lap(3)[:FRAME - 300]]); out.append((4, zigzag(v)))
-    v = np.concatenate([lap(2)[:1800], lap(6000)[:248]]); out.append((3, zigzag(v)))
-    # k extremes
-    out.append((19, zigzag(rng.integers(-(1 << 19), 1 << 19, FRAME))))
-    out.append((24, zigzag(rng.integers(-(1 << 23), 1 << 23, FRAME))))
-    out.append((31, rng.integers(0, 1 << 31, FRAME).astype(np.uint64)))
-    # full-scale noise: the longest streams 16-bit audio produces
-    out.append((16, zigzag(rng.integers(-65535, 65536, FRAME))))
-    return [(k, pack_stream(us, k), us) for k, us in out]
 
 
 @pytest.mark.parametrize("split", SPLITS)
