@@ -339,7 +339,9 @@ int selab200_lpc_samples(const int32_t *residues, uint32_t n_sub, const uint8_t 
  * independent inputs.  values: [n_streams][stride] int32, counts[i] <= stride
  * <= 2048 used from row i.  Outputs per stream: rice_param, n_words, and the
  * words at words[i*words_stride ...]; SELAB200_ERR_CAPACITY if a stream needs
- * more than words_stride words (n_words[] still holds the required sizes). */
+ * more than words_stride words (n_words[] still holds the required sizes). After
+ * SELAB200_ERR_CAPACITY, rice_param[] holds every stream's parameter and every
+ * stream that fits has its words; the rows of the others are undefined. */
 int selab200_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t n_streams,
                          uint32_t stride, uint32_t *rice_param, uint32_t *n_words,
                          uint32_t *words, uint32_t words_stride);

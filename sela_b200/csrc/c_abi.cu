@@ -502,8 +502,12 @@ int launch_rice_residues(const DecodeParams &p, void *aux, cudaStream_t stream)
 {
     const size_t n_sub = (size_t)p.n_frames * p.channels;
     const int log2s = rice_split_log2(n_sub);
-    if (log2s < 0 || (reinterpret_cast<uintptr_t>(p.ws_res) & 15) != 0)
+    if (log2s < 0 || (reinterpret_cast<uintptr_t>(p.ws_res) & 15) != 0) {
+        // the general parser alone: nothing is flagged.  Zero the flags that selab200_rice_decode_flagged counts,
+        // which would otherwise count whatever the last call that used this scratch left there.
+        CUDA_TRY(cudaMemsetAsync(static_cast<uint32_t *>(aux) + n_sub * 15, 0, n_sub * 4, stream));
         return launch_rice_decode(p, 1, stream);
+    }
     RiceVsParams q;
     q.descs = p.descs;
     q.n_sub = (uint32_t)n_sub;

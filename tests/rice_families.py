@@ -20,7 +20,7 @@ import functools
 import numpy as np
 
 import exact_rice as XR
-from crafted import pack_stream, zigzag
+from exact_rice import pack_stream, zigzag
 from oracle_lib import DESC_DTYPE
 
 FRAME = 2048

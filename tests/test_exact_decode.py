@@ -6,6 +6,7 @@ import pytest
 
 import crafted as CR
 import exact_decode as X
+import exact_rice as XR
 import oracle_lib as ol
 
 FRAME = 2048
@@ -100,7 +101,7 @@ def test_rice_code_matches_reference_encoder_and_decodes_every_int32(P):
     rng = np.random.default_rng(3)
     x = rng.integers(-(1 << 20), 1 << 20, FRAME)
     k, w = CR.rice_code(P, x)
-    assert np.array_equal(CR.pack_stream(CR.zigzag(x), k), w)          # both paths lay out the same bits
+    assert np.array_equal(XR.pack_stream(XR.zigzag(x), k), w)          # both paths lay out the same bits
     x[[0, 5, 700, 2047]] = [X.I32_MIN, X.I32_MAX, X.I32_MIN + 1, -(1 << 30)]
     k, w = CR.rice_code(P, x)
     assert np.array_equal(P.rice_decode(w, k, FRAME), x)

@@ -6,10 +6,12 @@ import pytest
 
 import exact_rice as XR
 import oracle_lib as ol
+import rice_encode_families as REF
 import rice_families as RF
-from crafted import pack_stream
+from exact_rice import pack_stream
 
 FRAME = 2048
+I32_MIN, I32_MAX = -(1 << 31), (1 << 31) - 1
 WHICH = ["port", pytest.param("ref", marks=pytest.mark.ref)]
 
 
@@ -98,6 +100,50 @@ def test_families_reach_what_they_claim():
     assert all(40000 <= w.size <= 0xFFFF for _, w in RF.family("long"))
     _, bits = XR.parse_batch(RF.family("short"), FRAME)
     assert (bits > 32 * np.array([w.size for _, w in RF.family("short")])).all()
+
+
+# ------------------------------------------------------------------------------------------- encoder --
+
+@pytest.mark.parametrize("which", WHICH)
+@pytest.mark.parametrize("name", REF.NAMES)
+def test_encoder_model_equals_reference_encoder(name, which):
+    """(k, words) of the encoder model on every stream of every family that lies in the reference's domain
+    (|x| < 2^30), against rice::RiceEncoder."""
+    O = ol.load(which)
+    n = 0
+    for b in REF.family(name):
+        for i in REF.in_reference_domain(b):
+            k, w = O.rice_encode(b.values[i, :b.counts[i]])
+            assert (k, w.size) == (b.enc.k[i], b.enc.n_words[i]), (name, i)
+            assert np.array_equal(w, b.enc.words[i]), (name, i)
+            n += 1
+    assert n >= (6 if name == "extremes" else 20), n                      # extremes: the +-(2^30 - 1) streams
+
+
+@pytest.mark.parametrize("name", REF.NAMES)
+def test_encoder_model_round_trips(name):
+    """Every family (each builder asserts its own property through the model) parses back to its values with the
+    parse model, ending on the encoder's last bit; the totals are the textbook sums."""
+    for b in REF.family(name):
+        values, bits = XR.parse_batch(list(zip(b.enc.k, b.enc.words)), b.counts)
+        for i, c in enumerate(b.counts):
+            assert np.array_equal(values[i, :c], b.values[i, :c]), (name, i)
+        assert np.array_equal(bits, b.enc.bits)
+        assert np.array_equal(b.enc.n_words, [w.size for w in b.enc.words])
+        for i in range(0, len(b.counts), 97):
+            us = [int(u) for u in XR.zigzag(b.values[i, :b.counts[i]])]
+            assert [sum(u >> k for u in us) + len(us) * (1 + k) for k in range(20)] == b.enc.totals[i].tolist()
+
+
+def test_encoder_model_search_and_layout():
+    """The first arg-min wins a tie; zig-zag in the uint32 domain; the layout, bit by bit."""
+    assert XR.encode([1, 1])[0] == 0                                      # u = 2: totals 6, 6, 8, ...
+    assert XR.encode([])[0] == 0 and XR.encode([])[1].size == 0
+    assert XR.zigzag([0, -1, 1, I32_MIN, I32_MAX]).tolist() == [0, 1, 2, (1 << 32) - 1, (1 << 32) - 2]
+    k, w = XR.encode([3, -2, 0])                                         # u = 6, 3, 0: totals 12, 10, 10, 12
+    assert k == 1
+    bits = "111" "0" "0" + "1" "0" "1" + "0" "0"                         # q ones, a zero, the payload bit
+    assert w.tolist() == [int(bits[::-1], 2)]
 
 
 def test_acceptance_predicate():

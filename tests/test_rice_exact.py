@@ -115,6 +115,18 @@ def test_values_every_family(model, monkeypatch, split):
         assert flagged[name] <= bound, (name, split, S[name], flagged)
 
 
+def test_general_parser_alone_flags_nothing(model, monkeypatch):
+    """With the general parser alone (S = 0) no stream is flagged, whatever the scratch the flags live in held
+    before: a stage-level encode of 1 024 streams first leaves its non-zero counts there (the flag count once
+    reported them)."""
+    vals = np.random.default_rng(1).integers(1, 1 << 20, (1024, FRAME)).astype(np.int32)
+    sela_b200.rice_encode(vals)
+    _split(monkeypatch, "0")
+    s, v, _ = model["random"]
+    res, flagged = rice_decode_frames(*RF.layout(_res(s)), 1)
+    assert flagged == 0 and np.array_equal(res, v)
+
+
 def exact_end_streams(rng):
     """Random symbols at every k, the last one lengthened so that the stream ends on the last bit of its last word."""
     out = []
@@ -263,10 +275,10 @@ def test_reflection_streams():
         for k in {order % 32, (order + 11) % 32, (order + 22) % 32}:
             q = CR.draw_q(rng, order)
             r = rng.integers(-300, 301, FRAME).astype(np.int32)
-            w = CR.pack_stream(CR.zigzag(q), k)
+            w = XR.pack_stream(XR.zigzag(q), k)
             if len(subs) % 2:
                 w = np.concatenate([w, rng.integers(0, 1 << 32, 1 + len(subs) % 5, dtype=np.uint64).astype(np.uint32)])
-            subs.append(dict(order=order, refl=(k, w), res=(9, CR.pack_stream(CR.zigzag(r), 9))))
+            subs.append(dict(order=order, refl=(k, w), res=(9, XR.pack_stream(XR.zigzag(r), 9))))
             crafted.append(CR.Sub(0, 0, 0, order, q, r))
     assert {s["refl"][0] for s in subs} == set(range(32))
     descs, arena = RF.layout(subs)
@@ -280,7 +292,7 @@ def test_reflection_streams():
         by_k.setdefault(s["refl"][0], i)
     for k, i in sorted(by_k.items()):
         kk, w = subs[i]["refl"]
-        need = -(-XR.code_bits(CR.zigzag(crafted[i].q), kk) // 32)
+        need = -(-XR.code_bits(XR.zigzag(crafted[i].q), kk) // 32)
         bad = list(subs[:130])
         bad.insert(k * 4 % 130, dict(subs[i], refl=(kk, w[:need - 1])))
         descs, arena = RF.layout(bad)

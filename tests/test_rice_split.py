@@ -7,7 +7,7 @@ import pytest
 
 import oracle_lib as ol
 import sela_b200
-from crafted import pack_stream, zigzag
+from exact_rice import pack_stream, zigzag
 from rice_families import synthetic_streams
 from sela_b200 import _lib, synth
 from sela_b200.device import rice_decode_frames
