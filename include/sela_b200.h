@@ -392,6 +392,30 @@ int selab200_quantise_probe(const double *k, size_t n, int32_t *out);
 int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
                        int32_t *residues);
 
+/* For tests: selab200_fir_probe through the instantiation of the FIR that the lossless encode runs, which also tests
+ * every output for a tie: (int32)((2^34 + sum) >> 35) + (int32)((2^34 - sum) >> 35) != 0, both sums taken mod
+ * 2^64 (DESIGN.md 7.2).  Arguments and domain as selab200_fir_probe; ties[n] receives 1 for a signal with a tie
+ * at any output, else 0. */
+int selab200_fir_tie_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                           int32_t *residues, uint8_t *ties);
+
+/* A quantised predictor: the order and the quantised reflection coefficients, zero past the order. */
+typedef struct selab200_predictor { /* 404 bytes */
+    int32_t order;   /* 0..100 */
+    int32_t q[100];  /* [-64, 63] */
+} selab200_predictor;
+
+/* For tests: selab200_encode_frames_lossless on one device and one batch, except that every analysis unit is coded
+ * with the predictor pred[unit] instead of the one its analysis chooses.  pred holds one record per analysis unit,
+ * in the order of selab200_encode_trace's.  Everything after the quantiser runs as in the lossless encode: the tie
+ * test, the repair (whose candidates edit the given predictor), the stereo decision and the report.  A predictor
+ * outside the domain (order, q or a non-zero q past the order) -> SELAB200_ERR_RANGE.  The other arguments as
+ * selab200_encode_frames_lossless. */
+int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                    const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                    size_t words_capacity, size_t *words_used, selab200_lossless_entry *entries,
+                                    size_t entries_capacity, size_t *n_entries);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,6 +51,10 @@ LOSSLESS_DTYPE = np.dtype([
 ], align=True)
 assert LOSSLESS_DTYPE.itemsize == 16
 
+# mirrors selab200_predictor, 404 bytes
+PREDICTOR_DTYPE = np.dtype([("order", "<i4"), ("q", "<i4", (100,))], align=True)
+assert PREDICTOR_DTYPE.itemsize == 404
+
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
 
@@ -107,6 +111,8 @@ _SIGNATURES = {
     "selab200_encode_trace": (_I, [_V, _U32, _U32, _V, _V, _SZ, _V, _V]),
     "selab200_quantise_probe": (_I, [_V, _SZ, _V]),
     "selab200_fir_probe": (_I, [_V, _V, _V, _U32, _I, _V]),
+    "selab200_fir_tie_probe": (_I, [_V, _V, _V, _U32, _I, _V, _V]),
+    "selab200_encode_lossless_forced": (_I, [_V, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _SZ, _V]),
 }
 
 

@@ -19,8 +19,9 @@ error behaviour as in include/sela_b200.h):
                                     not in the reference: encodes that decode back to their source, re-coding
                                     the few subframes the reference decoder would not reproduce (DESIGN.md 7.2)
     encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
-    / fir_probe                     order threshold and quantiser on chosen values, and its FIR residual
-                                    on chosen signals and predictors
+    / fir_probe / fir_tie_probe     order threshold and quantiser on chosen values, its FIR residual
+                                    (and tie test) on chosen signals and predictors, and the lossless
+    encode_lossless_forced          encode with chosen predictors
 
 Everything computes on the GPU through the C ABI; NumPy only carries host buffers.
 The C++ mirror of the same interface (data::, frame::, file::, sela:: classes and
@@ -31,8 +32,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, LOSSLESS_DTYPE, MAX_ORDER, TRACE_DTYPE, VERIFY_DTYPE, SelaB200Error,  # noqa: F401
-                   check, init, lib)
+from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, LOSSLESS_DTYPE, MAX_ORDER, PREDICTOR_DTYPE, TRACE_DTYPE,  # noqa: F401
+                   VERIFY_DTYPE, SelaB200Error, check, init, lib)
 
 
 def _c(a, dtype):
@@ -100,6 +101,50 @@ def fir_probe(samples, orders, c, wide, device=0):
     check(lib().selab200_fir_probe(samples.ctypes.data, orders.ctypes.data, c.ctypes.data, n, int(bool(wide)),
                                    res.ctypes.data))
     return res
+
+
+def fir_tie_probe(samples, orders, c, wide, device=0):
+    """fir_probe through the lossless encode's FIR, which also tests every output for a tie -> (residues int32
+    [n, 2048], ties bool[n]: whether any output of the signal ties)."""
+    init(device)
+    samples = _c(samples, np.int32).reshape(-1, FRAME)
+    n = samples.shape[0]
+    orders = _c(orders, np.int32).reshape(n)
+    c = _c(c, np.int64).reshape(n, MAX_ORDER + 1)
+    res = np.zeros((n, FRAME), np.int32)
+    ties = np.zeros(max(n, 1), np.uint8)
+    check(lib().selab200_fir_tie_probe(samples.ctypes.data, orders.ctypes.data, c.ctypes.data, n, int(bool(wide)),
+                                       res.ctypes.data, ties.ctypes.data))
+    return res, ties[:n].astype(bool)
+
+
+def encode_lossless_forced(pcm, channels, predictors, device=0):
+    """encode_frames_lossless on one batch, every analysis unit coded with its predictor from `predictors`
+    (PREDICTOR_DTYPE[n_units], or a sequence of (order, q) pairs, in encode_trace's unit order) instead of its
+    analysis' -> (descs, words, report)."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    n_units = n_frames * (3 if channels == 2 else channels)
+    if isinstance(predictors, np.ndarray) and predictors.dtype == PREDICTOR_DTYPE:
+        pred = _c(predictors, PREDICTOR_DTYPE)
+    else:
+        pred = np.zeros(len(predictors), PREDICTOR_DTYPE)
+        for rec, (order, q) in zip(pred, predictors):
+            rec["order"] = order
+            rec["q"][:order] = np.asarray(q)[:order]
+    if pred.size != n_units:
+        raise ValueError("%d predictors for %d analysis units" % (pred.size, n_units))
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used = C.c_size_t(0)
+    report = np.zeros(max(n_frames * channels, 1), LOSSLESS_DTYPE)
+    n = C.c_size_t(0)
+    check(L.selab200_encode_lossless_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
+                                            words.ctypes.data, cap, C.addressof(used), report.ctypes.data, report.size,
+                                            C.addressof(n)))
+    return descs, words[:used.value].copy(), report[:n.value].copy()
 
 
 def decode_frames(descs, words, channels, device=0):

@@ -304,38 +304,40 @@ int launch_unit_means(const void *src, size_t n_units, uint32_t channels, double
     return launch_check("k_unit_means");
 }
 
-// k_encode_units<STEREO, TRACE, CHECK>, a warp per analysis unit.
-template <bool STEREO, bool TRACE, bool CHECK = false>
-int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis_trace *d_trace, cudaStream_t stream)
+// k_encode_units<STEREO, TRACE, CHECK, FORCE>, a warp per analysis unit.
+template <bool STEREO, bool TRACE, bool CHECK = false, bool FORCE = false>
+int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis_trace *d_trace, cudaStream_t stream,
+                        const selab200_predictor *d_pred = nullptr)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_encode_units<STEREO, TRACE, CHECK>, smem))
+    if (int rc = set_smem(k_encode_units<STEREO, TRACE, CHECK, FORCE>, smem))
         return rc;
-    k_encode_units<STEREO, TRACE, CHECK><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace);
+    k_encode_units<STEREO, TRACE, CHECK, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace, d_pred);
     return launch_check("k_encode_units");
 }
 
 // The lossless repair between k_encode_units<S, false, true> and the scan (lossless.cuh).  Every launch has a grid
 // of a fixed size: nothing here depends on what the check found.  The warp kernels use at most one residue row
-// per unit of the batch.
-template <bool STEREO>
-int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream)
+// per unit of the batch.  FORCE: the units' predictors are d_pred's (selab200_encode_lossless_forced).
+template <bool STEREO, bool FORCE = false>
+int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream,
+                  const selab200_predictor *d_pred = nullptr)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_lossless_candidates<STEREO>, smem))
+    if (int rc = set_smem(k_lossless_candidates<STEREO, FORCE>, smem))
         return rc;
-    if (int rc = set_smem(k_lossless_repack<STEREO>, smem))
+    if (int rc = set_smem(k_lossless_repack<STEREO, FORCE>, smem))
         return rc;
     k_lossless_select<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, r);
     if (int rc = launch_check("k_lossless_select"))
         return rc;
     const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
     for (int round = 0; round < 2; round++) {
-        k_lossless_candidates<STEREO><<<warps, 32, smem, stream>>>(p, r, round);
+        k_lossless_candidates<STEREO, FORCE><<<warps, 32, smem, stream>>>(p, r, round, d_pred);
         if (int rc = launch_check("k_lossless_candidates"))
             return rc;
     }
-    k_lossless_repack<STEREO><<<warps, 32, smem, stream>>>(p, r);
+    k_lossless_repack<STEREO, FORCE><<<warps, 32, smem, stream>>>(p, r, d_pred);
     if (int rc = launch_check("k_lossless_repack"))
         return rc;
     k_lossless_report<<<(unsigned)std::min((n_frames + 255) / 256, (size_t)g.sms), 256, 0, stream>>>(p, r);
@@ -364,6 +366,7 @@ struct EncodeOptions {
     unsigned long long sub_base = 0;            // ... where the batch's first subframe is subframe sub_base
     selab200_analysis_trace *d_trace = nullptr; // the tracing unit kernel writes every unit's analysis here
     const LosslessArgs *lossless = nullptr;     // encode lossless (DESIGN.md 7.2) and report the re-coded pairs
+    const selab200_predictor *d_pred = nullptr; // lossless only: every unit's predictor (selab200_encode_lossless_forced)
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -413,12 +416,21 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         r.n_entries = o.lossless->n_entries;
         r.frame_base = o.lossless->frame_base;
         CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
-        if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
-                            : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
-            return rc;
-        if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream)
-                            : launch_repair<false>(p, r, n_frames, n_units, stream))
-            return rc;
+        if (o.d_pred) {
+            if (int rc = stereo ? launch_encode_units<true, false, true, true>(p, n_units, nullptr, stream, o.d_pred)
+                                : launch_encode_units<false, false, true, true>(p, n_units, nullptr, stream, o.d_pred))
+                return rc;
+            if (int rc = stereo ? launch_repair<true, true>(p, r, n_frames, n_units, stream, o.d_pred)
+                                : launch_repair<false, true>(p, r, n_frames, n_units, stream, o.d_pred))
+                return rc;
+        } else {
+            if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
+                                : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
+                return rc;
+            if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream)
+                                : launch_repair<false>(p, r, n_frames, n_units, stream))
+                return rc;
+        }
     } else {
         const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
                                                  : launch_encode_units<true, false>(p, n_units, nullptr, stream))
@@ -1041,6 +1053,7 @@ int selab200_rice_decode_flagged(uint32_t *n_flagged)
 
 static_assert(sizeof(selab200_analysis_trace) == 2832, "selab200_analysis_trace layout (include/sela_b200.h)");
 static_assert(sizeof(selab200_lossless_entry) == 16, "selab200_lossless_entry layout (include/sela_b200.h)");
+static_assert(sizeof(selab200_predictor) == 404, "selab200_predictor layout (include/sela_b200.h)");
 
 // Bytes of container in front of frame f when `words` Rice words precede it.
 static unsigned long long container_frame_byte(unsigned long long f, uint32_t channels, unsigned long long words)
@@ -2063,10 +2076,79 @@ int selab200_quantise_probe(const double *k, size_t n, int32_t *out)
     return 0;
 }
 
-int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
-                       int32_t *residues)
+// For tests: one unpipelined lossless batch through encode_device, every unit coded with its predictor from pred.
+int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                    const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                    size_t words_capacity, size_t *words_used, selab200_lossless_entry *entries,
+                                    size_t entries_capacity, size_t *n_entries)
 {
     std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !pred || !descs || !words || !words_used || (!entries && entries_capacity) || !n_entries)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    *words_used = 0;
+    *n_entries = 0;
+    if (n_frames == 0)
+        return 0;
+    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
+    for (size_t u = 0; u < n_units; u++) {
+        const int o = pred[u].order;
+        if (o < 0 || o > kMaxOrder)
+            return fail(SELAB200_ERR_RANGE, "order %d of unit %zu outside 0..%d", o, u, kMaxOrder);
+        for (int i = 0; i < kMaxOrder; i++)
+            if (i < o ? pred[u].q[i] < -64 || pred[u].q[i] > 63 : pred[u].q[i] != 0)
+                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of unit %zu (order %d) outside [-64, 63], or not zero "
+                            "past the order", i, pred[u].q[i], u, o);
+    }
+    const size_t ws_bytes = selab200_encode_lossless_workspace_bytes(n_frames, channels);
+    const size_t rec_bytes = 256 + n_sub * sizeof(selab200_lossless_entry);
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
+    if (int rc = g.work.ensure(ws_bytes)) return rc;
+    if (int rc = g.aux.ensure(n_units * sizeof(selab200_predictor))) return rc;
+    if (int rc = g.lossless.ensure(rec_bytes)) return rc;
+    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
+    const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
+    unsigned long long *d_count = static_cast<unsigned long long *>(g.lossless.ptr);
+    selab200_lossless_entry *d_entries =
+        reinterpret_cast<selab200_lossless_entry *>(static_cast<char *>(g.lossless.ptr) + 256);
+    CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, rec_bytes, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    const LosslessArgs la{d_entries, d_count, 0};
+    EncodeOptions o;
+    o.lossless = &la;
+    o.d_pred = d_pred;
+    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
+                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
+                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    uint64_t used;
+    memcpy(&used, g.h_small + 2, 8);
+    *words_used = (size_t)used;
+    if (g.h_small[0] != 0)
+        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (used > words_capacity)
+        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
+    std::vector<selab200_lossless_entry> rec;
+    if (int rc = collect_records(d_count, nullptr, d_entries, n_sub, g.stream, rec))
+        return rc;
+    return deliver_records(rec, entries, entries_capacity, n_entries);
+}
+
+// selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).
+static int fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                     int32_t *residues, uint8_t *ties)
+{
     if (int rc = require_ready())
         return rc;
     if (!samples || !orders || !c || !residues)
@@ -2083,19 +2165,44 @@ int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int6
     const size_t sig = (size_t)n * kFrame * 4, cb = (size_t)n * (kMaxOrder + 1) * 8;
     if (int rc = g.in.ensure(sig)) return rc;
     if (int rc = g.work.ensure(sig)) return rc;
-    if (int rc = g.aux.ensure(cb + (size_t)n * 4)) return rc;
+    if (int rc = g.aux.ensure(cb + (size_t)n * 5)) return rc;
     long long *d_c = static_cast<long long *>(g.aux.ptr);
     int32_t *d_orders = reinterpret_cast<int32_t *>(d_c + (size_t)n * (kMaxOrder + 1));
+    uint8_t *d_ties = reinterpret_cast<uint8_t *>(d_orders + n);
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, samples, sig, cudaMemcpyHostToDevice, g.stream));
     CUDA_TRY(cudaMemcpyAsync(d_c, c, cb, cudaMemcpyHostToDevice, g.stream));
     CUDA_TRY(cudaMemcpyAsync(d_orders, orders, (size_t)n * 4, cudaMemcpyHostToDevice, g.stream));
-    k_fir_probe<<<n, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_orders, d_c, wide,
-                                        static_cast<int32_t *>(g.work.ptr));
+    if (ties)
+        k_fir_probe<true><<<n, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_orders, d_c, wide,
+                                                  static_cast<int32_t *>(g.work.ptr), d_ties);
+    else
+        k_fir_probe<<<n, 32, 0, g.stream>>>(static_cast<const int32_t *>(g.in.ptr), d_orders, d_c, wide,
+                                            static_cast<int32_t *>(g.work.ptr), nullptr);
     if (int rc = launch_check("k_fir_probe"))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(residues, g.work.ptr, sig, cudaMemcpyDeviceToHost, g.stream));
+    if (ties)
+        CUDA_TRY(cudaMemcpyAsync(ties, d_ties, n, cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaStreamSynchronize(g.stream));
     return 0;
+}
+
+int selab200_fir_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                       int32_t *residues)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    return fir_probe(samples, orders, c, n, wide, residues, nullptr);
+}
+
+int selab200_fir_tie_probe(const int32_t *samples, const int32_t *orders, const int64_t *c, uint32_t n, int wide,
+                           int32_t *residues, uint8_t *ties)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!ties)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    return fir_probe(samples, orders, c, n, wide, residues, ties);
 }
 
 // ---------------------------------------------------------------- stages --

@@ -240,9 +240,11 @@ enum { kUnitEncode = 0, kUnitCheck = 1, kUnitCandidate = 2, kUnitRepack = 3 };
 // The work of one analysis unit by one warp.
 // TRACE (tests only, selab200_encode_trace): also copies the unit's analysis intermediates to trace[unit] as they
 // are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.
-template <bool STEREO, bool TRACE, int MODE>
+// FORCE (tests only, selab200_encode_lossless_forced): the unit is coded with the predictor pred[unit] in place of the
+// one its analysis chose; every step after the quantiser, the repair's edits included, runs as in production.
+template <bool STEREO, bool TRACE, int MODE, bool FORCE = false>
 __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_analysis_trace *trace, const uint32_t unit,
-                                            RepairUnit *ru, uint32_t cand)
+                                            RepairUnit *ru, uint32_t cand, const selab200_predictor *pred = nullptr)
 {
     constexpr int kRow = kHistoryPad + kFrame;
     constexpr int kLoWords = (kHistoryPad + kFrame) / 32; // parity bits of a difference signal
@@ -323,6 +325,13 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
     }
     warp_schur(scratch);
     int order = warp_order_and_quantise(scratch, cf);
+    if constexpr (FORCE) { // q past the forced order is zero (the entry point checks it), as the quantiser leaves it
+        const selab200_predictor &f = pred[unit];
+        for (int i = lane; i < kMaxOrder; i += 32)
+            cf.q[i] = f.q[i];
+        order = f.order;
+        __syncwarp();
+    }
     if constexpr (MODE == kUnitCandidate || MODE == kUnitRepack) {
         const PredictorEdit e = repair_edit(order, (int)cand);
         if (e.delta) {
@@ -399,12 +408,13 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
 }
 
 // k_encode_units: encode_unit for unit blockIdx.x.  CHECK: the kUnitCheck instantiation (lossless encodes).
-// `trace` is a kernel argument of its own rather than a field of EncodeParams: a longer EncodeParams would move
-// the parameter offsets of the kernels that take arguments after it.
-template <bool STEREO, bool TRACE = false, bool CHECK = false>
-__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_analysis_trace *trace)
+// `trace` and `pred` (FORCE, tests only) are kernel arguments of their own rather than fields of EncodeParams: a
+// longer EncodeParams would move the parameter offsets of the kernels that take arguments after it.
+template <bool STEREO, bool TRACE = false, bool CHECK = false, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_encode_units(EncodeParams p, selab200_analysis_trace *trace,
+                                                     const selab200_predictor *pred)
 {
-    encode_unit<STEREO, TRACE, CHECK ? kUnitCheck : kUnitEncode>(p, trace, blockIdx.x, nullptr, 0);
+    encode_unit<STEREO, TRACE, CHECK ? kUnitCheck : kUnitEncode, FORCE>(p, trace, blockIdx.x, nullptr, 0, pred);
 }
 
 template <bool STEREO>
@@ -1084,8 +1094,10 @@ __global__ void __launch_bounds__(32) k_lpc_residues(const int32_t *samples, con
 
 // selab200_fir_probe: the encoder's FIR on chosen samples and predictors, a warp per signal.  wide = 0: the int16 row
 // of a channel unit (|s| <= 32767), else the row + parity bits of a 17-bit unit (|s| <= 65535).
+// CHECK (selab200_fir_tie_probe): the instantiation with the tie test, whose flag goes to ties[signal].
+template <bool CHECK = false>
 __global__ void __launch_bounds__(32) k_fir_probe(const int32_t *samples, const int32_t *orders, const long long *c,
-                                                  int wide, int32_t *residues)
+                                                  int wide, int32_t *residues, uint8_t *ties)
 {
     __shared__ __align__(16) AnalysisScratch scratch;
     __shared__ __align__(16) CoefSmem cf;
@@ -1108,10 +1120,10 @@ __global__ void __launch_bounds__(32) k_fir_probe(const int32_t *samples, const 
     __syncwarp();
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
     int32_t *res = residues + (size_t)sub * kFrame;
-    if (wide)
-        warp_fir_residual<true>(sig, cf, order, planes, res);
-    else
-        warp_fir_residual<false>(sig, cf, order, planes, res);
+    const bool tie = wide ? warp_fir_residual<true, CHECK>(sig, cf, order, planes, res)
+                          : warp_fir_residual<false, CHECK>(sig, cf, order, planes, res);
+    if (CHECK && lane == 0)
+        ties[sub] = tie;
 }
 
 // lpc::SampleGenerator::process for one signal per (1-warp) CTA: the decoder's recurrence on one segment at lane 0.

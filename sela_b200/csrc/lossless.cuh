@@ -77,8 +77,10 @@ __global__ void __launch_bounds__(256) k_lossless_select(EncodeParams p, RepairP
 
 // Round 0: the candidates of round 1 of every listed unit; round 1: those of round 2, for units without a round-1
 // winner.  A warp per (unit, candidate) at a time, residue row = the warp's (the grid is at most the batch's units).
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_lossless_candidates(EncodeParams p, RepairParams r, int round)
+// FORCE and `pred` as for k_encode_units (tests only).
+template <bool STEREO, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_lossless_candidates(EncodeParams p, RepairParams r, int round,
+                                                            const selab200_predictor *pred)
 {
     const uint32_t n = *reinterpret_cast<volatile uint32_t *>(&r.count[1]);
     const uint32_t stride = round == 0 ? 7u : (uint32_t)kRepairRound2Max;
@@ -90,12 +92,12 @@ __global__ void __launch_bounds__(32) k_lossless_candidates(EncodeParams p, Repa
                        : cand >= (uint32_t)repair_candidates(o) || ru->best < (1ull << 63)) // round 1 has a winner
             continue;
         __syncwarp();
-        encode_unit<STEREO, false, kUnitCandidate>(p, nullptr, ru->unit, ru, cand);
+        encode_unit<STEREO, false, kUnitCandidate, FORCE>(p, nullptr, ru->unit, ru, cand, pred);
     }
 }
 
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_lossless_repack(EncodeParams p, RepairParams r)
+template <bool STEREO, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_lossless_repack(EncodeParams p, RepairParams r, const selab200_predictor *pred)
 {
     const uint32_t n = *reinterpret_cast<volatile uint32_t *>(&r.count[1]);
     for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
@@ -103,7 +105,7 @@ __global__ void __launch_bounds__(32) k_lossless_repack(EncodeParams p, RepairPa
         if (ru.best == kNoCandidate) // cannot happen (order 1 is a candidate); the flag left set fails the scan
             continue;
         __syncwarp();
-        encode_unit<STEREO, false, kUnitRepack>(p, nullptr, ru.unit, nullptr, (uint32_t)ru.best);
+        encode_unit<STEREO, false, kUnitRepack, FORCE>(p, nullptr, ru.unit, nullptr, (uint32_t)ru.best, pred);
     }
 }
 

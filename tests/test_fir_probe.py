@@ -7,6 +7,8 @@
 The model is pinned to the C port's residues (CPU); the device function runs through selab200_fir_probe, for both
 row forms: the int16 row of a channel unit and the row + parity bits of a 17-bit unit.
 """
+import functools
+
 import numpy as np
 import pytest
 
@@ -84,6 +86,12 @@ def test_no_cpu_fallback_without_device():
     c = np.zeros(MAX_ORDER + 1, np.int64)
     res = np.zeros(FRAME, np.int32)
     assert L.selab200_fir_probe(s.ctypes.data, orders.ctypes.data, c.ctypes.data, 1, 0, res.ctypes.data) == -7
+    ties = np.zeros(1, np.uint8)
+    assert L.selab200_fir_tie_probe(s.ctypes.data, orders.ctypes.data, c.ctypes.data, 1, 0, res.ctypes.data,
+                                    ties.ctypes.data) == -7
+    from sela_b200 import SelaB200Error, codec
+    with pytest.raises(SelaB200Error):
+        codec.fir_tie_probe(s, orders, c, False)
 
 
 # ----------------------------------------------------------------------------------------------------- GPU --
@@ -150,6 +158,125 @@ def test_alternating_parity():
     for i in range(S.shape[0]):
         C[i, 1:] = _with_digits(rng, 1 + i % 8, MAX_ORDER)
     _probe_both(S, C, orders, True)
+
+
+# ------------------------------------------------------------------------------ the tie flag (CHECK) --
+
+@functools.lru_cache(maxsize=None)
+def _planted_rows(wide, offset, seed):
+    """A signal per output position i = 1 .. 2047 with random full-range c and random samples, whose prediction at
+    i is set to 2^34 + offset mod 2^35 by the placer (offset 0: a tie; +-1: a near miss).  Where the placer finds no
+    solution the low taps are drawn again; at the first outputs, which see one or two samples, c[1] is solved for
+    instead (its low 35 bits; the high ones stay random)."""
+    from exact_lossless import M35, place_tie, prediction
+    rng = np.random.default_rng(seed)
+    lim = 65535 if wide else 32767
+    lo = -lim - (not wide)
+    S = rng.integers(lo, lim + 1, size=(FRAME - 1, FRAME)).astype(np.int64)
+    C = rng.integers(-2 ** 63, 2 ** 63 - 1, size=(FRAME - 1, MAX_ORDER + 1), dtype=np.int64, endpoint=True)
+    C[:, 0] = 0
+    orders = rng.integers(8, MAX_ORDER + 1, FRAME - 1)
+    C[np.arange(MAX_ORDER + 1)[None, :] > orders[:, None]] = 0   # the taps the placer sees are the FIR's
+    for r, i in enumerate(range(1, FRAME)):
+        if i <= 2:
+            S[r, i - 1] |= 1
+            rest = (prediction(S[r], C[r], i) - int(C[r, 1]) * int(S[r, i - 1])) % M35
+            low = (HALF + offset - rest) * pow(int(S[r, i - 1]) % M35, -1, M35) % M35
+            v = (int(C[r, 1]) >> Q << Q | low) % (1 << 64)
+            C[r, 1] = v - (1 << 64) if v >= 1 << 63 else v
+            assert prediction(S[r], C[r], i) == (HALF + offset) % M35
+            continue
+        for attempt in range(16):
+            if attempt:
+                C[r, 1:9] = rng.integers(-2 ** 63, 2 ** 63 - 1, 8, dtype=np.int64, endpoint=True)
+            if place_tie(S[r], C[r], i, lo, lim, target=HALF + offset, rng=rng, near=False):
+                break
+        else:
+            raise AssertionError("nothing placed at %d" % i)
+    return S, C, orders
+
+
+def _tie_model(S, C, orders):
+    from exact_lossless import fir
+    res, first = [], []
+    for s, c, o in zip(S, C, orders):
+        r, tie = fir(s, c, int(o))
+        res.append(r)
+        first.append(int(np.argmax(tie)) if tie.any() else -1)
+    return np.stack(res), np.array(first)
+
+
+def _tie_probe(S, C, orders, wide):
+    from sela_b200 import codec
+    res, ties = codec.fir_tie_probe(S, orders, C, wide)
+    want_res, first = _tie_model(S, C, orders)
+    assert np.array_equal(res, want_res)
+    assert np.array_equal(res, fir_residues(S, C, orders))
+    bad = np.nonzero(ties != (first >= 0))[0]
+    assert bad.size == 0, "signals %s: device %s, model first tie %s" % (bad[:8], ties[bad[:8]], first[bad[:8]])
+    return ties, first
+
+
+def test_placer_on_full_range_predictors():
+    """The planted rows (CPU): one tie, at the planted output, and none for a near miss."""
+    for wide in (False, True):
+        S, C, orders = _planted_rows(wide, 0, 40 + wide)
+        _, first = _tie_model(S[::97], C[::97], orders[::97])
+        assert np.array_equal(first, np.arange(1, FRAME)[::97])
+        S, C, orders = _planted_rows(wide, 1, 44 + wide)
+        _, first = _tie_model(S[::97], C[::97], orders[::97])
+        assert (first == -1).all()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("wide", [False, True])
+def test_tie_at_every_output(wide):
+    """One planted tie per signal at every output position 1 .. 2047: every slot of the mma epilogue."""
+    S, C, orders = _planted_rows(wide, 0, 40 + wide)
+    ties, first = _tie_probe(S, C, orders, wide)
+    assert ties.all() and np.array_equal(first, np.arange(1, FRAME))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("wide", [False, True])
+def test_near_misses_do_not_tie(wide):
+    """P = 2^34 +- 1 mod 2^35 at every output position, and rows with no tie anywhere: the flag stays clear."""
+    S1, C1, o1 = _planted_rows(wide, 1, 44 + wide)
+    S2, C2, o2 = _planted_rows(wide, -1, 46 + wide)
+    rng = np.random.default_rng(48 + wide)
+    lim = 65535 if wide else 32767
+    S3 = rng.integers(-lim, lim + 1, size=(64, FRAME))
+    C3 = rng.integers(-2 ** 40, 2 ** 40, size=(64, MAX_ORDER + 1))
+    o3 = np.arange(64) % 3   # orders 0 .. 2
+    S = np.concatenate([S1, S2, S3])
+    ties, first = _tie_probe(S, np.concatenate([C1, C2, C3]), np.concatenate([o1, o2, o3]), wide)
+    assert not ties.any()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("wide", [False, True])
+def test_wrap_territory(wide):
+    """Saturated +-2^63 coefficients and sums at and near +-2^63, where the 64-bit wrap decides: the sum of the two
+    roundings is then -2^29 or 1 - 2^29 instead of 0 or 1, and the device must follow the formula bit for bit."""
+    rng = np.random.default_rng(50 + wide)
+    lim = 65535 if wide else 32767
+    rows_S, rows_C, rows_o = [], [], []
+    for c1 in (-2 ** 63, 2 ** 63 - 1, 2 ** 62, -2 ** 62, 3 * 2 ** 61, -(2 ** 63) + 2 ** 34, 2 ** 63 - 2 ** 34):
+        for order in (1, 2, 100):
+            for odd_at in (None, 0, 1, 7, 1000, FRAME - 2):
+                s = 2 * rng.integers(-(lim // 2), lim // 2 + 1, FRAME)
+                if odd_at is not None:
+                    s[odd_at] += 1
+                c = np.zeros(MAX_ORDER + 1, np.int64)
+                c[1:order + 1] = c1
+                if order == 100:
+                    c[2:101:2] = -c1 if c1 != -2 ** 63 else c1
+                rows_S.append(s)
+                rows_C.append(c)
+                rows_o.append(order)
+    S, C, o = np.stack(rows_S), np.stack(rows_C), np.array(rows_o)
+    ties, first = _tie_probe(S, C, o, wide)
+    assert ties.any() and not ties.all()
 
 
 @pytest.mark.gpu

@@ -2,12 +2,12 @@
 `sela -L`): every subframe the reference decoder would not bring back to its source is re-coded with a tie-free
 predictor, inside the format (DESIGN.md 7.2).
 
-The expected output comes from the CPU model below, built on the plain-C port (oracle/liboracle.so): the tie
-criterion in NumPy (int64 wrap), and the repair rule -- candidates, rounds, fewest words, first candidate on a
-tie -- over the port's lpc_coefficients and rice_size.  Every decode check uses the port's decoder, and the
-compiled reference where it has been built."""
+The expected output comes from the CPU model in exact_lossless.py, built on the plain-C port
+(oracle/liboracle.so): the tie criterion in NumPy (int64 wrap), and the repair rule -- candidates, rounds, fewest
+words, first candidate on a tie -- over the port's lpc_coefficients and rice_size.  Every decode check uses the
+port's decoder, and the compiled reference where it has been built.  test_lossless_repair.py drives the repair
+through chosen predictors and planted ties."""
 import ctypes as C
-import os
 import pathlib
 import subprocess
 
@@ -16,6 +16,8 @@ import pytest
 
 import analysis_corpus
 import oracle_lib as ol
+from exact_lossless import (analyse, as_tuples, check_against_model, expected_report, fir, model_batch, repair,
+                            repair_edit)
 from sela_b200 import _lib, synth, wavio
 
 GOLD = np.load(pathlib.Path(__file__).parent / "golden" / "golden_frames.npz")
@@ -27,119 +29,6 @@ REF_CLI = ROOT / "oracle" / "_ref" / "sela_ref_cli"
 LOSSY = GOLD["pcm_oct_reference_lossy"].reshape(2, FRAME, 8)
 L0 = LOSSY[0, :, 1].astype(np.int64)  # order 86, a tie at sample 1
 L1 = LOSSY[1, :, 4].astype(np.int64)  # order 29, a tie at sample 1
-U64 = np.uint64
-
-
-# ------------------------------------------------------------- CPU model --
-
-def fir(s, c, order):
-    """The encoder's residual and the tie test of every output: (res int32[2048], tie bool[2048])."""
-    s = np.asarray(s, np.int64)
-    su = s.astype(U64)
-    cu = np.asarray(c, np.int64).astype(U64)
-    P = np.zeros(s.size, U64)
-    for j in range(1, order + 1):
-        P[j:] += cu[j] * su[:-j]
-    total = P + U64(1 << 34)
-    enc = total.view(np.int64) >> 35                   # (2^34 + P) >> 35
-    dec = (U64(1 << 35) - total).view(np.int64) >> 35  # (2^34 - P) >> 35
-    tie = ((enc + dec) & 0xFFFFFFFF) != 0              # as int32: enc + dec != 0
-    return (s - enc).astype(np.int32), tie
-
-
-def rice_words(O, x):
-    x = np.ascontiguousarray(x, np.int32)
-    k, bits = C.c_uint32(0), C.c_uint64(0)
-    O.lib.sela_oracle_rice_size.restype = C.c_size_t
-    return int(O.lib.sela_oracle_rice_size(x.ctypes.data, x.size, C.byref(k), C.byref(bits)))
-
-
-def repair_edit(o, c):
-    """Candidate c of a unit of order o (kernels.cuh repair_edit): (order, j, delta)."""
-    n1 = 5 if o == 2 else 7
-    if c < n1:
-        if c == n1 - 1:
-            return o - 1, 0, 0
-        return o, (c >> 1) if (c >> 1) < 2 else o - 1, 1 if c & 1 else -1
-    c -= n1
-    n_edits = 2 * (o - 3) if o > 3 else 0
-    if c < n_edits:
-        return o, 2 + (c >> 1), 1 if c & 1 else -1
-    return o - 2 - (c - n_edits), 0, 0
-
-
-class Unit:
-    def __init__(self, O, s, order, q):
-        self.s, self.order, self.q = s, order, np.asarray(q, np.int32)
-        self.c = O.lpc_coefficients(self.q, order)
-        self.res, ties = fir(s, self.c, order)
-        self.tie = bool(ties.any())
-        self.words = rice_words(O, self.q[:order]) + rice_words(O, self.res)
-
-
-def analyse(O, s):
-    a = O.lpc_analyse(np.asarray(s, np.int32))
-    q = np.zeros(100, np.int32)
-    q[:a["order"]] = a["q"]
-    return Unit(O, s, a["order"], q)
-
-
-def repair(O, u):
-    """The winner of the repair of a unit with a tie, as a Unit (+ .cand)."""
-    o = u.order
-    n1 = 5 if o == 2 else 7
-    for cands in (range(n1), range(n1, 3 * o - 1)):
-        best = None
-        for cand in cands:
-            order, j, delta = repair_edit(o, cand)
-            q = u.q.copy()
-            q[order:] = 0
-            if delta:
-                q[j] += delta
-                if not -64 <= q[j] <= 63:
-                    continue
-            v = Unit(O, u.s, order, q)
-            if not v.tie and (best is None or v.words < best.words):
-                best, best.cand = v, cand
-        if best is not None:
-            return best
-    raise AssertionError("order 1 is always a candidate")
-
-
-def emitted(units, channels):
-    """(unit index, subframe type) per channel: the encoder's stereo decision (difference iff strictly smaller)."""
-    if channels != 2:
-        return [(k, 0) for k in range(channels)]
-    return [(0, 0), (2, 1) if units[2].words < units[1].words else (1, 0)]
-
-
-def model_frame(O, planes, channels):
-    """planes: the frame's unit signals in encoder order -> (emitted units per channel with their type, report
-    entries (channel, ref_order, ref_words, order, words))."""
-    units = [analyse(O, s) for s in planes]
-    ref = emitted(units, channels)
-    if not any(units[k].tie for k, _ in ref):
-        return [(units[k], t) for k, t in ref], []
-    now_units = [repair(O, u) if u.tie else u for u in units]
-    now = emitted(now_units, channels)
-    report = []
-    for ch in range(channels):
-        (ka, _), (kb, _) = ref[ch], now[ch]
-        if ka != kb or units[kb].tie:
-            report.append((ch, units[ka].order, units[ka].words, now_units[kb].order, now_units[kb].words))
-    return [(now_units[k], t) for k, t in now], report
-
-
-def model_batch(O, pcm, channels):
-    """-> {frame: (emitted, report)} for the frames the model re-codes."""
-    out = {}
-    units = analysis_corpus.units(pcm, channels)
-    per = 3 if channels == 2 else channels
-    for f in range(units.shape[0] // per):
-        em, rep = model_frame(O, units[f * per:(f + 1) * per], channels)
-        if rep:
-            out[f] = (em, rep)
-    return out
 
 
 # ------------------------------------------------------------------- CPU --
@@ -207,42 +96,21 @@ def test_lossless_entry_points_have_no_cpu_fallback():
     assert L.selab200_encode_frames_lossless_device(pcm.ctypes.data, 1, 1, descs.ctypes.data, words.ctypes.data,
                                                     words.size, blob.ctypes.data, rep.ctypes.data, blob.ctypes.data,
                                                     blob.ctypes.data, blob.ctypes.data, blob.size, None) == -7
+    pred = np.zeros(1, _lib.PREDICTOR_DTYPE)
+    assert L.selab200_encode_lossless_forced(pcm.ctypes.data, 1, 1, pred.ctypes.data, descs.ctypes.data,
+                                             words.ctypes.data, words.size, C.addressof(used), rep.ctypes.data, 1,
+                                             C.addressof(n)) == -7
     assert L.selab200_encode_lossless_workspace_bytes(10, 2) > L.selab200_encode_workspace_bytes(10, 2)
     assert _lib.LOSSLESS_DTYPE.itemsize == 16
     import sela_b200
+    from sela_b200 import codec
     with pytest.raises(sela_b200.SelaB200Error):
         sela_b200.encode_frames_lossless(pcm, 1)
+    with pytest.raises(sela_b200.SelaB200Error):
+        codec.encode_lossless_forced(pcm, 1, [(1, [0])])
 
 
 # ------------------------------------------------------------------- GPU --
-
-def as_tuples(report):
-    return [(int(e["frame"]), int(e["channel"]), int(e["ref_order"]), int(e["ref_words"]), int(e["order"]),
-             int(e["words"])) for e in report]
-
-
-def expected_report(model):
-    return [(f, ch, ro, rw, o, w) for f in sorted(model) for ch, ro, rw, o, w in model[f][1]]
-
-
-def check_against_model(O, descs, words, pcm, channels, model):
-    """The re-coded frames' subframes equal the model's, field for field and word for word, and the whole
-    batch decodes back to its source under the port (and the compiled reference, where built)."""
-    d = descs.reshape(-1, channels)
-    for f, (em, _) in model.items():
-        for ch, (u, t) in enumerate(em):
-            s = d[f][ch]
-            assert (int(s["lpc_order"]), int(s["subframe_type"])) == (u.order, t), (f, ch)
-            kq, wq = O.rice_encode(u.q[:u.order])
-            kr, wr = O.rice_encode(u.res)
-            assert (int(s["refl_rice_param"]), int(s["res_rice_param"])) == (kq, kr), (f, ch)
-            got_q = words[int(s["refl_offset"]):int(s["refl_offset"]) + int(s["refl_words"])]
-            got_r = words[int(s["res_offset"]):int(s["res_offset"]) + int(s["res_words"])]
-            assert np.array_equal(got_q, wq) and np.array_equal(got_r, wr), (f, ch)
-    src = np.asarray(pcm, np.int16).reshape(-1)
-    for D in [O] + ([ol.load("ref")] if ol.have_ref() else []):
-        assert np.array_equal(D.decode_frames(descs, words, channels), src)
-
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", [c for c in CASES if c != "oct_reference_lossy"])
