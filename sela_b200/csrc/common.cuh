@@ -23,7 +23,6 @@ constexpr unsigned kFull = 0xffffffffu;
 // The decoder's offset, 2^31: s ^ 2^31 == s + 2^31 maps every int32 onto [0, 2^32), so the
 // same unsigned products are exact for any sample a stream can decode to (lpc.cuh, K6).
 constexpr uint32_t kSynthBias = 0x80000000u;
-__device__ __forceinline__ uint32_t synth_biased(int s) { return (uint32_t)s ^ kSynthBias; }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }
@@ -45,16 +44,6 @@ __device__ __forceinline__ double shfl_down_d(double v, int delta)
 __device__ __forceinline__ unsigned long long shfl_u64(unsigned long long v, int src)
 {
     return __shfl_sync(kFull, v, src);
-}
-
-// d = a*b + c with a 32x32->64 multiply (IMAD.WIDE.U32).  Spelled in PTX because NVVM
-// likes to hoist the zero-extension of a loop-invariant operand into a 64-bit register,
-// after which ptxas emits a full 64x32 multiply (an extra IMAD + IADD per tap).
-__device__ __forceinline__ unsigned long long mad_wide_u32(uint32_t a, uint32_t b, unsigned long long c)
-{
-    unsigned long long d;
-    asm("mad.wide.u32 %0, %1, %2, %3;" : "=l"(d) : "r"(a), "r"(b), "l"(c));
-    return d;
 }
 
 __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)

@@ -517,13 +517,13 @@ __device__ bool warp_fir_residual(const Signal &sig, const CoefSmem &cf, int ord
 // known every lane adds c[j]*s'[i] to the accumulator of output i+j; the accumulator
 // of output i+1 (tap 1, first lane) is then complete, that lane finishes the sample and
 // broadcasts it, and every accumulator moves one tap down (one 64-bit shuffle per
-// lane, register renaming inside a lane).  Critical path per sample: one IMAD, a
-// 64-bit subtract, a shift and ONE shuffle -- instead of a five-level reduction.
+// lane, register renaming inside a lane).  Critical path per sample: the two multiplies of
+// tap 1, a shift-and-add, an add and ONE shuffle -- instead of a five-level reduction.
 //
 // A warp runs as many subframes as fit, each on a SEGMENT of consecutive lanes.  A subframe of
 // order o owns n = max(1, ceil(o / kTapsPerLane)) lanes; lane k of the segment owns taps kTapsPerLane*k + 1 ..
-// kTapsPerLane*(k+1) (zero beyond o).  Every segment runs the recurrence at once: the segment's top lane takes 0
-// where the others take the accumulator of the lane above, and the finished sample reaches the segment from its
+// kTapsPerLane*(k+1) (zero beyond o).  Every segment runs the recurrence at once: the segment's top lane starts a new
+// output where the others take the accumulator of the lane above, and the finished sample reaches the segment from its
 // first lane.  Taps per lane are fixed, so the multiplies a warp issues follow the orders it holds.
 constexpr int kTapsPerLane = 8;
 constexpr int kMaxWidth = (kMaxOrder + kTapsPerLane - 1) / kTapsPerLane; // 13 lanes for order 100
@@ -552,7 +552,7 @@ struct SegSmem {
 // (k = lane - start), the loop runs to the largest order in the warp.  Same operations in the same order per
 // element as warp_coefficients.  Returns this lane's taps kTapsPerLane*k + 1 .. as Q35 words.
 __device__ __forceinline__ void segment_coefficients(SegSmem &sm, int start, int k, int n, int order, int order_max,
-                                                     uint32_t (&cl)[kTapsPerLane], int32_t (&ch)[kTapsPerLane])
+                                                     uint32_t (&cl)[kTapsPerLane], uint32_t (&ch)[kTapsPerLane])
 {
     double *t = sm.t + kTapsPerLane * start;
     const int32_t *q = sm.q + kTapsPerLane * start;
@@ -583,30 +583,32 @@ __device__ __forceinline__ void segment_coefficients(SegSmem &sm, int start, int
         const int j = kTapsPerLane * k + m; // tap j + 1
         const long long v = (live && j < order) ? __double2ll_rz(dmul(scale, -t[j])) : 0;
         cl[m] = (uint32_t)v;
-        ch[m] = (int32_t)(v >> 32);
+        ch[m] = (uint32_t)((unsigned long long)v >> 32);
     }
     __syncwarp(); // t is dead: its bytes become the output rows
 }
 
 struct SegState {
     uint32_t cl[kTapsPerLane];
-    int32_t ch[kTapsPerLane];
-    unsigned long long alo[kTapsPerLane];
-    uint32_t ahi[kTapsPerLane];
+    uint32_t ch[kTapsPerLane];
+    unsigned long long acc[kTapsPerLane];
     uint32_t sp;
-    unsigned long long steady; // 2^34 + 2^31 * sum_j c[j]: the rounding constant and the sample bias, at the first lane
+    unsigned long long fresh; // what the accumulator of a new output starts from: ~(2^34 + 2^31 * sum_j c[j])
 };
 
 // Accumulators before the first product: slot m of lane k is output j = kTapsPerLane*k + m + 1, and it starts with
 // what the samples before the subframe contribute in biased form, 2^31 * sum_{j < j' <= order} c[j'] (s[<0] = 0 is
-// s' = 2^31).  Every output then carries the bias of every tap, and one constant removes it from each of them.
-__device__ __forceinline__ void segment_state(SegState &st, int k, int n)
+// s' = 2^31).  Every output then carries the bias of every tap.  Every output also starts from
+// fresh = ~(2^34 + 2^31 * sum_j c[j]), so that its finished accumulator is a = ~y with y = 2^34 - sum_j c[j]*s[i-j],
+// the reference's operand of the rounding shift (mod 2^64).  Then -(int32)(y >> 35) == (int32)(a >> 35) + 1 for every
+// 64-bit y, because an arithmetic shift commutes with ~: finishing a sample is a shift-and-add and an add.
+__device__ __forceinline__ void segment_state(SegState &st, int k, int n, int src)
 {
     unsigned long long tot = 0, loc[kTapsPerLane];
 #pragma unroll
     for (int m = kTapsPerLane - 1; m >= 0; m--) {
         loc[m] = tot; // taps above m in this lane
-        tot += (unsigned long long)(((unsigned long long)(uint32_t)st.ch[m] << 32) | st.cl[m]);
+        tot += ((unsigned long long)st.ch[m] << 32) | st.cl[m];
     }
     unsigned long long incl = tot; // sum over lanes k.. of the segment
 #pragma unroll
@@ -616,44 +618,62 @@ __device__ __forceinline__ void segment_state(SegState &st, int k, int n)
             incl += x;
     }
     const unsigned long long above = incl - tot;
+    st.fresh = ~((1ull << (kQ - 1)) + (__shfl_sync(kFull, incl, src) << 31));
 #pragma unroll
-    for (int m = 0; m < kTapsPerLane; m++) {
-        st.alo[m] = (above + loc[m]) << 31;
-        st.ahi[m] = 0;
-    }
-    st.steady = (1ull << (kQ - 1)) + (incl << 31);
+    for (int m = 0; m < kTapsPerLane; m++)
+        st.acc[m] = ((above + loc[m]) << 31) + st.fresh;
 }
 
-// One block of kSegBlock outputs.  in_row / out_row: this segment's staging rows; src: its first lane.
+// acc += c * s' mod 2^64, c = ch:cl: one IMAD.WIDE.U32 with the accumulator as addend and one IMAD into its high word.
+// Spelled as a carry chain: ptxas fuses mad.lo.cc + madc.hi into that IMAD.WIDE.U32, while it splits mad.wide.u32 with
+// a register addend into a product into RZ plus an IADD3 / IADD3.X pair (four instructions per tap instead of two).
+__device__ __forceinline__ unsigned long long segment_tap(unsigned long long acc, uint32_t cl, uint32_t ch, uint32_t sp)
+{
+    unsigned long long d;
+    asm("{\n\t.reg .u32 lo, hi;\n\t"
+        "mov.b64 {lo, hi}, %4;\n\t"
+        "mad.lo.u32 hi, %2, %3, hi;\n\t"
+        "mad.lo.cc.u32 lo, %1, %3, lo;\n\t"
+        "madc.hi.u32 hi, %1, %3, hi;\n\t"
+        "mov.b64 %0, {lo, hi};\n\t}"
+        : "=l"(d) : "r"(cl), "r"(ch), "r"(sp), "l"(acc));
+    return d;
+}
+
+// One block of kSegBlock outputs.  in_row / out_row: this segment's staging rows; src: its first lane.  The staging
+// rows of finished samples hold them biased (s' = s ^ kSynthBias), four to a store.
 // FIRST: block 0, whose output 0 is s[0] = r[0].
 template <bool FIRST>
 __device__ __forceinline__ void segment_block(SegState &st, const int32_t *in_row, int32_t *out_row, int src, bool top,
                                               bool first)
 {
 #pragma unroll
-    for (int e = 0; e < kSegBlock; e++) {
-        const int r = in_row[e];
-        int v;
-        if (FIRST && e == 0) {
-            v = r;
-        } else {
-            const int u = (e + kTapsPerLane - 1) % kTapsPerLane; // == (t - 1) % kTapsPerLane, static
+    for (int g = 0; g < kSegBlock; g += 4) {
+        const int4 r4 = *reinterpret_cast<const int4 *>(in_row + g);
+        const uint32_t r[4] = {(uint32_t)r4.x, (uint32_t)r4.y, (uint32_t)r4.z, (uint32_t)r4.w};
+        uint32_t s[4];
 #pragma unroll
-            for (int m = 0; m < kTapsPerLane; m++) {
-                st.alo[(m + u) % kTapsPerLane] = mad_wide_u32(st.cl[m], st.sp, st.alo[(m + u) % kTapsPerLane]);
-                st.ahi[(m + u) % kTapsPerLane] += (uint32_t)st.ch[m] * st.sp;
+        for (int h = 0; h < 4; h++) {
+            const int e = g + h;
+            if (FIRST && e == 0) {
+                st.sp = r[0] ^ kSynthBias;
+            } else {
+                const int u = (e + kTapsPerLane - 1) % kTapsPerLane; // == (t - 1) % kTapsPerLane, static
+#pragma unroll
+                for (int m = 0; m < kTapsPerLane; m++)
+                    st.acc[(m + u) % kTapsPerLane] =
+                        segment_tap(st.acc[(m + u) % kTapsPerLane], st.cl[m], st.ch[m], st.sp);
+                const unsigned long long done = st.acc[u];
+                const unsigned long long incoming = __shfl_down_sync(kFull, done, 1);
+                // s' = r - (int32)(y >> 35) + 2^31 = r + (int32)(done >> 35) + 1 + 2^31 (segment_state)
+                const uint32_t v = r[h] + (uint32_t)((int32_t)(done >> 32) >> (kQ - 32)) + (1u + kSynthBias);
+                st.sp = __shfl_sync(kFull, v, src);
+                st.acc[u] = top ? st.fresh : incoming;
             }
-            const unsigned long long full0 = st.alo[u] + ((unsigned long long)st.ahi[u] << 32);
-            const unsigned long long incoming = __shfl_down_sync(kFull, full0, 1);
-            const unsigned long long tt = st.steady - full0;
-            v = r - (int32_t)((long long)tt >> kQ);
-            v = __shfl_sync(kFull, v, src);
-            st.alo[u] = top ? 0ull : incoming;
-            st.ahi[u] = 0;
+            s[h] = st.sp;
         }
         if (first)
-            out_row[e] = v;
-        st.sp = synth_biased(v);
+            *reinterpret_cast<int4 *>(out_row + g) = make_int4((int)s[0], (int)s[1], (int)s[2], (int)s[3]);
     }
 }
 
@@ -689,8 +709,7 @@ __device__ __forceinline__ void segment_synthesis(SegSmem &sm, int start, int k,
         order_max = max(order_max, __shfl_xor_sync(kFull, order_max, o));
     SegState st;
     segment_coefficients(sm, start, k, n, order, order_max, st.cl, st.ch);
-    segment_state(st, k, n);
-    st.sp = 0;
+    segment_state(st, k, n, start);
 
     // ---- recurrence + output ----
     const bool top = k == n - 1, first = k == 0;
@@ -707,7 +726,7 @@ __device__ __forceinline__ void segment_synthesis(SegSmem &sm, int start, int k,
         for (int i = lane >> 4; i < n_seg; i += 2) {
             const int mode = sm.row_mode[i];
             const int e = lane & 15, t = kSegBlock * B + e;
-            const int v = sm.out[i * kSegRow + e];
+            const int v = (int)((uint32_t)sm.out[i * kSegRow + e] ^ kSynthBias);
             if (mode == 1)
                 static_cast<int16_t *>(sm.row_out[i])[(size_t)t * stride] = (int16_t)(uint16_t)v;
             else if (mode == 2)
