@@ -77,7 +77,8 @@ typedef struct selab200_subframe_desc {
 int  selab200_init(int device);
 /* Several devices of one box (SURVEY.md 8b: selagpu_init(device_count, device_ids)): every device gets a
  * context of its own (streams, events, pools).  The host-buffer batch calls (selab200_encode_frames,
- * selab200_decode_frames, selab200_encode_container, selab200_container_decode and their verify and lossless forms) then cut the frames into one contiguous block per device
+ * selab200_decode_frames, selab200_encode_container, selab200_container_decode and their verify, lossless and
+ * search forms) then cut the frames into one contiguous block per device
  * -- n/D frames each, the last device takes the rest, the way sela::Encoder::processFrames cuts them for its
  * threads (src/sela/encoder.cpp:58-73) -- and run the blocks concurrently, reading and writing disjoint ranges
  * of the caller's buffers; results are byte-identical to a single device's.  devices[0] is the primary: it
@@ -316,6 +317,36 @@ int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_fram
                                            int32_t *d_status, void *d_workspace, size_t workspace_bytes,
                                            void *stream);
 
+/* ------------------------------------------------------- order search -- */
+
+/* Smaller files at a higher encode cost (DESIGN.md 7.3), like `flac -8`.  The reference encoder takes the predictor
+ * order from a threshold on the reflection coefficients; the search forms code every analysis unit (a channel, or
+ * for stereo ch0, ch1 and ch0 - ch1) at the order 1..100 with the fewest words (reflection + residue) among those
+ * whose FIR has no tie, so that every subframe decodes back to its source under the reference decoder.  Between equal
+ * words the reference encoder's order wins if it is among them, else the lowest order.  The stereo decision then runs
+ * as always on the searched units.  The output is an ordinary stream that the unmodified reference decoder reads.
+ * *ref_words receives the words the reference encoder's choice takes for the same frames (the words_used of
+ * selab200_encode_frames), so that the caller sees the saving.  Frames are split over devices as for the other batch
+ * calls. */
+int selab200_encode_frames_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                  size_t *words_used, size_t *ref_words);
+
+/* selab200_encode_container, with the order search; *ref_bytes receives the size of selab200_encode_container's
+ * output for the same frames. */
+int selab200_encode_container_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                     uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                     size_t capacity, size_t *bytes_used, size_t *ref_bytes);
+
+/* Device-resident form of selab200_encode_frames_search: arguments as selab200_encode_frames_device, with
+ * selab200_encode_search_workspace_bytes() of workspace; *d_ref_words (uint64, device) receives the reference
+ * encoder's words.  Stream-ordered, no synchronisation. */
+size_t selab200_encode_search_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                         selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
+                                         uint64_t *d_words_used, uint64_t *d_ref_words, int32_t *d_status,
+                                         void *d_workspace, size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------ stage level (host buffers) -- */
 
 /* lpc::ResidueGenerator::process (src/lpc/residue_generator.cpp:121-134) for
@@ -415,6 +446,15 @@ int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint3
                                     const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                     size_t words_capacity, size_t *words_used, selab200_lossless_entry *entries,
                                     size_t entries_capacity, size_t *n_entries);
+
+/* For tests: selab200_encode_frames_search on one device and one batch, except that every analysis unit takes
+ * pred[unit].q[0..99] as its 100 quantised reflection coefficients (values past the order included) and
+ * pred[unit].order as the reference encoder's order, instead of what its analysis gives.  pred holds one record per
+ * analysis unit, in the order of selab200_encode_trace's.  An order outside 1..100 or any q outside [-64, 63] ->
+ * SELAB200_ERR_RANGE.  The other arguments as selab200_encode_frames_search. */
+int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                  size_t words_capacity, size_t *words_used, size_t *ref_words);
 
 #ifdef __cplusplus
 }

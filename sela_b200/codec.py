@@ -18,10 +18,14 @@ error behaviour as in include/sela_b200.h):
     encode_frames_lossless / encode_container_lossless
                                     not in the reference: encodes that decode back to their source, re-coding
                                     the few subframes the reference decoder would not reproduce (DESIGN.md 7.2)
+    encode_frames_search / encode_container_search
+                                    not in the reference: smaller files at a higher encode cost, every subframe
+                                    coded at the predictor order with the fewest words (DESIGN.md 7.3)
     encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
     / fir_probe / fir_tie_probe     order threshold and quantiser on chosen values, its FIR residual
                                     (and tie test) on chosen signals and predictors, and the lossless
-    encode_lossless_forced          encode with chosen predictors
+    encode_lossless_forced          encode with chosen predictors, and the order search with chosen
+    / encode_search_forced          coefficients
 
 Everything computes on the GPU through the C ABI; NumPy only carries host buffers.
 The C++ mirror of the same interface (data::, frame::, file::, sela:: classes and
@@ -372,3 +376,58 @@ def encode_container_lossless(pcm, channels, sample_rate, bits_per_sample=16, ca
                                                out.ctypes.data, cap, C.addressof(used), report.ctypes.data,
                                                report.size, C.addressof(n)))
     return out[:used.value], report[:n.value].copy()
+
+
+def encode_frames_search(pcm, channels, words_capacity=None, device=0):
+    """encode_frames with the order search (DESIGN.md 7.3) -> (descs, words, ref_words): ref_words is the number of
+    words encode_frames writes for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_frames_search(pcm.ctypes.data, n_frames, channels, descs.ctypes.data, words.ctypes.data,
+                                          cap, C.addressof(used), C.addressof(ref)))
+    return descs, words[:used.value].copy(), ref.value
+
+
+def encode_container_search(pcm, channels, sample_rate, bits_per_sample=16, capacity=None, device=0):
+    """encode_container with the order search -> (bytes, ref_bytes): ref_bytes is the size of encode_container's
+    output for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_container_search(pcm.ctypes.data, n_frames, channels, sample_rate, bits_per_sample,
+                                             out.ctypes.data, cap, C.addressof(used), C.addressof(ref)))
+    return out[:used.value], ref.value
+
+
+def encode_search_forced(pcm, channels, predictors, device=0):
+    """encode_frames_search on one batch, every analysis unit taking its 100 quantised reflection coefficients and
+    its reference order from `predictors` (PREDICTOR_DTYPE[n_units], or a sequence of (order, q[100]) pairs, in
+    encode_trace's unit order) instead of its analysis -> (descs, words, ref_words)."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    n_units = n_frames * (3 if channels == 2 else channels)
+    if isinstance(predictors, np.ndarray) and predictors.dtype == PREDICTOR_DTYPE:
+        pred = _c(predictors, PREDICTOR_DTYPE)
+    else:
+        pred = np.zeros(len(predictors), PREDICTOR_DTYPE)
+        for rec, (order, q) in zip(pred, predictors):
+            rec["order"] = order
+            rec["q"][:] = np.asarray(q)[:MAX_ORDER]
+    if pred.size != n_units:
+        raise ValueError("%d predictors for %d analysis units" % (pred.size, n_units))
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
+                                          words.ctypes.data, cap, C.addressof(used), C.addressof(ref)))
+    return descs, words[:used.value].copy(), ref.value

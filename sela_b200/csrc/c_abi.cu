@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "lossless.cuh"
+#include "search.cuh"
 #include "verify.cuh"
 
 using namespace selab200;
@@ -344,6 +345,34 @@ int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames,
     return launch_check("k_lossless_report");
 }
 
+// The order search (search.cuh) in place of k_encode_units: analysis, candidates, repack, and the reference encoder's
+// words added to *d_ref_words.  The warp kernels have grids of a fixed size, at most one residue row per unit of the
+// batch.  FORCE: the units' q and reference orders are d_pred's (selab200_encode_search_forced).
+template <bool STEREO, bool FORCE = false>
+int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t n_units,
+                  unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred = nullptr)
+{
+    constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
+    if (int rc = set_smem(k_search_units<STEREO, FORCE>, smem))
+        return rc;
+    if (int rc = set_smem(k_search_candidates<STEREO>, smem_orders))
+        return rc;
+    if (int rc = set_smem(k_search_repack<STEREO>, smem_orders))
+        return rc;
+    k_search_units<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su);
+    if (int rc = launch_check("k_search_units"))
+        return rc;
+    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
+    k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
+    if (int rc = launch_check("k_search_candidates"))
+        return rc;
+    k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
+    if (int rc = launch_check("k_search_ref_words"))
+        return rc;
+    k_search_repack<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
+    return launch_check("k_search_repack");
+}
+
 // Where a lossless encode reports its re-coded subframes: the batch's per-pair records, their count, and the frame
 // number of the batch's first frame.
 struct LosslessArgs {
@@ -366,7 +395,10 @@ struct EncodeOptions {
     unsigned long long sub_base = 0;            // ... where the batch's first subframe is subframe sub_base
     selab200_analysis_trace *d_trace = nullptr; // the tracing unit kernel writes every unit's analysis here
     const LosslessArgs *lossless = nullptr;     // encode lossless (DESIGN.md 7.2) and report the re-coded pairs
-    const selab200_predictor *d_pred = nullptr; // lossless only: every unit's predictor (selab200_encode_lossless_forced)
+    unsigned long long *d_ref_words = nullptr;  // search the order (DESIGN.md 7.3) and add the reference encoder's
+                                                // words here
+    const selab200_predictor *d_pred = nullptr; // lossless or search only: every unit's predictor
+                                                // (selab200_encode_lossless_forced / selab200_encode_search_forced)
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -375,8 +407,9 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
 {
     if (int rc = check_channels(channels))
         return rc;
-    if (ws_bytes < (o.lossless ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
-                               : selab200_encode_workspace_bytes(n_frames, channels)))
+    if (ws_bytes < (o.lossless      ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
+                    : o.d_ref_words ? selab200_encode_search_workspace_bytes(n_frames, channels)
+                                    : selab200_encode_workspace_bytes(n_frames, channels)))
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
         return fail(SELAB200_ERR_ARGUMENT, "stereo PCM must be 16-byte aligned on the device");
@@ -431,6 +464,15 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
                                 : launch_repair<false>(p, r, n_frames, n_units, stream))
                 return rc;
         }
+    } else if (o.d_ref_words) {
+        SearchUnit *su = reinterpret_cast<SearchUnit *>(static_cast<char *>(d_ws) +
+                                                        align256(selab200_encode_workspace_bytes(n_frames, channels)));
+        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, o.d_ref_words, stream, o.d_pred)
+                                          : launch_search<false, true>(p, su, n_frames, n_units, o.d_ref_words, stream, o.d_pred))
+                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, o.d_ref_words, stream)
+                                          : launch_search<false>(p, su, n_frames, n_units, o.d_ref_words, stream));
+        if (rc)
+            return rc;
     } else {
         const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
                                                  : launch_encode_units<true, false>(p, n_units, nullptr, stream))
@@ -911,6 +953,12 @@ size_t selab200_encode_lossless_workspace_bytes(uint32_t n_frames, uint32_t chan
     return align256(selab200_encode_workspace_bytes(n_frames, channels)) + repair_lists_bytes(n_frames, channels);
 }
 
+size_t selab200_encode_search_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    return align256(selab200_encode_workspace_bytes(n_frames, channels)) +
+           encode_units(n_frames, channels) * sizeof(SearchUnit);
+}
+
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_sub = (size_t)n_frames * channels;
@@ -960,6 +1008,25 @@ int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_fram
     o.lossless = &la;
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, st, o);
+}
+
+int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                         selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
+                                         uint64_t *d_words_used, uint64_t *d_ref_words, int32_t *d_status,
+                                         void *d_workspace, size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_ref_words || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(d_ref_words, 0, sizeof(uint64_t), (cudaStream_t)stream));
+    EncodeOptions o;
+    o.d_ref_words = reinterpret_cast<unsigned long long *>(d_ref_words);
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
 
 int selab200_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint32_t channels,
@@ -1088,13 +1155,16 @@ struct EncodeTarget {
 // `report` (container form only): also verify the container image, chunk by chunk on the device, and return
 // the differing (frame, channel) pairs.
 // `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs.
+// `ref_words`: search the order (DESIGN.md 7.3) and return the words the reference encoder's choice takes.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
                        size_t *words_used, uint32_t frame_base, std::vector<selab200_verify_entry> *report,
-                       std::vector<selab200_lossless_entry> *recoded)
+                       std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr)
 {
     const size_t words_capacity = t.words_capacity;
     const bool to_container = t.form == EncodeForm::container;
     *words_used = 0;
+    if (ref_words)
+        *ref_words = 0;
     if (report)
         report->clear();
     if (recoded)
@@ -1107,8 +1177,9 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
     const bool verify = report && to_container;
-    const size_t ws_bytes = recoded ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
-                                    : selab200_encode_workspace_bytes(plan.max_frames, channels);
+    const size_t ws_bytes = recoded     ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
+                            : ref_words ? selab200_encode_search_workspace_bytes(plan.max_frames, channels)
+                                        : selab200_encode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(container_frame_byte(n_frames, channels, words_capacity) + 64)) return rc;
@@ -1128,6 +1199,8 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         if (int rc = g.lane_work[kEncLanes + i].ensure(selab200_verify_workspace_bytes(plan.max_frames, channels))) return rc;
     int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
     uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
+    // search: the reference encoder's words, summed over the chunks
+    unsigned long long *d_ref_words = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
     uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
@@ -1137,7 +1210,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     if (verify)
         if (int rc = verify_area(n_sub, arena_words, g.s_compute[0], va)) return rc;
 
-    CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
+    CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, ref_words ? 24 : 16, g.s_compute[0]));
     if (recoded)
         CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, 256 + n_sub * sizeof(selab200_lossless_entry), g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
@@ -1160,6 +1233,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         o.d_container = to_container ? static_cast<uint8_t *>(g.words.ptr) : nullptr;
         o.sub_base = (unsigned long long)f0 * channels;
         o.lossless = recoded ? &la : nullptr;
+        o.d_ref_words = ref_words ? d_ref_words : nullptr;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
                                    d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, o))
             return rc;
@@ -1216,11 +1290,13 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     }
     for (int i = 0; i < (verify ? kLanes : kEncLanes); i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.s_d2h));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, ref_words ? 24 : 16, cudaMemcpyDeviceToHost, g.s_d2h));
     CUDA_TRY(cudaStreamSynchronize(g.s_d2h));
     uint64_t used;
     memcpy(&used, g.h_small + 2, 8);
     *words_used = (size_t)used; // for CAPACITY: the size the caller needs
+    if (ref_words)
+        memcpy(ref_words, g.h_small + 4, 8);
     if (g.h_small[0] != 0)
         return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
     if (recoded)
@@ -1432,6 +1508,7 @@ struct DevicePart {
     char err[sizeof g_error] = "";
     std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
     std::vector<selab200_lossless_entry> recoded; // lossless calls: this block's re-coded pairs, file-global frames
+    unsigned long long ref_words = 0;             // search calls: the reference encoder's words of this block
 };
 
 static std::vector<DevicePart> device_parts(uint32_t n_frames)
@@ -1554,9 +1631,10 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
 }
 
 // Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.
+// `ref_words`: the order search, and the reference encoder's words of all blocks.
 static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
                          size_t *words_used, std::vector<selab200_verify_entry> *report,
-                         std::vector<selab200_lossless_entry> *recoded)
+                         std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr)
 {
     const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
@@ -1566,7 +1644,7 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
             block = EncodeTarget{t.form, true, t.descs ? t.descs + (size_t)p.f0 * channels : nullptr, nullptr, nullptr,
                                  selab200_encode_words_bound(p.nf, channels)};
         return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, &p.used, p.f0, report ? &p.report : nullptr,
-                           recoded ? &p.recoded : nullptr);
+                           recoded ? &p.recoded : nullptr, ref_words ? &p.ref_words : nullptr);
     });
     if (report)
         *report = std::move(b.report);
@@ -1576,6 +1654,11 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
     for (const DevicePart &p : b.parts)
         total += p.used;
     *words_used = total;
+    if (ref_words) {
+        *ref_words = 0;
+        for (const DevicePart &p : b.parts)
+            *ref_words += p.ref_words;
+    }
     if (b.rc || !split)
         return b.rc;
     return place_blocks(b.parts, channels, t, total);
@@ -1618,6 +1701,24 @@ int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint3
     return deliver_records(rec, entries, capacity, n_entries);
 }
 
+int selab200_encode_frames_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                  size_t *words_used, size_t *ref_words)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !ref_words)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
+    unsigned long long ref = 0;
+    const int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr, &ref);
+    *ref_words = (size_t)ref;
+    return rc;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -1625,12 +1726,12 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 
 } // extern "C"
 
-// selab200_encode_container, and with `report` its verified form, with `recoded` its lossless form (g_mutex held
-// by the caller).
+// selab200_encode_container, and with `report` its verified form, with `recoded` its lossless form, with `ref_bytes`
+// its order-search form (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
                                  std::vector<selab200_verify_entry> *report,
-                                 std::vector<selab200_lossless_entry> *recoded)
+                                 std::vector<selab200_lossless_entry> *recoded, size_t *ref_bytes = nullptr)
 {
     if (int rc = require_ready())
         return rc;
@@ -1650,8 +1751,12 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     memcpy(container, header, sizeof header);
     size_t words_used = 0;
     const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4)};
-    const int rc = encode_blocks(pcm, n_frames, channels, t, &words_used, report, recoded);
+    unsigned long long ref_words = 0;
+    const int rc = encode_blocks(pcm, n_frames, channels, t, &words_used, report, recoded,
+                                 ref_bytes ? &ref_words : nullptr);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
+    if (ref_bytes)
+        *ref_bytes = (size_t)container_frame_byte(n_frames, channels, ref_words);
     return rc;
 }
 
@@ -1699,6 +1804,21 @@ int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, ui
                                        bytes_used, nullptr, &rec))
         return rc;
     return deliver_records(rec, entries, entries_capacity, n_entries);
+}
+
+int selab200_encode_container_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                                     uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
+                                     size_t *ref_bytes)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!ref_bytes) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    *ref_bytes = 0;
+    return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
+                                 nullptr, nullptr, ref_bytes);
 }
 
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -2143,6 +2263,68 @@ int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint3
     if (int rc = collect_records(d_count, nullptr, d_entries, n_sub, g.stream, rec))
         return rc;
     return deliver_records(rec, entries, entries_capacity, n_entries);
+}
+
+// For tests: one unpipelined order-search batch through encode_device, every unit's q[0..99] and reference order
+// taken from pred.
+int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                  size_t words_capacity, size_t *words_used, size_t *ref_words)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !pred || !descs || !words || !words_used || !ref_words)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    *words_used = 0;
+    *ref_words = 0;
+    if (n_frames == 0)
+        return 0;
+    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
+    for (size_t u = 0; u < n_units; u++) {
+        const int o = pred[u].order;
+        if (o < 1 || o > kMaxOrder)
+            return fail(SELAB200_ERR_RANGE, "order %d of unit %zu outside 1..%d", o, u, kMaxOrder);
+        for (int i = 0; i < kMaxOrder; i++)
+            if (pred[u].q[i] < -64 || pred[u].q[i] > 63)
+                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of unit %zu outside [-64, 63]", i, pred[u].q[i], u);
+    }
+    const size_t ws_bytes = selab200_encode_search_workspace_bytes(n_frames, channels);
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
+    if (int rc = g.work.ensure(ws_bytes)) return rc;
+    if (int rc = g.aux.ensure(n_units * sizeof(selab200_predictor))) return rc;
+    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
+    unsigned long long *d_ref = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
+    CUDA_TRY(cudaMemsetAsync(d_ref, 0, 8, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    EncodeOptions o;
+    o.d_ref_words = d_ref;
+    o.d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
+    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
+                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
+                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 24, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    uint64_t used, ref;
+    memcpy(&used, g.h_small + 2, 8);
+    memcpy(&ref, g.h_small + 4, 8);
+    *words_used = (size_t)used;
+    *ref_words = (size_t)ref;
+    if (g.h_small[0] != 0)
+        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (used > words_capacity)
+        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    return 0;
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

@@ -2,7 +2,8 @@
 //
 //   encode   k_unit_means<KIND> (lane per analysis unit: the mean of its samples)
 //            k_encode_units<STEREO> (warp per analysis unit: PCM -> ... -> Rice pack into a private slot; its
-//            CHECK instantiation also flags ties, and lossless.cuh re-codes flagged units through encode_unit)
+//            CHECK instantiation also flags ties, and lossless.cuh re-codes flagged units through encode_unit;
+//            search.cuh runs its kUnitSearch mode and codes other orders on the staged signal of stage_unit)
 //            k_encode_sizes + k_encode_scan (stereo decision, prefix sum, descriptors)
 //            k_encode_gather / k_encode_gather_container (slot -> word arena / .sela byte stream)
 //   decode   k_container_unpack (.sela bytes -> word arena)
@@ -229,36 +230,36 @@ struct RepairUnit {
 };
 constexpr unsigned long long kNoCandidate = ~0ull;
 
+// ---- order search (DESIGN.md 7.3) ----
+// What the search's analysis leaves per unit for the candidate kernels (search.cuh): all 100 quantised reflection
+// coefficients, the reference encoder's order and its words (reflection + residue), and the best order so far as the
+// key words << 8 | (order == ref_order ? 0 : order), so that one atomicMin keeps the fewest words and, between equal
+// words, the reference order, else the lowest.  q is kept as int32, as the quantiser produces it.
+struct __align__(16) SearchUnit {
+    int32_t q[kMaxOrder];
+    uint32_t ref_order, ref_words;
+    unsigned long long best;
+};
+static_assert(sizeof(SearchUnit) == 416, "SearchUnit layout");
+
 // What encode_unit does with the unit:
 //   kUnitEncode     analyse, FIR, Rice, pack into the unit's slot and write its record (production)
 //   kUnitCheck      kUnitEncode, and bit 1 of the record's flags when the FIR has a tie
 //   kUnitCandidate  analyse, apply candidate `cand`, FIR with the tie check, Rice sizes: a tie-free candidate enters
 //                   ru->best; nothing is packed
 //   kUnitRepack     analyse, apply candidate `cand`, FIR, Rice, pack into the unit's slot and rewrite its record
-enum { kUnitEncode = 0, kUnitCheck = 1, kUnitCandidate = 2, kUnitRepack = 3 };
+//   kUnitSearch     kUnitEncode with the tie check, and su[unit] filled in: every q, the reference order and words,
+//                   and as the best so far the reference order, if it has no tie
+enum { kUnitEncode = 0, kUnitCheck = 1, kUnitCandidate = 2, kUnitRepack = 3, kUnitSearch = 4 };
 
-// The work of one analysis unit by one warp.
-// TRACE (tests only, selab200_encode_trace): also copies the unit's analysis intermediates to trace[unit] as they
-// are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.
-// FORCE (tests only, selab200_encode_lossless_forced): the unit is coded with the predictor pred[unit] in place of the
-// one its analysis chose; every step after the quantiser, the repair's edits included, runs as in production.
-template <bool STEREO, bool TRACE, int MODE, bool FORCE = false>
-__device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_analysis_trace *trace, const uint32_t unit,
-                                            RepairUnit *ru, uint32_t cand, const selab200_predictor *pred = nullptr)
+// Stages the signal of analysis unit `unit` at smem, as one planar int16 row with kHistoryPad zeros in front (for a
+// stereo difference d = ch0 - ch1: d >> 1 in the row, d & 1 in the bit array behind it).
+template <bool STEREO>
+__device__ __forceinline__ Signal stage_unit(const EncodeParams &p, const uint32_t unit, unsigned char *smem)
 {
     constexpr int kRow = kHistoryPad + kFrame;
-    constexpr int kLoWords = (kHistoryPad + kFrame) / 32; // parity bits of a difference signal
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    int16_t *s16 = reinterpret_cast<int16_t *>(smem_raw);                    // [pad + 2048]
-    uint32_t *lo_bits = reinterpret_cast<uint32_t *>(smem_raw + kRow * 2);    // [pad/32 + 64] (stereo only)
-    constexpr size_t kSigBytes = kRow * 2 + (STEREO ? kLoWords * 4 : 0);
-    AnalysisScratch &scratch = *reinterpret_cast<AnalysisScratch *>(smem_raw + kSigBytes);
-    // The predictor lives in the part of the analysis scratch that is dead once the Schur recursion has taken
-    // the autocorrelation into registers (the tail of the ring and ac[]): 7.7 instead of 9 KB per unit, 29
-    // instead of 23 units per SM.
-    static_assert(kCoefAlias + sizeof(CoefSmem) <= sizeof(AnalysisScratch) && kCoefAlias % 16 == 0, "predictor alias");
-    CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kCoefAlias);
-
+    int16_t *s16 = reinterpret_cast<int16_t *>(smem);                    // [pad + 2048]
+    uint32_t *lo_bits = reinterpret_cast<uint32_t *>(smem + kRow * 2);    // [pad/32 + 64] (stereo only)
     const int lane = lane_id();
     const uint32_t frame = STEREO ? unit / 3 : unit / p.channels;
     const uint32_t role = STEREO ? unit % 3 : unit % p.channels; // stereo: 0 ch0, 1 ch1, 2 ch0-ch1
@@ -309,6 +310,39 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
             row[j] = src[(size_t)j * p.channels + role];
     }
     __syncwarp();
+    return sig;
+}
+
+// Shared memory of the signal staged by stage_unit.
+template <bool STEREO>
+__host__ __device__ constexpr size_t unit_signal_bytes()
+{
+    return (size_t)(kHistoryPad + kFrame) * 2 + (STEREO ? (kHistoryPad + kFrame) / 8 : 0);
+}
+
+// The work of one analysis unit by one warp.
+// TRACE (tests only, selab200_encode_trace): also copies the unit's analysis intermediates to trace[unit] as they
+// are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.
+// FORCE (tests only, selab200_encode_lossless_forced): the unit is coded with the predictor pred[unit] in place of the
+// one its analysis chose; every step after the quantiser, the repair's edits included, runs as in production.
+// SEARCH (kUnitSearch only): the units' search records.
+template <bool STEREO, bool TRACE, int MODE, bool FORCE = false>
+__device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_analysis_trace *trace, const uint32_t unit,
+                                            RepairUnit *ru, uint32_t cand, const selab200_predictor *pred = nullptr,
+                                            SearchUnit *su = nullptr)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
+    AnalysisScratch &scratch = *reinterpret_cast<AnalysisScratch *>(smem_raw + kSigBytes);
+    // The predictor lives in the part of the analysis scratch that is dead once the Schur recursion has taken
+    // the autocorrelation into registers (the tail of the ring and ac[]): 7.7 instead of 9 KB per unit, 29
+    // instead of 23 units per SM.
+    static_assert(kCoefAlias + sizeof(CoefSmem) <= sizeof(AnalysisScratch) && kCoefAlias % 16 == 0, "predictor alias");
+    CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kCoefAlias);
+
+    const int lane = lane_id();
+    const uint32_t role = STEREO ? unit % 3 : unit % p.channels; // stereo: 0 ch0, 1 ch1, 2 ch0-ch1
+    const Signal sig = stage_unit<STEREO>(p, unit, smem_raw);
 
     // ---- analysis ----
     // the residue row: the unit's own, or in the repair (which runs several candidates of a unit at once) the warp's
@@ -360,10 +394,15 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
         if (lane == 0)
             tr.order = order;
     }
+    if constexpr (MODE == kUnitSearch) { // every q, from k[] (still intact) or as forced
+        for (int i = lane; i < kMaxOrder; i += 32)
+            su[unit].q[i] = FORCE ? cf.q[i] : quantise_reflection(i, scratch.kk()[i]);
+        __syncwarp();
+    }
     // the digit planes of the FIR overlay k[] and the step-up row, dead now (the trace has copied k)
     static_assert(kPlaneBytes <= kCoefAlias, "FIR digit planes");
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
-    constexpr bool kCheck = MODE == kUnitCheck || MODE == kUnitCandidate;
+    constexpr bool kCheck = MODE == kUnitCheck || MODE == kUnitCandidate || MODE == kUnitSearch;
     bool tie;
     if (STEREO && role == 2)
         tie = warp_fir_residual<true, kCheck>(sig, cf, order, planes, res);
@@ -401,9 +440,15 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
         u.refl_words = cq.words;
         u.res_k = cr.k;
         u.res_words = cr.words;
-        u.flags = (too_large ? 1u : 0u) | (tie ? 2u : 0u); // 2: not lossless (kUnitCheck only)
+        u.flags = (too_large ? 1u : 0u) | (MODE != kUnitSearch && tie ? 2u : 0u); // 2: not lossless (kUnitCheck only)
         u.pad[0] = u.pad[1] = 0;
         p.units[unit] = u;
+        if constexpr (MODE == kUnitSearch) {
+            SearchUnit &s = su[unit];
+            s.ref_order = order;
+            s.ref_words = cq.words + cr.words;
+            s.best = tie ? kNoCandidate : (unsigned long long)(cq.words + cr.words) << 8;
+        }
     }
 }
 

@@ -1,0 +1,200 @@
+// search.cuh -- the kernels of the order search (sm_90a, DESIGN.md 7.3): every unit is coded at the predictor order
+// 1..100 with the fewest words whose FIR has no tie, inside the format.
+//
+//   k_search_units<S, FORCE>   the ordinary analysis kernel (encode_unit<kUnitSearch>): codes the unit at the
+//                              reference order into its slot, and leaves all 100 q, the reference order and its words
+//                              in the unit's SearchUnit
+//   k_search_candidates<S>     warp per (unit, slice of orders): carries one step-up forward through the slice's
+//                              orders; per order the FIR with the tie check and both Rice sizes; a tie-free order
+//                              enters the unit's atomicMin key
+//   k_search_repack<S>         warp per unit whose winner is not the reference order: the winner packed into the
+//                              unit's slot, record rewritten
+//   k_search_ref_words         thread per frame: the words the reference encoder's choice takes (its orders, its
+//                              stereo decision), summed into one counter
+// Then k_encode_sizes / k_encode_scan / k_encode_gather(_container) run as for every encode, and the stereo decision
+// there sees the searched sizes.  The candidate and repack kernels have grids of a fixed size and loop over the work.
+#pragma once
+
+#include "kernels.cuh"
+
+namespace selab200 {
+
+// The orders 1..100 in slices of about equal work, one warp per (unit, slice).  An order costs its FIR k-steps
+// ((order + 8) / 32 rounded up: 1 up to order 24, then 2, 3, 4) and two Rice sizings, which cost about a k-step
+// together; a slice also repeats the step-up of the orders below it, which is small beside these.
+constexpr int kSearchSlices = 4;
+__host__ __device__ constexpr int search_slice_first(int s) // first order of slice s; s = kSearchSlices: 101
+{
+    return s == 0 ? 1 : s == 1 ? 41 : s == 2 ? 65 : s == 3 ? 85 : kMaxOrder + 1;
+}
+
+// Shared memory of a search warp: the signal as stage_unit stages it, the step-up row, the predictor and the FIR's
+// digit planes.
+constexpr size_t kSearchStepBytes = 104 * sizeof(double);
+template <bool STEREO>
+constexpr size_t search_smem_bytes()
+{
+    return unit_signal_bytes<STEREO>() + kSearchStepBytes + sizeof(CoefSmem) + kPlaneBytes;
+}
+
+// One iteration i of the step-up of warp_coefficients (the same operations in the same order): afterwards t[0..i]
+// is the predictor of order i + 1, for i >= 1.
+__device__ __forceinline__ void step_up(double *t, int i, int q)
+{
+    const int lane = lane_id();
+    const double ki = dequantise(i, q);
+    const int half = i >> 1;
+    for (int j = lane; j < half; j += 32) {
+        double a = t[j];
+        double b = t[i - 1 - j];
+        t[j] = dadd(a, dmul(ki, b));
+        t[i - 1 - j] = dadd(b, dmul(ki, a));
+    }
+    if (lane == 0) {
+        if (i & 1) {
+            double mid = t[half];
+            t[half] = dadd(mid, dmul(mid, ki));
+        }
+        t[i] = ki;
+    }
+    __syncwarp();
+}
+
+// Unit `unit` at the orders o_lo..o_hi, one after the other, on one carried step-up.  The order-1 predictor is zero
+// (linear_predictor.cpp:19-22), not row 0 of the step-up.  res: the warp's residue row.
+//   PACK = false  every order but the reference order (the analysis kernel has sized that one): FIR with the tie
+//                 check, Rice sizes, a tie-free order into su[unit].best
+//   PACK = true   (o_lo = o_hi) FIR, Rice, pack into the unit's slot and rewrite its record
+template <bool STEREO, bool PACK>
+__device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
+                                              int o_hi, int32_t *res)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
+    double *t = reinterpret_cast<double *>(smem_raw + kSigBytes);
+    CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kSearchStepBytes);
+    uint32_t *planes = reinterpret_cast<uint32_t *>(smem_raw + kSigBytes + kSearchStepBytes + sizeof(CoefSmem));
+    static_assert(kSearchStepBytes % 16 == 0 && sizeof(CoefSmem) % 16 == 0, "search shared memory layout");
+
+    const int lane = lane_id();
+    const bool wide = STEREO && unit % 3 == 2;
+    const Signal sig = stage_unit<STEREO>(p, unit, smem_raw);
+    SearchUnit &s = su[unit];
+    const int ref = (int)s.ref_order;
+    for (int i = lane; i < 104; i += 32)
+        cf.q[i] = i < kMaxOrder ? s.q[i] : 0;
+    for (int i = lane; i < 112; i += 32) {
+        cf.clo[i] = 0;
+        cf.chi[i] = 0;
+    }
+    __syncwarp();
+    const double scale = 34359738368.0; // 2^35
+    int done = 0;                       // step-up iterations applied to t
+    for (int o = o_lo; o <= o_hi; o++) {
+        if (!PACK && o == ref)
+            continue;
+        if (o >= 2) {
+            for (; done < o; done++)
+                step_up(t, done, cf.q[done]);
+            for (int m = lane; m < o; m += 32) {
+                const long long v = __double2ll_rz(dmul(scale, -t[m]));
+                cf.clo[m] = (uint32_t)v;
+                cf.chi[m] = (int32_t)(v >> 32);
+            }
+            __syncwarp();
+        }
+        const bool tie = wide ? warp_fir_residual<true, !PACK>(sig, cf, o, planes, res)
+                              : warp_fir_residual<false, !PACK>(sig, cf, o, planes, res);
+        const RiceChoice cq = warp_rice_choose(cf.q, o);
+        const RiceChoice cr = warp_rice_choose(res, kFrame);
+        if constexpr (!PACK) {
+            const unsigned long long words = cq.words + cr.words;
+            if (lane == 0 && !tie)
+                atomicMin(&s.best, words << 8 | (unsigned long long)o);
+        } else {
+            const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
+            if (!too_large) {
+                uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
+                warp_rice_pack(cf.q, o, cq, slot);
+                warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
+            }
+            if (lane == 0) {
+                UnitRecord u;
+                u.order = o;
+                u.refl_k = cq.k;
+                u.refl_words = cq.words;
+                u.res_k = cr.k;
+                u.res_words = cr.words;
+                u.flags = too_large ? 1u : 0u;
+                u.pad[0] = u.pad[1] = 0;
+                p.units[unit] = u;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// The search's analysis kernel: encode_unit for unit blockIdx.x.  FORCE and `pred` (tests only,
+// selab200_encode_search_forced): the unit's q[0..99] and reference order are pred[unit]'s.
+template <bool STEREO, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_search_units(EncodeParams p, const selab200_predictor *pred, SearchUnit *su)
+{
+    encode_unit<STEREO, false, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su);
+}
+
+// Work item w = (unit w / kSearchSlices, slice w % kSearchSlices): the slices of a unit go to neighbouring warps,
+// which read the same PCM.  Residue row = the warp's (the grid is at most the batch's units).
+template <bool STEREO>
+__global__ void __launch_bounds__(32) k_search_candidates(EncodeParams p, SearchUnit *su)
+{
+    const size_t work = (size_t)encode_units(p.n_frames, p.channels) * kSearchSlices;
+    int32_t *res = p.residues + (size_t)blockIdx.x * kFrame;
+    for (size_t w = blockIdx.x; w < work; w += gridDim.x) {
+        const int sl = (int)(w % kSearchSlices);
+        __syncwarp();
+        search_orders<STEREO, false>(p, su, (uint32_t)(w / kSearchSlices), search_slice_first(sl),
+                                     search_slice_first(sl + 1) - 1, res);
+    }
+    __syncwarp();
+    for (int l = lane_id(); l < kFrame * 4 / 128; l += 32) // the row only ever lived in L2
+        asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
+}
+
+template <bool STEREO>
+__global__ void __launch_bounds__(32) k_search_repack(EncodeParams p, SearchUnit *su)
+{
+    const uint32_t n = encode_units(p.n_frames, p.channels);
+    int32_t *res = p.residues + (size_t)blockIdx.x * kFrame;
+    for (uint32_t u = blockIdx.x; u < n; u += gridDim.x) {
+        const int o = (int)(su[u].best & 0xffu);
+        if (o == 0 || o > kMaxOrder) // the reference order won (its slot and record stand); > 100: no tie-free
+            continue;                // order, which cannot happen (order 1 has none)
+        __syncwarp();
+        search_orders<STEREO, true>(p, su, u, o, o, res);
+    }
+}
+
+// The words of the reference encoder's subframes of each frame (its orders, its stereo decision: difference iff
+// strictly fewer words) into *ref_words.
+__global__ void __launch_bounds__(256) k_search_ref_words(EncodeParams p, const SearchUnit *su,
+                                                          unsigned long long *ref_words)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long w = 0;
+    if (f < p.n_frames) {
+        if (p.channels == 2) {
+            const SearchUnit *fs = su + (size_t)f * 3;
+            const uint32_t a = fs[1].ref_words, d = fs[2].ref_words;
+            w = (unsigned long long)fs[0].ref_words + (d < a ? d : a);
+        } else {
+            const SearchUnit *fs = su + (size_t)f * p.channels;
+            for (uint32_t c = 0; c < p.channels; c++)
+                w += fs[c].ref_words;
+        }
+    }
+    w = warp_sum_u64(w);
+    if (lane_id() == 0 && w)
+        atomicAdd(ref_words, w);
+}
+
+} // namespace selab200

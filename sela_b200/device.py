@@ -67,6 +67,21 @@ class DeviceCodec:
         rec = self.ll_entries.cpu().numpy().view(LOSSLESS_DTYPE)[:self.n_sub]
         return rec[rec["words"] != 0].copy()
 
+    def encode_search(self, pcm):
+        """encode with the order search (DESIGN.md 7.3).  Asynchronous; self.ref_words (int64 cuda tensor) receives
+        the words encode() writes for the same frames.  The search workspace is allocated on first use."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.numel() == self.n_sub * FRAME
+        L = lib()
+        if not hasattr(self, "search_ws"):
+            self.search_ws_bytes = L.selab200_encode_search_workspace_bytes(self.n_frames, self.channels)
+            self.search_ws = torch.zeros(self.search_ws_bytes, dtype=torch.uint8, device=self.device)
+            self.ref_words = torch.zeros(1, dtype=torch.int64, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_encode_frames_search_device(
+            pcm.data_ptr(), self.n_frames, self.channels, self.descs.data_ptr(), self.words.data_ptr(),
+            self.capacity, self.words_used.data_ptr(), self.ref_words.data_ptr(), self.status.data_ptr(),
+            self.search_ws.data_ptr(), self.search_ws_bytes, C.c_void_p(stream)))
+
     def decode(self, pcm_out, n_words):
         """Decode self.descs / self.words[:n_words] into pcm_out (int16 cuda tensor). Asynchronous."""
         assert pcm_out.dtype == torch.int16 and pcm_out.is_cuda and pcm_out.numel() == self.n_sub * FRAME

@@ -122,7 +122,8 @@ struct RecodedEntry {
 class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
-    void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded);
+    void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
+                  size_t *refBytes = nullptr);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -141,6 +142,11 @@ public:
     // reference decoder (selab200_encode_container_lossless).  Frames without a tie keep processTo()'s bytes;
     // `recoded` receives every (frame, channel) coded differently, in order.
     void processLosslessTo(std::ofstream &outputFile, std::vector<RecodedEntry> &recoded);
+    // Not in the reference: processTo() writing a smaller file at a higher encode cost: every subframe at the
+    // predictor order with the fewest words whose FIR has no tie (selab200_encode_container_search), so it also
+    // decodes back to its source under the unmodified reference decoder.  Returns the bytes written; `refBytes`
+    // receives the bytes processTo() writes for the same input.
+    size_t processSearchTo(std::ofstream &outputFile, size_t &refBytes);
 };
 class Decoder {
     void readFrames();

@@ -7,6 +7,9 @@
 // source, 2 when some do not (one stderr line per (frame, channel), then a summary), 1 on errors.
 // `-L in.wav out.sela`: a lossless encode (a file that decodes back to the WAV under the reference decoder, the same
 // bytes as -e where -e's already do), one line with the number of re-coded subframes.
+// `-S in.wav out.sela`: a smaller file at a higher encode cost (every subframe at the predictor order with the fewest
+// words, and decoding back to the WAV under the reference decoder), one line with the bytes written and the bytes -e
+// writes.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -98,6 +101,8 @@ int usage(const std::string &prog)
               << " -V path/to/input.wav path/to/output.sela\n\n"
               << "Encoding a file so that it decodes back to the input (H100 build):\n" << prog
               << " -L path/to/input.wav path/to/output.sela\n\n"
+              << "Encoding a file smaller, searching every subframe's predictor order (H100 build):\n" << prog
+              << " -S path/to/input.wav path/to/output.sela\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -164,6 +169,13 @@ int main(int argc, char **argv)
             std::vector<sela::RecodedEntry> recoded;
             sela::Encoder(in).processLosslessTo(out, recoded);
             std::cout << "Re-coded " << recoded.size() << " subframes" << std::endl;
+        } else if (mode == "-S" && argc == 4) {
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Encoding with the order search: " << argv[2] << std::endl;
+            size_t refBytes = 0;
+            const size_t written = sela::Encoder(in).processSearchTo(out, refBytes);
+            std::cout << "Wrote " << written << " bytes (-e: " << refBytes << " bytes)" << std::endl;
         } else if (mode == "-t" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ifstream wav(argv[3], std::ios::binary);

@@ -796,9 +796,17 @@ void Encoder::processLosslessTo(std::ofstream &outputFile, std::vector<RecodedEn
     encodeTo(outputFile, nullptr, &recoded);
 }
 
+size_t Encoder::processSearchTo(std::ofstream &outputFile, size_t &refBytes)
+{
+    const std::streampos at = outputFile.tellp();
+    encodeTo(outputFile, nullptr, nullptr, &refBytes);
+    return (size_t)(outputFile.tellp() - at);
+}
+
 // processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
-// selab200_encode_container_lossless.
-void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded)
+// selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search.
+void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
+                       size_t *refBytes)
 {
     if (report)
         report->clear();
@@ -828,6 +836,8 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         raise("sela_b200: too many frames");
     if (n_frames == 0) { // header only, as SelaFile::writeToFile does for an empty frame list
         file::SelaFile(w.fmt.sampleRate, w.fmt.bitsPerSample, (uint8_t)channels, {}).writeToFile(outputFile);
+        if (refBytes)
+            *refBytes = 15;
         return;
     }
     const size_t cap = selab200_container_bound((uint32_t)n_frames, channels);
@@ -851,6 +861,11 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         for (size_t i = 0; i < n && i < raw.size(); i++)
             recoded->push_back(RecodedEntry{raw[i].frame, raw[i].channel, raw[i].ref_order, raw[i].order,
                                             raw[i].ref_words, raw[i].words});
+    } else if (refBytes) {
+        Phase p("order-search encode (device)");
+        check(selab200_encode_container_search(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                               (uint32_t)n_frames, channels, w.fmt.sampleRate, w.fmt.bitsPerSample,
+                                               out, cap, &used, refBytes));
     } else {
         Phase p("encode (device)");
         check(selab200_encode_container(reinterpret_cast<const int16_t *>(file.data + dat.body), (uint32_t)n_frames,
