@@ -456,6 +456,43 @@ int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_
                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                   size_t words_capacity, size_t *words_used, size_t *ref_words);
 
+/* One candidate order of one analysis unit in the order search, as the search sized it.  32 bytes, naturally
+ * aligned.  With K = 0x9E3779B97F4A7C15 and K2 = 0xD6E8FEB86659FD93, all sums mod 2^64:
+ *   pred_digest = sum_{j=1..100} (c[j] + j * K2) * K, c the Q35 predictor the FIR ran (zero past the order);
+ *   res_digest  = sum_{i<2048} ((i << 32) | (uint32)r[i]) * K, r the residues.
+ * Every term is a bijection of its element, so any one changed coefficient or residue changes the digest. */
+typedef struct selab200_search_trace {
+    uint64_t pred_digest;
+    uint64_t res_digest;
+    uint32_t res_words;  /* residue Rice words                                               */
+    uint32_t visits;     /* how many times the order was sized (atomic): 1                   */
+    uint16_t refl_words; /* reflection-coefficient Rice words                                */
+    uint8_t  refl_k;     /* reflection-coefficient Rice parameter                            */
+    uint8_t  res_k;      /* residue Rice parameter                                           */
+    uint8_t  tie;        /* 1 if the FIR has a tie at any output                             */
+    uint8_t  reserved[3];
+} selab200_search_trace;
+
+/* What the order search's analysis left for one analysis unit: every quantised reflection coefficient, the
+ * reference encoder's order and its words, and the winner's key words << 8 | (order == ref_order ? 0 : order).
+ * 416 bytes. */
+typedef struct selab200_search_unit {
+    int32_t  q[100];
+    uint32_t ref_order;
+    uint32_t ref_words;
+    uint64_t best;
+} selab200_search_unit;
+
+/* For tests: selab200_encode_frames_search on one device and one batch (selab200_encode_search_forced's when pred
+ * is not NULL), through the tracing instantiations of the search kernels.  trace[unit * 100 + order - 1] receives
+ * the record of every analysis unit at every order 1..100: the reference order's from the analysis kernel, every
+ * other order's from the candidate kernel.  units[unit] receives the unit's search record once the candidates have
+ * run.  descs, words, *words_used and *ref_words as selab200_encode_frames_search. */
+int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                 const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                 size_t words_capacity, size_t *words_used, size_t *ref_words,
+                                 selab200_search_unit *units, selab200_search_trace *trace);
+
 #ifdef __cplusplus
 }
 #endif

@@ -55,6 +55,18 @@ assert LOSSLESS_DTYPE.itemsize == 16
 PREDICTOR_DTYPE = np.dtype([("order", "<i4"), ("q", "<i4", (100,))], align=True)
 assert PREDICTOR_DTYPE.itemsize == 404
 
+# mirrors selab200_search_trace, 32 bytes
+SEARCH_TRACE_DTYPE = np.dtype([
+    ("pred_digest", "<u8"), ("res_digest", "<u8"), ("res_words", "<u4"), ("visits", "<u4"), ("refl_words", "<u2"),
+    ("refl_k", "u1"), ("res_k", "u1"), ("tie", "u1"), ("reserved", "u1", (3,)),
+], align=True)
+assert SEARCH_TRACE_DTYPE.itemsize == 32
+
+# mirrors selab200_search_unit, 416 bytes
+SEARCH_UNIT_DTYPE = np.dtype([("q", "<i4", (100,)), ("ref_order", "<u4"), ("ref_words", "<u4"), ("best", "<u8")],
+                             align=True)
+assert SEARCH_UNIT_DTYPE.itemsize == 416
+
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
 
@@ -118,6 +130,7 @@ _SIGNATURES = {
     "selab200_fir_tie_probe": (_I, [_V, _V, _V, _U32, _I, _V, _V]),
     "selab200_encode_lossless_forced": (_I, [_V, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _SZ, _V]),
     "selab200_encode_search_forced": (_I, [_V, _U32, _U32, _V, _V, _V, _SZ, _V, _V]),
+    "selab200_encode_search_trace": (_I, [_V, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _V, _V]),
 }
 
 

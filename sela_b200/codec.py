@@ -36,8 +36,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, LOSSLESS_DTYPE, MAX_ORDER, PREDICTOR_DTYPE, TRACE_DTYPE,  # noqa: F401
-                   VERIFY_DTYPE, SelaB200Error, check, init, lib)
+from ._lib import (DESC_DTYPE, FRAME, INFO_DTYPE, LOSSLESS_DTYPE, MAX_ORDER, PREDICTOR_DTYPE,  # noqa: F401
+                   SEARCH_TRACE_DTYPE, SEARCH_UNIT_DTYPE, TRACE_DTYPE, VERIFY_DTYPE, SelaB200Error, check, init, lib)
 
 
 def _c(a, dtype):
@@ -413,7 +413,18 @@ def encode_search_forced(pcm, channels, predictors, device=0):
     encode_trace's unit order) instead of its analysis -> (descs, words, ref_words)."""
     init(device)
     pcm, n_frames = _whole_frames(pcm, channels)
-    n_units = n_frames * (3 if channels == 2 else channels)
+    pred = _search_predictors(predictors, n_frames * (3 if channels == 2 else channels))
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
+                                          words.ctypes.data, cap, C.addressof(used), C.addressof(ref)))
+    return descs, words[:used.value].copy(), ref.value
+
+
+def _search_predictors(predictors, n_units):
     if isinstance(predictors, np.ndarray) and predictors.dtype == PREDICTOR_DTYPE:
         pred = _c(predictors, PREDICTOR_DTYPE)
     else:
@@ -423,11 +434,28 @@ def encode_search_forced(pcm, channels, predictors, device=0):
             rec["q"][:] = np.asarray(q)[:MAX_ORDER]
     if pred.size != n_units:
         raise ValueError("%d predictors for %d analysis units" % (pred.size, n_units))
+    return pred
+
+
+def encode_search_trace(pcm, channels, predictors=None, device=0):
+    """encode_frames_search (encode_search_forced's with `predictors`) on one batch through the tracing search
+    kernels -> (descs, words, ref_words, units, trace).
+
+    units: SEARCH_UNIT_DTYPE[n_units], every analysis unit's q[100], reference order and words and winning key;
+    trace: SEARCH_TRACE_DTYPE[n_units, 100], the record of every unit at every order 1..100 (column order - 1).
+    Units in encode_trace's order."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    n_units = n_frames * (3 if channels == 2 else channels)
+    pred = None if predictors is None else _search_predictors(predictors, n_units)
     L = lib()
     cap = L.selab200_encode_words_bound(n_frames, channels)
     descs = np.zeros(n_frames * channels, DESC_DTYPE)
     words = np.empty(max(cap, 1), np.uint32)
+    units = np.zeros(n_units, SEARCH_UNIT_DTYPE)
+    trace = np.zeros((n_units, MAX_ORDER), SEARCH_TRACE_DTYPE)
     used, ref = C.c_size_t(0), C.c_size_t(0)
-    check(L.selab200_encode_search_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
-                                          words.ctypes.data, cap, C.addressof(used), C.addressof(ref)))
-    return descs, words[:used.value].copy(), ref.value
+    check(L.selab200_encode_search_trace(pcm.ctypes.data, n_frames, channels, None if pred is None else pred.ctypes.data,
+                                         descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
+                                         C.addressof(ref), units.ctypes.data, trace.ctypes.data))
+    return descs, words[:used.value].copy(), ref.value, units, trace

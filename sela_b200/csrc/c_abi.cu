@@ -347,10 +347,13 @@ int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames,
 
 // The order search (search.cuh) in place of k_encode_units: analysis, candidates, repack, and the reference encoder's
 // words added to *d_ref_words.  The warp kernels have grids of a fixed size, at most one residue row per unit of the
-// batch.  FORCE: the units' q and reference orders are d_pred's (selab200_encode_search_forced).
+// batch.  FORCE: the units' q and reference orders are d_pred's (selab200_encode_search_forced).  d_trace: the
+// analysis and candidate kernels are their tracing instantiations, which write every (unit, order) record there
+// (selab200_encode_search_trace).
 template <bool STEREO, bool FORCE = false>
 int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t n_units,
-                  unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred = nullptr)
+                  unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred = nullptr,
+                  selab200_search_trace *d_trace = nullptr)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
     if (int rc = set_smem(k_search_units<STEREO, FORCE>, smem))
@@ -359,11 +362,22 @@ int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t
         return rc;
     if (int rc = set_smem(k_search_repack<STEREO>, smem_orders))
         return rc;
-    k_search_units<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su);
+    if (d_trace) {
+        if (int rc = set_smem(k_search_units_trace<STEREO, FORCE>, smem))
+            return rc;
+        if (int rc = set_smem(k_search_candidates_trace<STEREO>, smem_orders))
+            return rc;
+        k_search_units_trace<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su, d_trace);
+    } else {
+        k_search_units<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su);
+    }
     if (int rc = launch_check("k_search_units"))
         return rc;
     const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
-    k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
+    if (d_trace)
+        k_search_candidates_trace<STEREO><<<warps, 32, smem_orders, stream>>>(p, su, d_trace);
+    else
+        k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
     if (int rc = launch_check("k_search_candidates"))
         return rc;
     k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
@@ -399,6 +413,8 @@ struct EncodeOptions {
                                                 // words here
     const selab200_predictor *d_pred = nullptr; // lossless or search only: every unit's predictor
                                                 // (selab200_encode_lossless_forced / selab200_encode_search_forced)
+    selab200_search_trace *d_search_trace = nullptr; // search only: the tracing search kernels write every
+                                                     // (unit, order) record here
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -467,10 +483,12 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     } else if (o.d_ref_words) {
         SearchUnit *su = reinterpret_cast<SearchUnit *>(static_cast<char *>(d_ws) +
                                                         align256(selab200_encode_workspace_bytes(n_frames, channels)));
-        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, o.d_ref_words, stream, o.d_pred)
-                                          : launch_search<false, true>(p, su, n_frames, n_units, o.d_ref_words, stream, o.d_pred))
-                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, o.d_ref_words, stream)
-                                          : launch_search<false>(p, su, n_frames, n_units, o.d_ref_words, stream));
+        unsigned long long *rw = o.d_ref_words;
+        selab200_search_trace *tr = o.d_search_trace;
+        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr)
+                                          : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr))
+                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr)
+                                          : launch_search<false>(p, su, n_frames, n_units, rw, stream, nullptr, tr));
         if (rc)
             return rc;
     } else {
@@ -2265,16 +2283,22 @@ int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint3
     return deliver_records(rec, entries, entries_capacity, n_entries);
 }
 
-// For tests: one unpipelined order-search batch through encode_device, every unit's q[0..99] and reference order
-// taken from pred.
-int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
-                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
-                                  size_t words_capacity, size_t *words_used, size_t *ref_words)
+static_assert(sizeof(selab200_search_trace) == 32, "selab200_search_trace layout (include/sela_b200.h)");
+static_assert(sizeof(selab200_search_unit) == sizeof(SearchUnit) &&
+                  offsetof(selab200_search_unit, ref_order) == offsetof(SearchUnit, ref_order) &&
+                  offsetof(selab200_search_unit, best) == offsetof(SearchUnit, best),
+              "selab200_search_unit mirrors SearchUnit");
+
+// For tests: one unpipelined order-search batch through encode_device.  pred (required when `forced`): every unit's
+// q[0..99] and reference order.  units, trace (both or neither): the search records and the tracing kernels' records.
+static int encode_search_batch(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const selab200_predictor *pred,
+                               selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                               size_t *words_used, size_t *ref_words, selab200_search_unit *units,
+                               selab200_search_trace *trace)
 {
-    std::lock_guard<std::mutex> lock(g_mutex);
     if (int rc = require_ready())
         return rc;
-    if (!pcm || !pred || !descs || !words || !words_used || !ref_words)
+    if (!pcm || !descs || !words || !words_used || !ref_words)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     if (int rc = check_channels(channels))
         return rc;
@@ -2283,7 +2307,7 @@ int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_
     if (n_frames == 0)
         return 0;
     const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    for (size_t u = 0; u < n_units; u++) {
+    for (size_t u = 0; pred && u < n_units; u++) {
         const int o = pred[u].order;
         if (o < 1 || o > kMaxOrder)
             return fail(SELAB200_ERR_RANGE, "order %d of unit %zu outside 1..%d", o, u, kMaxOrder);
@@ -2292,24 +2316,37 @@ int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_
                 return fail(SELAB200_ERR_RANGE, "q[%d] = %d of unit %zu outside [-64, 63]", i, pred[u].q[i], u);
     }
     const size_t ws_bytes = selab200_encode_search_workspace_bytes(n_frames, channels);
+    const size_t pred_bytes = pred ? align256(n_units * sizeof(selab200_predictor)) : 0;
+    const size_t trace_bytes = trace ? n_units * kMaxOrder * sizeof(selab200_search_trace) : 0;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
     if (int rc = g.work.ensure(ws_bytes)) return rc;
-    if (int rc = g.aux.ensure(n_units * sizeof(selab200_predictor))) return rc;
+    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
     int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
     uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
     unsigned long long *d_ref = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
+    selab200_search_trace *d_trace =
+        trace ? reinterpret_cast<selab200_search_trace *>(static_cast<char *>(g.aux.ptr) + pred_bytes) : nullptr;
     CUDA_TRY(cudaMemsetAsync(d_ref, 0, 8, g.stream));
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    if (pred)
+        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    if (trace)
+        CUDA_TRY(cudaMemsetAsync(d_trace, 0, trace_bytes, g.stream));
     EncodeOptions o;
     o.d_ref_words = d_ref;
-    o.d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
+    o.d_pred = pred ? static_cast<const selab200_predictor *>(g.aux.ptr) : nullptr;
+    o.d_search_trace = d_trace;
     if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
                                static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
                                words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
         return rc;
+    if (trace) { // the search records lie behind the encode workspace (encode_device)
+        const char *su = static_cast<const char *>(g.work.ptr) + align256(selab200_encode_workspace_bytes(n_frames, channels));
+        CUDA_TRY(cudaMemcpyAsync(units, su, n_units * sizeof(SearchUnit), cudaMemcpyDeviceToHost, g.stream));
+        CUDA_TRY(cudaMemcpyAsync(trace, d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
+    }
     CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 24, cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaStreamSynchronize(g.stream));
@@ -2325,6 +2362,29 @@ int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_
     CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaStreamSynchronize(g.stream));
     return 0;
+}
+
+int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                  size_t words_capacity, size_t *words_used, size_t *ref_words)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!pred)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    return encode_search_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, ref_words,
+                               nullptr, nullptr);
+}
+
+int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                 const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                 size_t words_capacity, size_t *words_used, size_t *ref_words,
+                                 selab200_search_unit *units, selab200_search_trace *trace)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!units || !trace)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    return encode_search_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, ref_words,
+                               units, trace);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

@@ -242,6 +242,37 @@ struct __align__(16) SearchUnit {
 };
 static_assert(sizeof(SearchUnit) == 416, "SearchUnit layout");
 
+// The search trace (tests only, selab200_encode_search_trace): the record of unit `unit` at order o, written by the
+// warp that sized that order, once its FIR (predictor cf, residues res, tie) and both Rice choices are done.  The
+// digests are those of include/sela_b200.h, over c[1..100] as the FIR read them and the whole residue row.
+constexpr unsigned long long kDigestK = 0x9E3779B97F4A7C15ull, kDigestK2 = 0xD6E8FEB86659FD93ull;
+__device__ __noinline__ void search_trace_record(selab200_search_trace *trace, uint32_t unit, int o,
+                                                 const CoefSmem &cf, const int32_t *res, bool tie, RiceChoice cq,
+                                                 RiceChoice cr)
+{
+    const int lane = lane_id();
+    __syncwarp();
+    unsigned long long dp = 0, dr = 0;
+    for (int j = lane + 1; j <= kMaxOrder; j += 32)
+        dp += ((unsigned long long)coef_at(cf, j) + (unsigned long long)j * kDigestK2) * kDigestK;
+    for (int i = lane; i < kFrame; i += 32)
+        dr += ((unsigned long long)i << 32 | (uint32_t)res[i]) * kDigestK;
+    dp = warp_sum_u64(dp);
+    dr = warp_sum_u64(dr);
+    if (lane == 0) {
+        selab200_search_trace &r = trace[(size_t)unit * kMaxOrder + (o - 1)];
+        r.pred_digest = dp;
+        r.res_digest = dr;
+        r.res_words = cr.words;
+        r.refl_words = (uint16_t)cq.words;
+        r.refl_k = (uint8_t)cq.k;
+        r.res_k = (uint8_t)cr.k;
+        r.tie = tie ? 1 : 0;
+        atomicAdd(&r.visits, 1u);
+    }
+    __syncwarp();
+}
+
 // What encode_unit does with the unit:
 //   kUnitEncode     analyse, FIR, Rice, pack into the unit's slot and write its record (production)
 //   kUnitCheck      kUnitEncode, and bit 1 of the record's flags when the FIR has a tie
@@ -322,14 +353,15 @@ __host__ __device__ constexpr size_t unit_signal_bytes()
 
 // The work of one analysis unit by one warp.
 // TRACE (tests only, selab200_encode_trace): also copies the unit's analysis intermediates to trace[unit] as they
-// are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.
+// are produced.  Production runs TRACE = false, where none of it exists and `trace` is null.  In kUnitSearch
+// (selab200_encode_search_trace) TRACE writes the reference order's search record to strace instead.
 // FORCE (tests only, selab200_encode_lossless_forced): the unit is coded with the predictor pred[unit] in place of the
 // one its analysis chose; every step after the quantiser, the repair's edits included, runs as in production.
 // SEARCH (kUnitSearch only): the units' search records.
 template <bool STEREO, bool TRACE, int MODE, bool FORCE = false>
 __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_analysis_trace *trace, const uint32_t unit,
                                             RepairUnit *ru, uint32_t cand, const selab200_predictor *pred = nullptr,
-                                            SearchUnit *su = nullptr)
+                                            SearchUnit *su = nullptr, selab200_search_trace *strace = nullptr)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
@@ -350,7 +382,8 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
     // one lane loads the mean and the warp gets it by shuffle: a warp-wide load of p.means[unit] moves the unit
     // index out of the uniform registers, and the stereo kernel then needs 78 registers instead of 72
     warp_autocorrelation(sig, scratch, shfl_d(lane == 0 ? p.means[unit] : 0.0, 0));
-    if constexpr (TRACE) { // before warp_schur: the predictor overlays ac[] from warp_order_and_quantise on
+    constexpr bool kTraceAnalysis = TRACE && MODE != kUnitSearch;
+    if constexpr (kTraceAnalysis) { // before warp_schur: the predictor overlays ac[] from warp_order_and_quantise on
         selab200_analysis_trace &tr = trace[unit];
         if (lane == 0)
             tr.mean = p.means[unit];
@@ -383,7 +416,7 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
         order = e.order;
     }
     warp_coefficients(cf, scratch.t(), order);
-    if constexpr (TRACE) { // k[] (ring[0, 100)) is still intact: t[] and the predictor lie behind it
+    if constexpr (kTraceAnalysis) { // k[] (ring[0, 100)) is still intact: t[] and the predictor lie behind it
         selab200_analysis_trace &tr = trace[unit];
         for (int i = lane; i < kMaxOrder; i += 32) {
             tr.k[i] = scratch.kk()[i];
@@ -412,6 +445,8 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
     // ---- Rice: parameter search, then pack into this unit's slot ----
     const RiceChoice cq = warp_rice_choose(cf.q, order);
     const RiceChoice cr = warp_rice_choose(res, kFrame);
+    if constexpr (TRACE && MODE == kUnitSearch)
+        search_trace_record(strace, unit, order, cf, res, tie, cq, cr);
     if constexpr (MODE == kUnitCandidate) {
         __syncwarp();
         for (int l = lane; l < kFrame * 4 / 128; l += 32)

@@ -13,6 +13,8 @@
 //                              stereo decision), summed into one counter
 // Then k_encode_sizes / k_encode_scan / k_encode_gather(_container) run as for every encode, and the stereo decision
 // there sees the searched sizes.  The candidate and repack kernels have grids of a fixed size and loop over the work.
+// k_search_units_trace and k_search_candidates_trace (tests only, selab200_encode_search_trace) also write the record
+// of every (unit, order) to a trace buffer.
 #pragma once
 
 #include "kernels.cuh"
@@ -65,9 +67,10 @@ __device__ __forceinline__ void step_up(double *t, int i, int q)
 //   PACK = false  every order but the reference order (the analysis kernel has sized that one): FIR with the tie
 //                 check, Rice sizes, a tie-free order into su[unit].best
 //   PACK = true   (o_lo = o_hi) FIR, Rice, pack into the unit's slot and rewrite its record
-template <bool STEREO, bool PACK>
+// TRACE (PACK = false, tests only, selab200_encode_search_trace): each order's record into trace as well.
+template <bool STEREO, bool PACK, bool TRACE = false>
 __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
-                                              int o_hi, int32_t *res)
+                                              int o_hi, int32_t *res, selab200_search_trace *trace = nullptr)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
@@ -108,6 +111,8 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
         const RiceChoice cq = warp_rice_choose(cf.q, o);
         const RiceChoice cr = warp_rice_choose(res, kFrame);
         if constexpr (!PACK) {
+            if constexpr (TRACE)
+                search_trace_record(trace, unit, o, cf, res, tie, cq, cr);
             const unsigned long long words = cq.words + cr.words;
             if (lane == 0 && !tie)
                 atomicMin(&s.best, words << 8 | (unsigned long long)o);
@@ -142,22 +147,44 @@ __global__ void __launch_bounds__(32) k_search_units(EncodeParams p, const selab
     encode_unit<STEREO, false, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su);
 }
 
+// Tests only (selab200_encode_search_trace): k_search_units, and the reference order's record into trace.
+template <bool STEREO, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_search_units_trace(EncodeParams p, const selab200_predictor *pred,
+                                                           SearchUnit *su, selab200_search_trace *trace)
+{
+    encode_unit<STEREO, true, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su, trace);
+}
+
 // Work item w = (unit w / kSearchSlices, slice w % kSearchSlices): the slices of a unit go to neighbouring warps,
 // which read the same PCM.  Residue row = the warp's (the grid is at most the batch's units).
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_search_candidates(EncodeParams p, SearchUnit *su)
+template <bool STEREO, bool TRACE>
+__device__ __forceinline__ void search_candidates(const EncodeParams &p, SearchUnit *su, selab200_search_trace *trace)
 {
     const size_t work = (size_t)encode_units(p.n_frames, p.channels) * kSearchSlices;
     int32_t *res = p.residues + (size_t)blockIdx.x * kFrame;
     for (size_t w = blockIdx.x; w < work; w += gridDim.x) {
         const int sl = (int)(w % kSearchSlices);
         __syncwarp();
-        search_orders<STEREO, false>(p, su, (uint32_t)(w / kSearchSlices), search_slice_first(sl),
-                                     search_slice_first(sl + 1) - 1, res);
+        search_orders<STEREO, false, TRACE>(p, su, (uint32_t)(w / kSearchSlices), search_slice_first(sl),
+                                            search_slice_first(sl + 1) - 1, res, trace);
     }
     __syncwarp();
     for (int l = lane_id(); l < kFrame * 4 / 128; l += 32) // the row only ever lived in L2
         asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
+}
+
+template <bool STEREO>
+__global__ void __launch_bounds__(32) k_search_candidates(EncodeParams p, SearchUnit *su)
+{
+    search_candidates<STEREO, false>(p, su, nullptr);
+}
+
+// Tests only (selab200_encode_search_trace): k_search_candidates, and every order's record into trace.
+template <bool STEREO>
+__global__ void __launch_bounds__(32) k_search_candidates_trace(EncodeParams p, SearchUnit *su,
+                                                                selab200_search_trace *trace)
+{
+    search_candidates<STEREO, true>(p, su, trace);
 }
 
 template <bool STEREO>

@@ -3,9 +3,11 @@
 (DESIGN.md 7.3).
 
 The expected output comes from the CPU model in exact_search.py (the exact analysis model's quantiser, the port's
-predictors, the FIR with the tie test, Rice words, the winner rule and the stereo decision).  The model costs about
-30 ms per unit, so large batches are compared on chosen frames and checked as a whole through ref_words and decoding.
-Every decode check uses the device decoder, the port's, and the compiled reference's where it has been built."""
+predictors, the FIR with the tie test, Rice words, the winner rule and the stereo decision).  Its per-unit form costs
+about 30 ms per unit and is used on small batches; the corpus batches are compared whole with its batched form
+(about 15 ms per unit, pinned to the per-unit form in test_exact_search.py).  The 4 800-frame batch and the chunked
+host forms are compared on chosen frames and checked as a whole through ref_words and decoding.  Every decode check
+uses the device decoder, the port's, and the compiled reference's where it has been built."""
 import ctypes as C
 import pathlib
 import subprocess
@@ -28,24 +30,25 @@ BIN = ROOT / "sela_b200" / "host" / "bin"
 REF_CLI = ROOT / "oracle" / "_ref" / "sela_ref_cli"
 
 
-def _frames(pcm, ch, frames):
-    return np.asarray(pcm, np.int16).reshape(-1, FRAME * ch)[frames].reshape(-1)
-
-
 def _decoders():
     return [ol.load("port")] + ([ol.load("ref")] if ol.have_ref() else [])
 
 
-def _check(pcm, ch, frames=None, preds=None, got=None):
+def _check(pcm, ch, frames=None, preds=None, got=None, batched=False):
     """The search of batch `pcm` (host form, or `got` = (descs, words, ref_words)) against the model on `frames` (all
-    by default), ref_words against the default encoder's words, and the whole batch decoding back."""
+    by default; the batched model, which takes whole batches, with `batched`), ref_words against the default
+    encoder's words, and the whole batch decoding back."""
     import sela_b200
     O = ol.load("port")
     pcm = np.asarray(pcm, np.int16).reshape(-1)
     if got is None:
         got = codec.encode_search_forced(pcm, ch, preds) if preds is not None else sela_b200.encode_frames_search(pcm, ch)
     descs, words, ref_words = got
-    model, model_ref = xs.model_batch(O, pcm, ch, frames=frames, preds=preds)
+    if batched:
+        assert frames is None
+        model, model_ref = xs.model_batch_all(pcm, ch, preds)[:2]
+    else:
+        model, model_ref = xs.model_batch(O, pcm, ch, frames=frames, preds=preds)
     xs.check_frames(O, descs, words, pcm, ch, model)
     assert np.array_equal(gpu_calls.decode_frames_device(descs, words, ch), pcm)
     if preds is None:
@@ -93,11 +96,10 @@ def test_search_entry_points_have_no_cpu_fallback():
 @pytest.mark.gpu
 @pytest.mark.parametrize("batch", [b[0] for b in analysis_corpus.batches()])
 def test_corpus_batches(batch):
-    """A slice of every analysis-corpus batch (mono, stereo, 3 and 8 channels): at most 40 frames, spread over it."""
+    """Every analysis-corpus batch whole (mono, stereo, 3 and 8 channels, every 3rd BASELINE frame), against the
+    batched model."""
     _, pcm, ch = next(b for b in analysis_corpus.batches() if b[0] == batch)
-    n = pcm.size // (FRAME * ch)
-    frames = sorted(set(np.linspace(0, n - 1, min(n, 40)).astype(int).tolist()))
-    _check(_frames(pcm, ch, frames), ch)
+    _check(pcm, ch, batched=True)
 
 
 @pytest.mark.gpu
