@@ -347,6 +347,38 @@ int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames
                                          uint64_t *d_words_used, uint64_t *d_ref_words, int32_t *d_status,
                                          void *d_workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------- channel pairing -- */
+
+/* Smaller files of correlated channels at a higher encode cost (DESIGN.md 7.4).  The format can code any channel of
+ * a frame as `parent - difference` against any independently coded channel of the frame; the reference encoder only
+ * ever tries channel 1 against channel 0 of a stereo file.  The pairing forms start from the lossless encode, size
+ * the difference ch_p - ch_c of every ordered pair of channels of every frame, coded as the stereo difference is, and
+ * emit per frame the assignment (each channel alone, or against one independently coded parent) with the fewest words
+ * in total; between equal totals the fewest difference subframes, then the lexicographically smallest parent vector.
+ * A subframe whose FIR has a tie is never emitted, so every output decodes back to its source, under this decoder and
+ * under the unmodified reference decoder.  A frame in which no difference wins keeps the bytes of the lossless encode.
+ * channels == 1 is the lossless encode.  *base_words receives the words_used of selab200_encode_frames_lossless for
+ * the same frames (words_used <= base_words always), *n_difference the number of difference subframes emitted.
+ * Frames are split over devices as for the other batch calls. */
+int selab200_encode_frames_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                   selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                   size_t *words_used, size_t *base_words, size_t *n_difference);
+
+/* selab200_encode_container, with the pairing; *base_bytes receives the size of selab200_encode_container_lossless's
+ * output for the same frames. */
+int selab200_encode_container_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                      uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                      size_t capacity, size_t *bytes_used, size_t *base_bytes, size_t *n_difference);
+
+/* Device-resident form of selab200_encode_frames_pairing: arguments as selab200_encode_frames_device, with
+ * selab200_encode_pairing_workspace_bytes() of workspace; *d_base_words and *d_n_difference (uint64, device) receive
+ * the two totals.  Stream-ordered, no synchronisation. */
+size_t selab200_encode_pairing_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_encode_frames_pairing_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                          selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
+                                          uint64_t *d_words_used, uint64_t *d_base_words, uint64_t *d_n_difference,
+                                          int32_t *d_status, void *d_workspace, size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------ stage level (host buffers) -- */
 
 /* lpc::ResidueGenerator::process (src/lpc/residue_generator.cpp:121-134) for
@@ -492,6 +524,27 @@ int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t
                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                  size_t words_capacity, size_t *words_used, size_t *ref_words,
                                  selab200_search_unit *units, selab200_search_trace *trace);
+
+/* For tests: selab200_encode_frames_pairing on one device and one batch, except that every unit is coded with a given
+ * predictor, as selab200_encode_lossless_forced codes the base's.  pred holds the base's analysis units first, in
+ * selab200_encode_trace's order, then one record per candidate in (frame, p, c) order with the p = c entries skipped
+ * (n_frames * channels * (channels - 1) records; stereo (0, 1) is the base's difference unit and its record is not
+ * read).  A predictor outside the domain -> SELAB200_ERR_RANGE. */
+int selab200_encode_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                   size_t words_capacity, size_t *words_used, size_t *base_words,
+                                   size_t *n_difference);
+
+/* For tests: selab200_encode_frames_pairing on one device and one batch (selab200_encode_pairing_forced's when pred is
+ * not NULL), and what the pairing kernels saw.  trace[(frame * channels + p) * channels + c] receives the record of
+ * the candidate ch_p - ch_c as it was sized, in the layout of the order search's trace with the candidate's order in
+ * reserved[0]; every p != c is visited once, except stereo (0, 1), which is the base's unit and is not sized again
+ * (visits 0), and the p = c records stay zero.  par[frame * channels + c] receives the parent chosen for channel c
+ * (c itself: coded alone). */
+int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                  size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference,
+                                  uint8_t *par, selab200_search_trace *trace);
 
 #ifdef __cplusplus
 }

@@ -24,6 +24,9 @@ error behaviour as in include/sela_b200.h):
     encode_trace / quantise_probe   for tests: the batch encoder's analysis intermediates, its
     / fir_probe / fir_tie_probe     order threshold and quantiser on chosen values, its FIR residual
                                     (and tie test) on chosen signals and predictors, and the lossless
+    encode_frames_pairing / encode_container_pairing
+                                    the encoder with the channel pairing (DESIGN.md 7.4), and its tests-only
+                                    forms encode_pairing_forced / encode_pairing_trace
     encode_lossless_forced          encode with chosen predictors, and the order search with chosen
     / encode_search_forced          coefficients
 
@@ -459,3 +462,90 @@ def encode_search_trace(pcm, channels, predictors=None, device=0):
                                          descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
                                          C.addressof(ref), units.ctypes.data, trace.ctypes.data))
     return descs, words[:used.value].copy(), ref.value, units, trace
+
+
+def encode_frames_pairing(pcm, channels, words_capacity=None, device=0):
+    """encode_frames with the channel pairing (DESIGN.md 7.4) -> (descs, words, base_words, n_difference): base_words
+    is the number of words encode_frames_lossless writes for the same frames, n_difference the number of difference
+    subframes emitted."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_frames_pairing(pcm.ctypes.data, n_frames, channels, descs.ctypes.data, words.ctypes.data,
+                                           cap, C.addressof(used), C.addressof(base), C.addressof(nd)))
+    return descs, words[:used.value].copy(), base.value, nd.value
+
+
+def encode_container_pairing(pcm, channels, sample_rate, bits_per_sample=16, capacity=None, device=0):
+    """encode_container with the channel pairing -> (bytes, base_bytes, n_difference): base_bytes is the size of
+    encode_container_lossless's output for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_container_pairing(pcm.ctypes.data, n_frames, channels, sample_rate, bits_per_sample,
+                                              out.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                              C.addressof(nd)))
+    return out[:used.value], base.value, nd.value
+
+
+def _pairing_predictors(predictors, n_frames, channels):
+    n = n_frames * ((3 if channels == 2 else channels) + channels * (channels - 1))
+    if isinstance(predictors, np.ndarray) and predictors.dtype == PREDICTOR_DTYPE:
+        pred = _c(predictors, PREDICTOR_DTYPE)
+    else:
+        pred = np.zeros(len(predictors), PREDICTOR_DTYPE)
+        for rec, (order, q) in zip(pred, predictors):
+            rec["order"] = order
+            rec["q"][:order] = np.asarray(q)[:order]
+    if pred.size != n:
+        raise ValueError("%d predictors for %d units and candidates" % (pred.size, n))
+    return pred
+
+
+def encode_pairing_trace(pcm, channels, predictors=None, device=0):
+    """encode_frames_pairing on one batch, and what the pairing kernels saw -> (descs, words, base_words,
+    n_difference, par, trace).
+
+    predictors (None: analyse): PREDICTOR_DTYPE records or (order, q) pairs, the base's analysis units in
+    encode_trace's order, then one per candidate in (frame, p, c) order without p = c.  par: uint8 [n_frames,
+    channels], the parent chosen per channel.  trace: SEARCH_TRACE_DTYPE [n_frames, channels, channels], entry
+    [f, p, c] the candidate ch_p - ch_c as it was sized, its order in reserved[0]."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    pred = None if predictors is None else _pairing_predictors(predictors, n_frames, channels)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    par = np.zeros((n_frames, channels), np.uint8)
+    trace = np.zeros((n_frames, channels, channels), SEARCH_TRACE_DTYPE)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_pairing_trace(pcm.ctypes.data, n_frames, channels,
+                                          None if pred is None else pred.ctypes.data, descs.ctypes.data,
+                                          words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                          C.addressof(nd), par.ctypes.data, trace.ctypes.data))
+    return descs, words[:used.value].copy(), base.value, nd.value, par, trace
+
+
+def encode_pairing_forced(pcm, channels, predictors, device=0):
+    """encode_frames_pairing on one batch with every unit and candidate coded with its predictor from `predictors`
+    (as encode_pairing_trace takes them) -> (descs, words, base_words, n_difference)."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    pred = _pairing_predictors(predictors, n_frames, channels)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_pairing_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
+                                           words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                           C.addressof(nd)))
+    return descs, words[:used.value].copy(), base.value, nd.value

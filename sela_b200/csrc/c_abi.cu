@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "lossless.cuh"
+#include "pairing.cuh"
 #include "search.cuh"
 #include "verify.cuh"
 
@@ -319,16 +320,22 @@ int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis
 
 // The lossless repair between k_encode_units<S, false, true> and the scan (lossless.cuh).  Every launch has a grid
 // of a fixed size: nothing here depends on what the check found.  The warp kernels use at most one residue row
-// per unit of the batch.  FORCE: the units' predictors are d_pred's (selab200_encode_lossless_forced).
+// per unit of the batch.  FORCE: the units' predictors are d_pred's (selab200_encode_lossless_forced).  pairing: the
+// base of a pairing encode, which keeps the tie flags that the select kernel clears and takes no report.
 template <bool STEREO, bool FORCE = false>
 int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream,
-                  const selab200_predictor *d_pred = nullptr)
+                  const selab200_predictor *d_pred = nullptr, const PairingParams *pairing = nullptr)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>();
     if (int rc = set_smem(k_lossless_candidates<STEREO, FORCE>, smem))
         return rc;
     if (int rc = set_smem(k_lossless_repack<STEREO, FORCE>, smem))
         return rc;
+    if (pairing) {
+        k_pairing_capture<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, *pairing);
+        if (int rc = launch_check("k_pairing_capture"))
+            return rc;
+    }
     k_lossless_select<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, r);
     if (int rc = launch_check("k_lossless_select"))
         return rc;
@@ -341,6 +348,8 @@ int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames,
     k_lossless_repack<STEREO, FORCE><<<warps, 32, smem, stream>>>(p, r, d_pred);
     if (int rc = launch_check("k_lossless_repack"))
         return rc;
+    if (pairing)
+        return 0;
     k_lossless_report<<<(unsigned)std::min((n_frames + 255) / 256, (size_t)g.sms), 256, 0, stream>>>(p, r);
     return launch_check("k_lossless_report");
 }
@@ -387,12 +396,45 @@ int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t
     return launch_check("k_search_repack");
 }
 
+// The channel pairing (pairing.cuh) between the lossless repair and the scan: means, candidates, choice, and the
+// winning differences packed in place of their channels.  The warp kernels have grids of a fixed size, at most one
+// residue row per unit of the batch.
+int launch_pairing(const EncodeParams &p, const PairingParams &q, size_t n_frames, size_t n_units, cudaStream_t stream)
+{
+    constexpr size_t smem = encode_smem_bytes<true>();
+    if (int rc = set_smem(k_pairing_candidates, smem))
+        return rc;
+    if (int rc = set_smem(k_pairing_repack, smem))
+        return rc;
+    const size_t n_pairs = n_frames * p.channels * p.channels;
+    k_pairing_means<<<(unsigned)((n_pairs + 127) / 128), 128, 0, stream>>>(p, q);
+    if (int rc = launch_check("k_pairing_means"))
+        return rc;
+    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
+    k_pairing_candidates<<<warps, 32, smem, stream>>>(p, q);
+    if (int rc = launch_check("k_pairing_candidates"))
+        return rc;
+    k_pairing_select<<<(unsigned)std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream>>>(p, q);
+    if (int rc = launch_check("k_pairing_select"))
+        return rc;
+    k_pairing_repack<<<warps, 32, smem, stream>>>(p, q);
+    return launch_check("k_pairing_repack");
+}
+
 // Where a lossless encode reports its re-coded subframes: the batch's per-pair records, their count, and the frame
 // number of the batch's first frame.
 struct LosslessArgs {
     selab200_lossless_entry *entries;
     unsigned long long *n_entries;
     uint32_t frame_base;
+};
+
+// What a pairing encode adds to: the words of its base (the lossless encode) and the difference subframes it chose.
+// d_pred, d_trace (tests only): the candidates' predictors and their trace records (PairingParams).
+struct PairingArgs {
+    unsigned long long *d_base_words, *d_n_difference;
+    const selab200_predictor *d_pred = nullptr;
+    selab200_search_trace *d_trace = nullptr;
 };
 
 // ---- device-resident cores (no synchronisation) --------------------------
@@ -415,6 +457,8 @@ struct EncodeOptions {
                                                 // (selab200_encode_lossless_forced / selab200_encode_search_forced)
     selab200_search_trace *d_search_trace = nullptr; // search only: the tracing search kernels write every
                                                      // (unit, order) record here
+    const PairingArgs *pairing = nullptr;       // pair the channels (DESIGN.md 7.4) on top of the lossless encode;
+                                                // `lossless` is not read
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -423,7 +467,8 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
 {
     if (int rc = check_channels(channels))
         return rc;
-    if (ws_bytes < (o.lossless      ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
+    if (ws_bytes < (o.pairing       ? selab200_encode_pairing_workspace_bytes(n_frames, channels)
+                    : o.lossless    ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
                     : o.d_ref_words ? selab200_encode_search_workspace_bytes(n_frames, channels)
                                     : selab200_encode_workspace_bytes(n_frames, channels)))
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
@@ -454,32 +499,51 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
                         : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
         return rc;
-    if (o.lossless) {
+    PairingParams q{};
+    if (o.pairing) {
+        const size_t n_pairs = n_units ? (size_t)n_frames * channels * channels : 0;
+        char *b = static_cast<char *>(d_ws) + align256(selab200_encode_lossless_workspace_bytes(n_frames, channels));
+        q.table = reinterpret_cast<PairRecord *>(b);
+        q.means = reinterpret_cast<double *>(b + align256(n_pairs * sizeof(PairRecord)));
+        q.par = reinterpret_cast<uint8_t *>(q.means) + align256(n_pairs * sizeof(double));
+        q.stale = reinterpret_cast<uint32_t *>(q.par + align256((size_t)n_frames * channels));
+        q.base_words = o.pairing->d_base_words;
+        q.n_difference = o.pairing->d_n_difference;
+        q.pred = o.pairing->d_pred;
+        q.trace = o.pairing->d_trace;
+    }
+    const PairingParams *pq = o.pairing ? &q : nullptr;
+    if (o.lossless || o.pairing) {
+        static const LosslessArgs no_report{nullptr, nullptr, 0};
+        const LosslessArgs &la = o.pairing ? no_report : *o.lossless;
         RepairParams r;
         char *b = static_cast<char *>(d_ws) + align256(selab200_encode_workspace_bytes(n_frames, channels));
         r.count = reinterpret_cast<uint32_t *>(b);
         r.frames = reinterpret_cast<uint32_t *>(b + 256);
         r.orig = reinterpret_cast<UnitRecord *>(b + 256 + align256((size_t)n_frames * 4));
         r.units = reinterpret_cast<RepairUnit *>(reinterpret_cast<char *>(r.orig) + align256(n_units * sizeof(UnitRecord)));
-        r.entries = o.lossless->entries;
-        r.n_entries = o.lossless->n_entries;
-        r.frame_base = o.lossless->frame_base;
+        r.entries = la.entries;
+        r.n_entries = la.n_entries;
+        r.frame_base = la.frame_base;
         CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
         if (o.d_pred) {
             if (int rc = stereo ? launch_encode_units<true, false, true, true>(p, n_units, nullptr, stream, o.d_pred)
                                 : launch_encode_units<false, false, true, true>(p, n_units, nullptr, stream, o.d_pred))
                 return rc;
-            if (int rc = stereo ? launch_repair<true, true>(p, r, n_frames, n_units, stream, o.d_pred)
-                                : launch_repair<false, true>(p, r, n_frames, n_units, stream, o.d_pred))
+            if (int rc = stereo ? launch_repair<true, true>(p, r, n_frames, n_units, stream, o.d_pred, pq)
+                                : launch_repair<false, true>(p, r, n_frames, n_units, stream, o.d_pred, pq))
                 return rc;
         } else {
             if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
                                 : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
                 return rc;
-            if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream)
-                                : launch_repair<false>(p, r, n_frames, n_units, stream))
+            if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream, nullptr, pq)
+                                : launch_repair<false>(p, r, n_frames, n_units, stream, nullptr, pq))
                 return rc;
         }
+        if (o.pairing)
+            if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
+                return rc;
     } else if (o.d_ref_words) {
         SearchUnit *su = reinterpret_cast<SearchUnit *>(static_cast<char *>(d_ws) +
                                                         align256(selab200_encode_workspace_bytes(n_frames, channels)));
@@ -509,6 +573,11 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = launch_check("k_encode_scan"))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(d_used, p.residues, 8, cudaMemcpyDeviceToDevice, stream)); // the new fill level (see k_encode_scan)
+    if (o.pairing) {
+        k_pairing_patch<<<(unsigned)((n_sub + 255) / 256), 256, 0, stream>>>(p, q);
+        if (int rc = launch_check("k_pairing_patch"))
+            return rc;
+    }
     // The fill level this chunk leaves behind must be captured BEFORE the next chunk's scan (on the
     // other compute lane) may overwrite *d_used: copy it out now and only then release the event.
     if (o.h_fill_after)
@@ -971,6 +1040,11 @@ size_t selab200_encode_lossless_workspace_bytes(uint32_t n_frames, uint32_t chan
     return align256(selab200_encode_workspace_bytes(n_frames, channels)) + repair_lists_bytes(n_frames, channels);
 }
 
+size_t selab200_encode_pairing_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    return align256(selab200_encode_lossless_workspace_bytes(n_frames, channels)) + pairing_tables_bytes(n_frames, channels);
+}
+
 size_t selab200_encode_search_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     return align256(selab200_encode_workspace_bytes(n_frames, channels)) +
@@ -1043,6 +1117,28 @@ int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames
     CUDA_TRY(cudaMemsetAsync(d_ref_words, 0, sizeof(uint64_t), (cudaStream_t)stream));
     EncodeOptions o;
     o.d_ref_words = reinterpret_cast<unsigned long long *>(d_ref_words);
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
+}
+
+int selab200_encode_frames_pairing_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                          selab200_subframe_desc *d_descs, uint32_t *d_words, size_t words_capacity,
+                                          uint64_t *d_words_used, uint64_t *d_base_words, uint64_t *d_n_difference,
+                                          int32_t *d_status, void *d_workspace, size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_base_words || !d_n_difference || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(d_base_words, 0, sizeof(uint64_t), (cudaStream_t)stream));
+    CUDA_TRY(cudaMemsetAsync(d_n_difference, 0, sizeof(uint64_t), (cudaStream_t)stream));
+    const PairingArgs pa{reinterpret_cast<unsigned long long *>(d_base_words),
+                         reinterpret_cast<unsigned long long *>(d_n_difference)};
+    EncodeOptions o;
+    o.pairing = &pa;
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
@@ -1174,15 +1270,22 @@ struct EncodeTarget {
 // the differing (frame, channel) pairs.
 // `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs.
 // `ref_words`: search the order (DESIGN.md 7.3) and return the words the reference encoder's choice takes.
+// `pairing`: pair the channels (DESIGN.md 7.4) and return the words of the lossless encode and the differences chosen.
+struct PairingTotals {
+    unsigned long long base_words = 0, n_difference = 0;
+};
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
                        size_t *words_used, uint32_t frame_base, std::vector<selab200_verify_entry> *report,
-                       std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr)
+                       std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr,
+                       PairingTotals *pairing = nullptr)
 {
     const size_t words_capacity = t.words_capacity;
     const bool to_container = t.form == EncodeForm::container;
     *words_used = 0;
     if (ref_words)
         *ref_words = 0;
+    if (pairing)
+        *pairing = PairingTotals();
     if (report)
         report->clear();
     if (recoded)
@@ -1195,7 +1298,8 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
     const bool verify = report && to_container;
-    const size_t ws_bytes = recoded     ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
+    const size_t ws_bytes = pairing     ? selab200_encode_pairing_workspace_bytes(plan.max_frames, channels)
+                            : recoded   ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
                             : ref_words ? selab200_encode_search_workspace_bytes(plan.max_frames, channels)
                                         : selab200_encode_workspace_bytes(plan.max_frames, channels);
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
@@ -1219,6 +1323,9 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
     // search: the reference encoder's words, summed over the chunks
     unsigned long long *d_ref_words = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
+    // pairing: the base's words and the differences chosen, summed over the chunks
+    unsigned long long *d_pairing = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 64);
+    const PairingArgs pa{d_pairing, d_pairing + 1};
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
     uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
@@ -1229,6 +1336,8 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         if (int rc = verify_area(n_sub, arena_words, g.s_compute[0], va)) return rc;
 
     CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, ref_words ? 24 : 16, g.s_compute[0]));
+    if (pairing)
+        CUDA_TRY(cudaMemsetAsync(d_pairing, 0, 16, g.s_compute[0]));
     if (recoded)
         CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, 256 + n_sub * sizeof(selab200_lossless_entry), g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
@@ -1252,6 +1361,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         o.sub_base = (unsigned long long)f0 * channels;
         o.lossless = recoded ? &la : nullptr;
         o.d_ref_words = ref_words ? d_ref_words : nullptr;
+        o.pairing = pairing ? &pa : nullptr;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
                                    d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, o))
             return rc;
@@ -1309,12 +1419,18 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     for (int i = 0; i < (verify ? kLanes : kEncLanes); i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
     CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, ref_words ? 24 : 16, cudaMemcpyDeviceToHost, g.s_d2h));
+    if (pairing)
+        CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d_pairing, 16, cudaMemcpyDeviceToHost, g.s_d2h));
     CUDA_TRY(cudaStreamSynchronize(g.s_d2h));
     uint64_t used;
     memcpy(&used, g.h_small + 2, 8);
     *words_used = (size_t)used; // for CAPACITY: the size the caller needs
     if (ref_words)
         memcpy(ref_words, g.h_small + 4, 8);
+    if (pairing) {
+        memcpy(&pairing->base_words, g.h_small + 8, 8);
+        memcpy(&pairing->n_difference, g.h_small + 10, 8);
+    }
     if (g.h_small[0] != 0)
         return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
     if (recoded)
@@ -1527,6 +1643,7 @@ struct DevicePart {
     std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
     std::vector<selab200_lossless_entry> recoded; // lossless calls: this block's re-coded pairs, file-global frames
     unsigned long long ref_words = 0;             // search calls: the reference encoder's words of this block
+    unsigned long long base_words = 0, n_difference = 0; // pairing calls: this block's totals
 };
 
 static std::vector<DevicePart> device_parts(uint32_t n_frames)
@@ -1649,10 +1766,12 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
 }
 
 // Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.
-// `ref_words`: the order search, and the reference encoder's words of all blocks.
+// `ref_words`: the order search, and the reference encoder's words of all blocks.  `pairing`: the channel pairing, and
+// its totals over all blocks.
 static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
                          size_t *words_used, std::vector<selab200_verify_entry> *report,
-                         std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr)
+                         std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr,
+                         PairingTotals *pairing = nullptr)
 {
     const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
@@ -1661,8 +1780,13 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
         if (split) // the block stays on its device; its words are counted from its own start
             block = EncodeTarget{t.form, true, t.descs ? t.descs + (size_t)p.f0 * channels : nullptr, nullptr, nullptr,
                                  selab200_encode_words_bound(p.nf, channels)};
-        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, &p.used, p.f0, report ? &p.report : nullptr,
-                           recoded ? &p.recoded : nullptr, ref_words ? &p.ref_words : nullptr);
+        PairingTotals pt;
+        const int rc = encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, &p.used, p.f0,
+                                   report ? &p.report : nullptr, recoded ? &p.recoded : nullptr,
+                                   ref_words ? &p.ref_words : nullptr, pairing ? &pt : nullptr);
+        p.base_words = pt.base_words;
+        p.n_difference = pt.n_difference;
+        return rc;
     });
     if (report)
         *report = std::move(b.report);
@@ -1676,6 +1800,13 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
         *ref_words = 0;
         for (const DevicePart &p : b.parts)
             *ref_words += p.ref_words;
+    }
+    if (pairing) {
+        *pairing = PairingTotals();
+        for (const DevicePart &p : b.parts) {
+            pairing->base_words += p.base_words;
+            pairing->n_difference += p.n_difference;
+        }
     }
     if (b.rc || !split)
         return b.rc;
@@ -1737,6 +1868,25 @@ int selab200_encode_frames_search(const int16_t *pcm, uint32_t n_frames, uint32_
     return rc;
 }
 
+int selab200_encode_frames_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                   selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                   size_t *words_used, size_t *base_words, size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !base_words || !n_difference)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
+    PairingTotals pt;
+    const int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr, nullptr, &pt);
+    *base_words = (size_t)pt.base_words;
+    *n_difference = (size_t)pt.n_difference;
+    return rc;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -1745,11 +1895,13 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 } // extern "C"
 
 // selab200_encode_container, and with `report` its verified form, with `recoded` its lossless form, with `ref_bytes`
-// its order-search form (g_mutex held by the caller).
+// its order-search form, with `pairing` its channel-pairing form, where *ref_bytes is the size of the lossless
+// form's output (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
                                  std::vector<selab200_verify_entry> *report,
-                                 std::vector<selab200_lossless_entry> *recoded, size_t *ref_bytes = nullptr)
+                                 std::vector<selab200_lossless_entry> *recoded, size_t *ref_bytes = nullptr,
+                                 PairingTotals *pairing = nullptr)
 {
     if (int rc = require_ready())
         return rc;
@@ -1771,7 +1923,9 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4)};
     unsigned long long ref_words = 0;
     const int rc = encode_blocks(pcm, n_frames, channels, t, &words_used, report, recoded,
-                                 ref_bytes ? &ref_words : nullptr);
+                                 ref_bytes && !pairing ? &ref_words : nullptr, pairing);
+    if (pairing)
+        ref_words = pairing->base_words;
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
     if (ref_bytes)
         *ref_bytes = (size_t)container_frame_byte(n_frames, channels, ref_words);
@@ -1837,6 +1991,25 @@ int selab200_encode_container_search(const int16_t *pcm, uint32_t n_frames, uint
     *ref_bytes = 0;
     return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
                                  nullptr, nullptr, ref_bytes);
+}
+
+int selab200_encode_container_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
+                                      uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
+                                      size_t *base_bytes, size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!base_bytes || !n_difference) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    *base_bytes = 0;
+    *n_difference = 0;
+    PairingTotals pt;
+    const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                         bytes_used, nullptr, nullptr, base_bytes, &pt);
+    *n_difference = (size_t)pt.n_difference;
+    return rc;
 }
 
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames, uint32_t channels,
@@ -2385,6 +2558,112 @@ int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     return encode_search_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, ref_words,
                                units, trace);
+}
+
+// For tests: one unpipelined pairing batch through encode_device.  pred: the base's units' predictors, then the
+// candidates'.  par, table, trace (all or none): the choice, the candidate records and their trace records.
+static int encode_pairing_batch(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const selab200_predictor *pred,
+                                selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                size_t *words_used, size_t *base_words, size_t *n_difference, uint8_t *par,
+                                selab200_search_trace *trace)
+{
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !base_words || !n_difference)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    *words_used = *base_words = *n_difference = 0;
+    if (n_frames == 0)
+        return 0;
+    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
+    const size_t n_pairs = n_sub * channels, n_pred = n_units + n_sub * (channels - 1);
+    for (size_t u = 0; pred && u < n_pred; u++) {
+        const int o = pred[u].order;
+        if (o < 0 || o > kMaxOrder)
+            return fail(SELAB200_ERR_RANGE, "order %d of predictor %zu outside 0..%d", o, u, kMaxOrder);
+        for (int i = 0; i < kMaxOrder; i++)
+            if (i < o ? pred[u].q[i] < -64 || pred[u].q[i] > 63 : pred[u].q[i] != 0)
+                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of predictor %zu (order %d) outside [-64, 63], or not "
+                            "zero past the order", i, pred[u].q[i], u, o);
+    }
+    const size_t pred_bytes = pred ? align256(n_pred * sizeof(selab200_predictor)) : 0;
+    const size_t trace_bytes = trace ? n_pairs * sizeof(selab200_search_trace) : 0;
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
+    if (int rc = g.work.ensure(selab200_encode_pairing_workspace_bytes(n_frames, channels))) return rc;
+    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
+    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
+    unsigned long long *d_totals = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 64);
+    const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
+    selab200_search_trace *d_trace =
+        trace ? reinterpret_cast<selab200_search_trace *>(static_cast<char *>(g.aux.ptr) + pred_bytes) : nullptr;
+    CUDA_TRY(cudaMemsetAsync(d_totals, 0, 16, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    if (pred)
+        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_pred * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    if (trace)
+        CUDA_TRY(cudaMemsetAsync(d_trace, 0, trace_bytes, g.stream));
+    PairingArgs pa{d_totals, d_totals + 1};
+    pa.d_pred = pred ? d_pred + n_units : nullptr;
+    pa.d_trace = d_trace;
+    EncodeOptions o;
+    o.pairing = &pa;
+    o.d_pred = pred ? d_pred : nullptr;
+    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
+                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
+                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
+        return rc;
+    if (trace) { // par[] lies behind the candidate table and the means (encode_device)
+        const char *d_par = static_cast<const char *>(g.work.ptr) +
+                            align256(selab200_encode_lossless_workspace_bytes(n_frames, channels)) +
+                            align256(n_pairs * sizeof(PairRecord)) + align256(n_pairs * sizeof(double));
+        CUDA_TRY(cudaMemcpyAsync(par, d_par, n_sub, cudaMemcpyDeviceToHost, g.stream));
+        CUDA_TRY(cudaMemcpyAsync(trace, d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
+    }
+    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d_totals, 16, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    uint64_t used, base, n_diff;
+    memcpy(&used, g.h_small + 2, 8);
+    memcpy(&base, g.h_small + 8, 8);
+    memcpy(&n_diff, g.h_small + 10, 8);
+    *words_used = (size_t)used;
+    *base_words = (size_t)base;
+    *n_difference = (size_t)n_diff;
+    if (g.h_small[0] != 0)
+        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (used > words_capacity)
+        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    return 0;
+}
+
+int selab200_encode_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                   size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!pred)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    return encode_pairing_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, base_words,
+                                n_difference, nullptr, nullptr);
+}
+
+int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                                  size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference,
+                                  uint8_t *par, selab200_search_trace *trace)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!par || !trace)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    return encode_pairing_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, base_words,
+                                n_difference, par, trace);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

@@ -123,7 +123,7 @@ class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
     void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                  size_t *refBytes = nullptr);
+                  size_t *refBytes = nullptr, size_t *differences = nullptr);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -147,6 +147,11 @@ public:
     // decodes back to its source under the unmodified reference decoder.  Returns the bytes written; `refBytes`
     // receives the bytes processTo() writes for the same input.
     size_t processSearchTo(std::ofstream &outputFile, size_t &refBytes);
+    // Not in the reference: processLosslessTo() writing a smaller file of correlated channels: every channel of a
+    // frame coded alone or as its difference from another channel of the frame, whichever assignment takes the
+    // fewest words (selab200_encode_container_pairing).  Returns the bytes written; `losslessBytes` receives the
+    // bytes processLosslessTo() writes for the same input, `differences` the number of difference subframes.
+    size_t processPairingTo(std::ofstream &outputFile, size_t &losslessBytes, size_t &differences);
 };
 class Decoder {
     void readFrames();

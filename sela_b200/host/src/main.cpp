@@ -10,6 +10,10 @@
 // `-S in.wav out.sela`: a smaller file at a higher encode cost (every subframe at the predictor order with the fewest
 // words, and decoding back to the WAV under the reference decoder), one line with the bytes written and the bytes -e
 // writes.
+// `-P in.wav out.sela`: a smaller file of correlated channels at a higher encode cost (every channel of a frame coded
+// alone or as its difference from another, whichever takes the fewest words, for any channel count, and decoding back
+// to the WAV under the reference decoder), one line with the bytes written, the bytes -L writes and the number of
+// difference subframes.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -103,6 +107,8 @@ int usage(const std::string &prog)
               << " -L path/to/input.wav path/to/output.sela\n\n"
               << "Encoding a file smaller, searching every subframe's predictor order (H100 build):\n" << prog
               << " -S path/to/input.wav path/to/output.sela\n\n"
+              << "Encoding a file smaller, pairing the channels of every frame (H100 build):\n" << prog
+              << " -P path/to/input.wav path/to/output.sela\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -176,6 +182,14 @@ int main(int argc, char **argv)
             size_t refBytes = 0;
             const size_t written = sela::Encoder(in).processSearchTo(out, refBytes);
             std::cout << "Wrote " << written << " bytes (-e: " << refBytes << " bytes)" << std::endl;
+        } else if (mode == "-P" && argc == 4) {
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Encoding with the channel pairing: " << argv[2] << std::endl;
+            size_t losslessBytes = 0, differences = 0;
+            const size_t written = sela::Encoder(in).processPairingTo(out, losslessBytes, differences);
+            std::cout << "Wrote " << written << " bytes (-L: " << losslessBytes << " bytes), " << differences
+                      << " difference subframes" << std::endl;
         } else if (mode == "-t" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ifstream wav(argv[3], std::ios::binary);

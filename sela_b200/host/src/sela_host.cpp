@@ -803,11 +803,21 @@ size_t Encoder::processSearchTo(std::ofstream &outputFile, size_t &refBytes)
     return (size_t)(outputFile.tellp() - at);
 }
 
-// processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
-// selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search.
-void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                       size_t *refBytes)
+size_t Encoder::processPairingTo(std::ofstream &outputFile, size_t &losslessBytes, size_t &differences)
 {
+    const std::streampos at = outputFile.tellp();
+    encodeTo(outputFile, nullptr, nullptr, &losslessBytes, &differences);
+    return (size_t)(outputFile.tellp() - at);
+}
+
+// processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
+// selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search, with `differences`
+// as well through selab200_encode_container_pairing.
+void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
+                       size_t *refBytes, size_t *differences)
+{
+    if (differences)
+        *differences = 0;
     if (report)
         report->clear();
     if (recoded)
@@ -861,6 +871,11 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         for (size_t i = 0; i < n && i < raw.size(); i++)
             recoded->push_back(RecodedEntry{raw[i].frame, raw[i].channel, raw[i].ref_order, raw[i].order,
                                             raw[i].ref_words, raw[i].words});
+    } else if (differences) {
+        Phase p("pairing encode (device)");
+        check(selab200_encode_container_pairing(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                (uint32_t)n_frames, channels, w.fmt.sampleRate, w.fmt.bitsPerSample,
+                                                out, cap, &used, refBytes, differences));
     } else if (refBytes) {
         Phase p("order-search encode (device)");
         check(selab200_encode_container_search(reinterpret_cast<const int16_t *>(file.data + dat.body),
