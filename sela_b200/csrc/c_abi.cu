@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -69,6 +70,23 @@ struct DeviceBuffer {
     }
 };
 
+// The counters of the host-buffer, test and stage calls: at the front of g.small on the device, and in the pinned
+// g.h_small they come down to.  The encode counters (status .. n_difference) are reset and read back as one block.
+struct Counters {
+    int32_t status;                  // the device status of the call
+    uint64_t used;                   // encode: the word arena's fill level
+    unsigned long long ref_words;    // search: the words the reference encoder's choice takes
+    unsigned long long base_words;   // pairing: the words of its base, the lossless encode
+    unsigned long long n_difference; // pairing: the difference subframes chosen
+    uint32_t selftest;               // selab200_selftest: the mismatches
+    // host side only (collect_records): a count of set records, and the decode status that follows a verify count
+    unsigned long long n_records;
+    int32_t records_status;
+};
+constexpr size_t kEncodeCounterBytes = offsetof(Counters, selftest);
+static_assert(offsetof(Counters, records_status) == offsetof(Counters, n_records) + 8, "VerifyArea order");
+static_assert(sizeof(Counters) <= 256, "g.small holds the counters");
+
 constexpr int kMaxChunks = 72;
 constexpr int kLanes = 8; // concurrent compute streams of the pipelined host calls
 
@@ -81,10 +99,11 @@ struct Context {
     cudaStream_t s_compute[kLanes] = {};           // ... and compute lanes
     cudaEvent_t ev_h2d[kMaxChunks], ev_done[kMaxChunks], ev_scan[kMaxChunks], ev_reset;
     bool events = false;
-    DeviceBuffer in, descs, words, work, lane_work[kLanes], aux, small;
+    DeviceBuffer in, descs, words, work, lane_work[kLanes], aux;
+    DeviceBuffer small;                            // Counters
     DeviceBuffer verify;                           // verify paths: count, status, per-pair records (VerifyArea)
     DeviceBuffer lossless;                         // lossless host paths: count, per-pair records of re-coded subframes
-    int32_t *h_small = nullptr;                    // pinned: [0] status, [2..3] words_used, [12..14] verify count + status
+    Counters *h_small = nullptr;                   // pinned: where g.small's counters come down
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
     cudaStream_t last_rice_stream = nullptr;
@@ -102,6 +121,8 @@ int g_n_ctx = 0;
 Context *g_last_rice_ctx = nullptr; // the context selab200_rice_decode_frames_device last ran on (flag count query)
 thread_local Context *tl_ctx = &g_slots[0];
 #define g (*tl_ctx)
+
+Counters *device_counters() { return static_cast<Counters *>(g.small.ptr); }
 
 // What a container handle owns besides the walk result: the device image of the bytes, a pinned
 // descriptor table and the upload events.  Recycled through a small free list, because a process
@@ -318,14 +339,17 @@ int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis
     return launch_check("k_encode_units");
 }
 
-// The lossless repair between k_encode_units<S, false, true> and the scan (lossless.cuh).  Every launch has a grid
-// of a fixed size: nothing here depends on what the check found.  The warp kernels use at most one residue row
-// per unit of the batch.  FORCE: the units' predictors are d_pred's (selab200_encode_lossless_forced).  pairing: the
-// base of a pairing encode, which keeps the tie flags that the select kernel clears and takes no report.
+// The lossless encode (lossless.cuh) in place of k_encode_units: the analysis with the tie check,
+// k_encode_units<S, false, true>, then the repair.  Every repair launch has a grid of a fixed size: nothing here
+// depends on what the check found.  The warp kernels use at most one residue row per unit of the batch.  FORCE: the
+// units' predictors are d_pred's (selab200_encode_lossless_forced).  pairing: the base of a pairing encode, which
+// keeps the tie flags that the select kernel clears and takes no report.
 template <bool STEREO, bool FORCE = false>
-int launch_repair(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream,
-                  const selab200_predictor *d_pred = nullptr, const PairingParams *pairing = nullptr)
+int launch_lossless(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream,
+                    const selab200_predictor *d_pred, const PairingParams *pairing)
 {
+    if (int rc = launch_encode_units<STEREO, false, true, FORCE>(p, n_units, nullptr, stream, d_pred))
+        return rc;
     constexpr size_t smem = encode_smem_bytes<STEREO>();
     if (int rc = set_smem(k_lossless_candidates<STEREO, FORCE>, smem))
         return rc;
@@ -421,6 +445,58 @@ int launch_pairing(const EncodeParams &p, const PairingParams &q, size_t n_frame
     return launch_check("k_pairing_repack");
 }
 
+// Which encoder an encode call runs.  lossless: re-code every subframe the reference decoder would not reproduce
+// (DESIGN.md 7.2).  search: code every subframe at the predictor order with the fewest words (7.3).  pairing: code
+// channels as differences wherever that takes fewer words, on top of the lossless encode (7.4).
+enum class EncodeMode { plain, lossless, search, pairing };
+
+// Where every region of an encode workspace lies, as byte offsets from its base, and its size.  Every mode has the
+// plain encode's regions; lossless and pairing add the repair lists, search the SearchUnits, and pairing the pairing
+// tables behind the repair lists.  The offsets of the regions a mode lacks are 0.
+struct EncodeLayout {
+    size_t units, slots, means, residues;                       // EncodeParams
+    size_t repair_count, repair_frames, repair_orig, repair_units; // RepairParams
+    size_t search;                                              // SearchUnit[n_units]
+    size_t pair_table, pair_means, par, stale;                  // PairingParams
+    size_t bytes;                                               // selab200_encode_*_workspace_bytes
+};
+
+EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels)
+{
+    const size_t n_units = encode_units(n_frames, channels), n_sub = (size_t)n_frames * channels;
+    const size_t n_pairs = n_sub * channels;
+    EncodeLayout l{};
+    size_t at = 0;
+    auto region = [&at](size_t bytes) {
+        const size_t o = at;
+        at += align256(bytes);
+        return o;
+    };
+    l.units = region(n_units * sizeof(UnitRecord));
+    l.slots = region(n_units * (size_t)kSlotWords * 4);
+    l.means = region(n_units * sizeof(double));
+    l.residues = region(n_units * (size_t)kFrame * 4 + 256);
+    if (mode == EncodeMode::search) { // the last region, not padded
+        l.search = at;
+        l.bytes = at + n_units * sizeof(SearchUnit);
+        return l;
+    }
+    if (mode == EncodeMode::lossless || mode == EncodeMode::pairing) {
+        l.repair_count = region(256);
+        l.repair_frames = region((size_t)n_frames * 4);
+        l.repair_orig = region(n_units * sizeof(UnitRecord));
+        l.repair_units = region(n_units * sizeof(RepairUnit));
+    }
+    if (mode == EncodeMode::pairing) {
+        l.pair_table = region(n_pairs * sizeof(PairRecord));
+        l.pair_means = region(n_pairs * sizeof(double));
+        l.par = region(n_sub);
+        l.stale = region((size_t)n_frames * 4);
+    }
+    l.bytes = at;
+    return l;
+}
+
 // Where a lossless encode reports its re-coded subframes: the batch's per-pair records, their count, and the frame
 // number of the batch's first frame.
 struct LosslessArgs {
@@ -429,36 +505,31 @@ struct LosslessArgs {
     uint32_t frame_base;
 };
 
-// What a pairing encode adds to: the words of its base (the lossless encode) and the difference subframes it chose.
-// d_pred, d_trace (tests only): the candidates' predictors and their trace records (PairingParams).
-struct PairingArgs {
-    unsigned long long *d_base_words, *d_n_difference;
-    const selab200_predictor *d_pred = nullptr;
-    selab200_search_trace *d_trace = nullptr;
-};
-
 // ---- device-resident cores (no synchronisation) --------------------------
 
-// How encode_device chains into a pipelined call, and what it produces besides the word arena.  The defaults are
-// a stand-alone batch.
+// Which encoder encode_device runs, how it chains into a pipelined call, and what it produces besides the word arena.
+// The defaults are a stand-alone plain batch.  The fields from `lossless` on are read only by the modes they name.
 struct EncodeOptions {
-    bool fresh = true;                          // reset status and the arena fill level first; the pipelined host
-                                                // path resets once and then chains chunks through *d_used
+    EncodeMode mode = EncodeMode::plain;
+    bool fresh = true;                          // reset status, the arena fill level and the mode's counters and
+                                                // records first; the pipelined host path resets once and then
+                                                // chains chunks through *d_used
     cudaEvent_t before_scan = nullptr;          // the scan waits for it (the previous chunk's scan on another lane)
     cudaEvent_t after_scan = nullptr;           // recorded once this batch's fill level has been taken
     unsigned long long *h_fill_after = nullptr; // pinned: receives the fill level this batch leaves behind
     uint8_t *d_container = nullptr;             // gather into this byte-packed .sela image instead of the arena ...
     unsigned long long sub_base = 0;            // ... where the batch's first subframe is subframe sub_base
-    selab200_analysis_trace *d_trace = nullptr; // the tracing unit kernel writes every unit's analysis here
-    const LosslessArgs *lossless = nullptr;     // encode lossless (DESIGN.md 7.2) and report the re-coded pairs
-    unsigned long long *d_ref_words = nullptr;  // search the order (DESIGN.md 7.3) and add the reference encoder's
-                                                // words here
-    const selab200_predictor *d_pred = nullptr; // lossless or search only: every unit's predictor
-                                                // (selab200_encode_lossless_forced / selab200_encode_search_forced)
-    selab200_search_trace *d_search_trace = nullptr; // search only: the tracing search kernels write every
-                                                     // (unit, order) record here
-    const PairingArgs *pairing = nullptr;       // pair the channels (DESIGN.md 7.4) on top of the lossless encode;
-                                                // `lossless` is not read
+    LosslessArgs lossless{};                    // lossless: where the re-coded pairs are reported
+    unsigned long long *d_ref_words = nullptr;  // search: += the reference encoder's words
+    unsigned long long *d_base_words = nullptr; // pairing: += the words of its base, the lossless encode ...
+    unsigned long long *d_n_difference = nullptr; // ... and the difference subframes chosen
+    // tests only
+    selab200_analysis_trace *d_trace = nullptr;      // plain: the tracing unit kernel writes every unit's analysis here
+    const selab200_predictor *d_pred = nullptr;      // lossless, search, pairing: every unit's predictor (pairing: its
+                                                     // base's units)
+    const selab200_predictor *d_pair_pred = nullptr; // pairing: the candidates' predictors (PairingParams::pred)
+    selab200_search_trace *d_search_trace = nullptr; // search, pairing: the tracing kernels write every (unit, order) /
+                                                     // candidate record here
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -467,22 +538,33 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
 {
     if (int rc = check_channels(channels))
         return rc;
-    if (ws_bytes < (o.pairing       ? selab200_encode_pairing_workspace_bytes(n_frames, channels)
-                    : o.lossless    ? selab200_encode_lossless_workspace_bytes(n_frames, channels)
-                    : o.d_ref_words ? selab200_encode_search_workspace_bytes(n_frames, channels)
-                                    : selab200_encode_workspace_bytes(n_frames, channels)))
+    const EncodeLayout l = encode_layout(o.mode, n_frames, channels);
+    if (ws_bytes < l.bytes)
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
         return fail(SELAB200_ERR_ARGUMENT, "stereo PCM must be 16-byte aligned on the device");
+    const bool pairing = o.mode == EncodeMode::pairing;
+    const size_t n_sub = (size_t)n_frames * channels;
     if (o.fresh) {
         CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), stream));
         CUDA_TRY(cudaMemsetAsync(d_used, 0, sizeof(uint64_t), stream));
+        if (o.mode == EncodeMode::lossless) {
+            CUDA_TRY(cudaMemsetAsync(o.lossless.n_entries, 0, sizeof(unsigned long long), stream));
+            if (n_sub)
+                CUDA_TRY(cudaMemsetAsync(o.lossless.entries, 0, n_sub * sizeof(selab200_lossless_entry), stream));
+        }
+        if (o.mode == EncodeMode::search)
+            CUDA_TRY(cudaMemsetAsync(o.d_ref_words, 0, sizeof(unsigned long long), stream));
+        if (pairing) {
+            CUDA_TRY(cudaMemsetAsync(o.d_base_words, 0, sizeof(unsigned long long), stream));
+            CUDA_TRY(cudaMemsetAsync(o.d_n_difference, 0, sizeof(unsigned long long), stream));
+        }
     }
     if (n_frames == 0)
         return 0;
     const bool stereo = channels == 2;
     const size_t n_units = encode_units(n_frames, channels);
-    const size_t n_sub = (size_t)n_frames * channels;
+    char *ws = static_cast<char *>(d_ws);
     EncodeParams p;
     p.pcm = d_pcm;
     p.n_frames = n_frames;
@@ -492,61 +574,48 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     p.capacity = capacity;
     p.words_used = reinterpret_cast<unsigned long long *>(d_used);
     p.status = d_status;
-    p.units = static_cast<UnitRecord *>(d_ws);
-    p.slots = reinterpret_cast<uint32_t *>(static_cast<char *>(d_ws) + align256(n_units * sizeof(UnitRecord)));
-    p.means = reinterpret_cast<double *>(reinterpret_cast<char *>(p.slots) + align256(n_units * (size_t)kSlotWords * 4));
-    p.residues = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(p.means) + align256(n_units * sizeof(double)));
+    p.units = reinterpret_cast<UnitRecord *>(ws + l.units);
+    p.slots = reinterpret_cast<uint32_t *>(ws + l.slots);
+    p.means = reinterpret_cast<double *>(ws + l.means);
+    p.residues = reinterpret_cast<int32_t *>(ws + l.residues);
     if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
                         : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
         return rc;
     PairingParams q{};
-    if (o.pairing) {
-        const size_t n_pairs = n_units ? (size_t)n_frames * channels * channels : 0;
-        char *b = static_cast<char *>(d_ws) + align256(selab200_encode_lossless_workspace_bytes(n_frames, channels));
-        q.table = reinterpret_cast<PairRecord *>(b);
-        q.means = reinterpret_cast<double *>(b + align256(n_pairs * sizeof(PairRecord)));
-        q.par = reinterpret_cast<uint8_t *>(q.means) + align256(n_pairs * sizeof(double));
-        q.stale = reinterpret_cast<uint32_t *>(q.par + align256((size_t)n_frames * channels));
-        q.base_words = o.pairing->d_base_words;
-        q.n_difference = o.pairing->d_n_difference;
-        q.pred = o.pairing->d_pred;
-        q.trace = o.pairing->d_trace;
+    if (pairing) {
+        q.table = reinterpret_cast<PairRecord *>(ws + l.pair_table);
+        q.means = reinterpret_cast<double *>(ws + l.pair_means);
+        q.par = reinterpret_cast<uint8_t *>(ws + l.par);
+        q.stale = reinterpret_cast<uint32_t *>(ws + l.stale);
+        q.base_words = o.d_base_words;
+        q.n_difference = o.d_n_difference;
+        q.pred = o.d_pair_pred;
+        q.trace = o.d_search_trace;
     }
-    const PairingParams *pq = o.pairing ? &q : nullptr;
-    if (o.lossless || o.pairing) {
-        static const LosslessArgs no_report{nullptr, nullptr, 0};
-        const LosslessArgs &la = o.pairing ? no_report : *o.lossless;
+    const PairingParams *pq = pairing ? &q : nullptr;
+    if (o.mode == EncodeMode::lossless || pairing) {
+        const LosslessArgs la = pairing ? LosslessArgs{} : o.lossless; // the pairing's base takes no report
         RepairParams r;
-        char *b = static_cast<char *>(d_ws) + align256(selab200_encode_workspace_bytes(n_frames, channels));
-        r.count = reinterpret_cast<uint32_t *>(b);
-        r.frames = reinterpret_cast<uint32_t *>(b + 256);
-        r.orig = reinterpret_cast<UnitRecord *>(b + 256 + align256((size_t)n_frames * 4));
-        r.units = reinterpret_cast<RepairUnit *>(reinterpret_cast<char *>(r.orig) + align256(n_units * sizeof(UnitRecord)));
+        r.count = reinterpret_cast<uint32_t *>(ws + l.repair_count);
+        r.frames = reinterpret_cast<uint32_t *>(ws + l.repair_frames);
+        r.orig = reinterpret_cast<UnitRecord *>(ws + l.repair_orig);
+        r.units = reinterpret_cast<RepairUnit *>(ws + l.repair_units);
         r.entries = la.entries;
         r.n_entries = la.n_entries;
         r.frame_base = la.frame_base;
         CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
-        if (o.d_pred) {
-            if (int rc = stereo ? launch_encode_units<true, false, true, true>(p, n_units, nullptr, stream, o.d_pred)
-                                : launch_encode_units<false, false, true, true>(p, n_units, nullptr, stream, o.d_pred))
-                return rc;
-            if (int rc = stereo ? launch_repair<true, true>(p, r, n_frames, n_units, stream, o.d_pred, pq)
-                                : launch_repair<false, true>(p, r, n_frames, n_units, stream, o.d_pred, pq))
-                return rc;
-        } else {
-            if (int rc = stereo ? launch_encode_units<true, false, true>(p, n_units, nullptr, stream)
-                                : launch_encode_units<false, false, true>(p, n_units, nullptr, stream))
-                return rc;
-            if (int rc = stereo ? launch_repair<true>(p, r, n_frames, n_units, stream, nullptr, pq)
-                                : launch_repair<false>(p, r, n_frames, n_units, stream, nullptr, pq))
-                return rc;
-        }
-        if (o.pairing)
+        const selab200_predictor *pr = o.d_pred;
+        const int rc = pr ? (stereo ? launch_lossless<true, true>(p, r, n_frames, n_units, stream, pr, pq)
+                                    : launch_lossless<false, true>(p, r, n_frames, n_units, stream, pr, pq))
+                          : (stereo ? launch_lossless<true>(p, r, n_frames, n_units, stream, nullptr, pq)
+                                    : launch_lossless<false>(p, r, n_frames, n_units, stream, nullptr, pq));
+        if (rc)
+            return rc;
+        if (pairing)
             if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
                 return rc;
-    } else if (o.d_ref_words) {
-        SearchUnit *su = reinterpret_cast<SearchUnit *>(static_cast<char *>(d_ws) +
-                                                        align256(selab200_encode_workspace_bytes(n_frames, channels)));
+    } else if (o.mode == EncodeMode::search) {
+        SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
         unsigned long long *rw = o.d_ref_words;
         selab200_search_trace *tr = o.d_search_trace;
         const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr)
@@ -573,7 +642,7 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     if (int rc = launch_check("k_encode_scan"))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(d_used, p.residues, 8, cudaMemcpyDeviceToDevice, stream)); // the new fill level (see k_encode_scan)
-    if (o.pairing) {
+    if (pairing) {
         k_pairing_patch<<<(unsigned)((n_sub + 255) / 256), 256, 0, stream>>>(p, q);
         if (int rc = launch_check("k_pairing_patch"))
             return rc;
@@ -731,10 +800,10 @@ int decode_device(const selab200_subframe_desc *d_descs, uint32_t n_frames, uint
 
 int read_status(cudaStream_t stream, const int32_t *d_status)
 {
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(&g.h_small->status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
+    if (g.h_small->status != 0)
+        return fail(g.h_small->status, "%s", status_text(g.h_small->status));
     return 0;
 }
 
@@ -816,11 +885,10 @@ int collect_records(const unsigned long long *d_count, const int32_t *d_status, 
                     cudaStream_t stream, std::vector<T> &out)
 {
     out.clear();
-    CUDA_TRY(cudaMemcpyAsync(g.h_small + 12, d_count, d_status ? 16 : 8, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(&g.h_small->n_records, d_count, d_status ? 16 : 8, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
-    unsigned long long count;
-    memcpy(&count, g.h_small + 12, 8);
-    const int32_t st = d_status ? g.h_small[14] : 0;
+    const unsigned long long count = g.h_small->n_records;
+    const int32_t st = d_status ? g.h_small->records_status : 0;
     if (st != 0)
         return fail(st, "%s", status_text(st));
     if (count == 0)
@@ -874,7 +942,7 @@ static int init_slot(int device, int slot)
     }
     CUDA_TRY(cudaEventCreateWithFlags(&g.ev_reset, cudaEventDisableTiming));
     g.events = true;
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_small), 64));
+    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_small), sizeof(Counters)));
     CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_totals), (kMaxChunks + 1) * 8));
     if (int rc = g.small.ensure(256))
         return rc;
@@ -1030,25 +1098,22 @@ size_t selab200_encode_words_bound(uint32_t n_frames, uint32_t channels)
 
 size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
-    const size_t n_units = encode_units(n_frames, channels);
-    return align256(n_units * sizeof(UnitRecord)) + align256(n_units * (size_t)kSlotWords * 4) +
-           align256(n_units * sizeof(double)) + n_units * (size_t)kFrame * 4 + 256;
+    return encode_layout(EncodeMode::plain, n_frames, channels).bytes;
 }
 
 size_t selab200_encode_lossless_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
-    return align256(selab200_encode_workspace_bytes(n_frames, channels)) + repair_lists_bytes(n_frames, channels);
+    return encode_layout(EncodeMode::lossless, n_frames, channels).bytes;
 }
 
 size_t selab200_encode_pairing_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
-    return align256(selab200_encode_lossless_workspace_bytes(n_frames, channels)) + pairing_tables_bytes(n_frames, channels);
+    return encode_layout(EncodeMode::pairing, n_frames, channels).bytes;
 }
 
 size_t selab200_encode_search_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
-    return align256(selab200_encode_workspace_bytes(n_frames, channels)) +
-           encode_units(n_frames, channels) * sizeof(SearchUnit);
+    return encode_layout(EncodeMode::search, n_frames, channels).bytes;
 }
 
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
@@ -1089,17 +1154,11 @@ int selab200_encode_frames_lossless_device(const int16_t *d_pcm, uint32_t n_fram
         return rc;
     if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_entries || !d_n_entries || !d_status || !d_workspace)
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    const cudaStream_t st = (cudaStream_t)stream;
-    CUDA_TRY(cudaMemsetAsync(d_n_entries, 0, sizeof(uint64_t), st));
-    if (n_frames)
-        CUDA_TRY(cudaMemsetAsync(d_entries, 0, (size_t)n_frames * channels * sizeof(selab200_lossless_entry), st));
-    const LosslessArgs la{d_entries, reinterpret_cast<unsigned long long *>(d_n_entries), 0};
     EncodeOptions o;
-    o.lossless = &la;
+    o.mode = EncodeMode::lossless;
+    o.lossless = LosslessArgs{d_entries, reinterpret_cast<unsigned long long *>(d_n_entries), 0};
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
-                         d_workspace, workspace_bytes, st, o);
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
 
 int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
@@ -1112,10 +1171,8 @@ int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames
         return rc;
     if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_ref_words || !d_status || !d_workspace)
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    CUDA_TRY(cudaMemsetAsync(d_ref_words, 0, sizeof(uint64_t), (cudaStream_t)stream));
     EncodeOptions o;
+    o.mode = EncodeMode::search;
     o.d_ref_words = reinterpret_cast<unsigned long long *>(d_ref_words);
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream, o);
@@ -1131,14 +1188,10 @@ int selab200_encode_frames_pairing_device(const int16_t *d_pcm, uint32_t n_frame
         return rc;
     if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_base_words || !d_n_difference || !d_status || !d_workspace)
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    CUDA_TRY(cudaMemsetAsync(d_base_words, 0, sizeof(uint64_t), (cudaStream_t)stream));
-    CUDA_TRY(cudaMemsetAsync(d_n_difference, 0, sizeof(uint64_t), (cudaStream_t)stream));
-    const PairingArgs pa{reinterpret_cast<unsigned long long *>(d_base_words),
-                         reinterpret_cast<unsigned long long *>(d_n_difference)};
     EncodeOptions o;
-    o.pairing = &pa;
+    o.mode = EncodeMode::pairing;
+    o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
+    o.d_n_difference = reinterpret_cast<unsigned long long *>(d_n_difference);
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
@@ -1263,33 +1316,60 @@ struct EncodeTarget {
     uint32_t *words;               // arena: the Rice words (unused with `defer`)
     uint8_t *container;            // container: the whole .sela stream, header written by the caller (unused with `defer`)
     size_t words_capacity;         // Rice words the output holds
+    bool verify = false;           // container: also verify the image, chunk by chunk on the device (Result::report)
 };
 
-// The pipelined encoder over host buffers, frames numbered from frame_base in what it reports.
-// `report` (container form only): also verify the container image, chunk by chunk on the device, and return
-// the differing (frame, channel) pairs.
-// `recoded`: encode lossless (DESIGN.md 7.2) and return the re-coded (frame, channel) pairs.
-// `ref_words`: search the order (DESIGN.md 7.3) and return the words the reference encoder's choice takes.
-// `pairing`: pair the channels (DESIGN.md 7.4) and return the words of the lossless encode and the differences chosen.
-struct PairingTotals {
-    unsigned long long base_words = 0, n_difference = 0;
+// What a host-buffer call returns besides its output arrays: for one block of frames (DevicePart), or, summed with
+// add(), for the whole call.  The lists' frames are file-global.
+struct Result {
+    size_t words = 0;                  // encode: the words used (for CAPACITY: the size the caller needs)
+    unsigned long long ref_words = 0;  // search: the words the reference encoder's choice takes
+    unsigned long long base_words = 0; // pairing: the words of its base, the lossless encode
+    unsigned long long n_difference = 0; // pairing: the difference subframes chosen
+    size_t ref_bytes = 0;              // container search / pairing: the size of the output it is measured against
+    std::vector<selab200_lossless_entry> recoded; // lossless: the re-coded (frame, channel) pairs
+    std::vector<selab200_verify_entry> report;    // verify: the (frame, channel) pairs that do not decode back
+    void add(const Result &b)
+    {
+        words += b.words;
+        ref_words += b.ref_words;
+        base_words += b.base_words;
+        n_difference += b.n_difference;
+        recoded.insert(recoded.end(), b.recoded.begin(), b.recoded.end());
+        report.insert(report.end(), b.report.begin(), b.report.end());
+    }
 };
+
+// Once the encode on `stream` is done: its counters (g.small) into r, and its status.
+static int read_counters(cudaStream_t stream, Result &r)
+{
+    CUDA_TRY(cudaMemcpyAsync(g.h_small, device_counters(), kEncodeCounterBytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    const Counters &c = *g.h_small;
+    r.words = (size_t)c.used;
+    r.ref_words = c.ref_words;
+    r.base_words = c.base_words;
+    r.n_difference = c.n_difference;
+    return c.status ? fail(c.status, "%s", status_text(c.status)) : 0;
+}
+
+// g.lossless sized for n_sub pairs: the count of re-coded pairs, then their per-pair records.
+static int lossless_area(size_t n_sub, LosslessArgs &la)
+{
+    if (int rc = g.lossless.ensure(256 + n_sub * sizeof(selab200_lossless_entry)))
+        return rc;
+    la.n_entries = static_cast<unsigned long long *>(g.lossless.ptr);
+    la.entries = reinterpret_cast<selab200_lossless_entry *>(static_cast<char *>(g.lossless.ptr) + 256);
+    return 0;
+}
+
+// The pipelined encoder over host buffers, running `mode`, into r; frames numbered from frame_base in what it
+// reports.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                       size_t *words_used, uint32_t frame_base, std::vector<selab200_verify_entry> *report,
-                       std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr,
-                       PairingTotals *pairing = nullptr)
+                       EncodeMode mode, uint32_t frame_base, Result &r)
 {
     const size_t words_capacity = t.words_capacity;
     const bool to_container = t.form == EncodeForm::container;
-    *words_used = 0;
-    if (ref_words)
-        *ref_words = 0;
-    if (pairing)
-        *pairing = PairingTotals();
-    if (report)
-        report->clear();
-    if (recoded)
-        recoded->clear();
     if (n_frames == 0)
         return 0;
     PipelineDrain drain;
@@ -1297,20 +1377,15 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const uint32_t n_chunks = plan.chunks();
     const size_t n_sub = (size_t)n_frames * channels;
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
-    const bool verify = report && to_container;
-    const size_t ws_bytes = pairing     ? selab200_encode_pairing_workspace_bytes(plan.max_frames, channels)
-                            : recoded   ? selab200_encode_lossless_workspace_bytes(plan.max_frames, channels)
-                            : ref_words ? selab200_encode_search_workspace_bytes(plan.max_frames, channels)
-                                        : selab200_encode_workspace_bytes(plan.max_frames, channels);
+    const bool verify = t.verify && to_container;
+    const bool lossless = mode == EncodeMode::lossless;
+    const size_t ws_bytes = encode_layout(mode, plan.max_frames, channels).bytes;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(container_frame_byte(n_frames, channels, words_capacity) + 64)) return rc;
-    // lossless: the count of re-coded pairs, then the per-pair records of the whole batch
-    if (recoded)
-        if (int rc = g.lossless.ensure(256 + n_sub * sizeof(selab200_lossless_entry))) return rc;
-    unsigned long long *d_recoded = static_cast<unsigned long long *>(g.lossless.ptr);
-    selab200_lossless_entry *d_rec_entries =
-        recoded ? reinterpret_cast<selab200_lossless_entry *>(static_cast<char *>(g.lossless.ptr) + 256) : nullptr;
+    LosslessArgs records{}; // lossless: the re-coded pairs of the whole batch
+    if (lossless)
+        if (int rc = lossless_area(n_sub, records)) return rc;
     constexpr int kEncLanes = 2;
     for (int i = 0; i < kEncLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
@@ -1319,13 +1394,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     constexpr int kVerifyLanes = kLanes - kEncLanes;
     for (int i = 0; verify && i < kVerifyLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[kEncLanes + i].ensure(selab200_verify_workspace_bytes(plan.max_frames, channels))) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
-    // search: the reference encoder's words, summed over the chunks
-    unsigned long long *d_ref_words = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
-    // pairing: the base's words and the differences chosen, summed over the chunks
-    unsigned long long *d_pairing = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 64);
-    const PairingArgs pa{d_pairing, d_pairing + 1};
+    Counters *d_ctr = device_counters(); // the mode's counters are summed over the chunks
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
     uint32_t *d_words = static_cast<uint32_t *>(g.words.ptr);
@@ -1335,17 +1404,14 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     if (verify)
         if (int rc = verify_area(n_sub, arena_words, g.s_compute[0], va)) return rc;
 
-    CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, ref_words ? 24 : 16, g.s_compute[0]));
-    if (pairing)
-        CUDA_TRY(cudaMemsetAsync(d_pairing, 0, 16, g.s_compute[0]));
-    if (recoded)
+    CUDA_TRY(cudaMemsetAsync(d_ctr, 0, kEncodeCounterBytes, g.s_compute[0]));
+    if (lossless)
         CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, 256 + n_sub * sizeof(selab200_lossless_entry), g.s_compute[0]));
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
     for (int i = 1; i < kLanes; i++)
         CUDA_TRY(cudaStreamWaitEvent(g.s_compute[i], g.ev_reset, 0));
     for (uint32_t c = 0; c < n_chunks; c++) {
         const uint32_t f0 = plan.start[c], nf = plan.start[c + 1] - f0;
-        const LosslessArgs la{d_rec_entries + (size_t)f0 * channels, d_recoded, frame_base + f0};
         CUDA_TRY(cudaMemcpyAsync(d_pcm + (size_t)f0 * channels * kFrame, pcm + (size_t)f0 * channels * kFrame,
                                  nf * frame_bytes, cudaMemcpyHostToDevice, g.s_h2d));
         CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
@@ -1353,17 +1419,20 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         DeviceBuffer &ws = g.lane_work[c % kEncLanes];
         CUDA_TRY(cudaStreamWaitEvent(cs, g.ev_h2d[c], 0));
         EncodeOptions o;
+        o.mode = mode;
         o.fresh = false;
         o.before_scan = c ? g.ev_scan[c - 1] : nullptr;
         o.after_scan = g.ev_scan[c];
         o.h_fill_after = &g.h_totals[c + 1];
         o.d_container = to_container ? static_cast<uint8_t *>(g.words.ptr) : nullptr;
         o.sub_base = (unsigned long long)f0 * channels;
-        o.lossless = recoded ? &la : nullptr;
-        o.d_ref_words = ref_words ? d_ref_words : nullptr;
-        o.pairing = pairing ? &pa : nullptr;
+        if (lossless)
+            o.lossless = LosslessArgs{records.entries + (size_t)f0 * channels, records.n_entries, frame_base + f0};
+        o.d_ref_words = &d_ctr->ref_words;
+        o.d_base_words = &d_ctr->base_words;
+        o.d_n_difference = &d_ctr->n_difference;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
-                                   d_words, words_capacity, d_used, d_status, ws.ptr, ws.bytes, cs, o))
+                                   d_words, words_capacity, &d_ctr->used, &d_ctr->status, ws.ptr, ws.bytes, cs, o))
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
         if (verify) {
@@ -1376,7 +1445,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
             DeviceBuffer &vws = g.lane_work[kEncLanes + c % kVerifyLanes];
             CUDA_TRY(cudaStreamWaitEvent(vs, g.ev_done[c], 0));
             k_verify_guard_descs<<<(unsigned)((chunk_sub + 255) / 256), 256, 0, vs>>>(d_descs + (size_t)f0 * channels,
-                                                                                   (uint32_t)chunk_sub, d_status, vd);
+                                                                                   (uint32_t)chunk_sub, &d_ctr->status, vd);
             if (int rc = launch_check("k_verify_guard_descs"))
                 return rc;
             k_container_unpack<<<(unsigned)((chunk_sub + 7) / 8), 256, 0, vs>>>(static_cast<const uint8_t *>(g.words.ptr), vd,
@@ -1418,25 +1487,12 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     }
     for (int i = 0; i < (verify ? kLanes : kEncLanes); i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, ref_words ? 24 : 16, cudaMemcpyDeviceToHost, g.s_d2h));
-    if (pairing)
-        CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d_pairing, 16, cudaMemcpyDeviceToHost, g.s_d2h));
-    CUDA_TRY(cudaStreamSynchronize(g.s_d2h));
-    uint64_t used;
-    memcpy(&used, g.h_small + 2, 8);
-    *words_used = (size_t)used; // for CAPACITY: the size the caller needs
-    if (ref_words)
-        memcpy(ref_words, g.h_small + 4, 8);
-    if (pairing) {
-        memcpy(&pairing->base_words, g.h_small + 8, 8);
-        memcpy(&pairing->n_difference, g.h_small + 10, 8);
-    }
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (recoded)
-        if (int rc = collect_records(d_recoded, nullptr, d_rec_entries, n_sub, g.s_d2h, *recoded))
+    if (int rc = read_counters(g.s_d2h, r))
+        return rc;
+    if (lossless)
+        if (int rc = collect_records(records.n_entries, nullptr, records.entries, n_sub, g.s_d2h, r.recoded))
             return rc;
-    return verify ? collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, *report) : 0;
+    return verify ? collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, r.report) : 0;
 }
 
 // The words n descriptors reference, [lo, hi) (descriptors need not be in arena order); hi <= lo if none.
@@ -1583,14 +1639,14 @@ static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t cha
     for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
     if (int rc = in.start(F0, NF, channels)) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    int32_t *d_status = &device_counters()->status;
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
     VerifyArea va;
     if (report) {
         if (int rc = verify_area(n_sub, 0, g.s_compute[0], va)) return rc;
     } else {
-        CUDA_TRY(cudaMemsetAsync(g.small.ptr, 0, 16, g.s_compute[0]));
+        CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), g.s_compute[0]));
     }
     CUDA_TRY(cudaEventRecord(g.ev_reset, g.s_compute[0]));
     for (int i = 1; i < kLanes; i++)
@@ -1638,12 +1694,8 @@ static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t cha
 struct DevicePart {
     uint32_t f0 = 0, nf = 0;
     int rc = 0;
-    size_t used = 0;
     char err[sizeof g_error] = "";
-    std::vector<selab200_verify_entry> report; // verify calls: this block's differing pairs, file-global frames
-    std::vector<selab200_lossless_entry> recoded; // lossless calls: this block's re-coded pairs, file-global frames
-    unsigned long long ref_words = 0;             // search calls: the reference encoder's words of this block
-    unsigned long long base_words = 0, n_difference = 0; // pairing calls: this block's totals
+    Result res; // this block's
 };
 
 static std::vector<DevicePart> device_parts(uint32_t n_frames)
@@ -1688,13 +1740,12 @@ static int run_on_devices(std::vector<DevicePart> &parts, F work)
     return 0;
 }
 
-// What run_blocks did: its blocks, and the blocks' reports and re-coded lists one after the other.  Blocks are
-// contiguous and in frame order, so the joined lists are in order too.
+// What run_blocks did: its blocks, and their results summed, the lists one after the other.  Blocks are contiguous
+// and in frame order, so the joined lists are in order too.
 struct Blocks {
     int rc = 0;
     std::vector<DevicePart> parts;
-    std::vector<selab200_verify_entry> report;
-    std::vector<selab200_lossless_entry> recoded;
+    Result total;
 };
 
 // Runs work(block) over frames [0, n_frames) of a host-buffer call: as one block on the primary context, or, with
@@ -1711,10 +1762,8 @@ static Blocks run_blocks(uint32_t n_frames, F work)
         b.parts[0].nf = n_frames;
         b.rc = work(b.parts[0]);
     }
-    for (const DevicePart &p : b.parts) {
-        b.report.insert(b.report.end(), p.report.begin(), p.report.end());
-        b.recoded.insert(b.recoded.end(), p.recoded.begin(), p.recoded.end());
-    }
+    for (const DevicePart &p : b.parts)
+        b.total.add(p.res);
     return b;
 }
 
@@ -1731,15 +1780,15 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
         const DevicePart &p = parts[d];
         CUDA_TRY(cudaSetDevice(g.device));
         if (to_container) {
-            const size_t body = (size_t)container_frame_byte(p.nf, channels, p.used) - kContainerHeaderBytes;
+            const size_t body = (size_t)container_frame_byte(p.nf, channels, p.res.words) - kContainerHeaderBytes;
             const size_t at = (size_t)container_frame_byte(p.f0, channels, base);
             if (body)
                 CUDA_TRY(cudaMemcpyAsync(t.container + at, static_cast<uint8_t *>(g.words.ptr) + kContainerHeaderBytes, body,
                                          cudaMemcpyDeviceToHost, g.s_d2h));
-        } else if (p.used) {
-            CUDA_TRY(cudaMemcpyAsync(t.words + base, g.words.ptr, p.used * 4, cudaMemcpyDeviceToHost, g.s_d2h));
+        } else if (p.res.words) {
+            CUDA_TRY(cudaMemcpyAsync(t.words + base, g.words.ptr, p.res.words * 4, cudaMemcpyDeviceToHost, g.s_d2h));
         }
-        base += p.used;
+        base += p.res.words;
     }
     if (!to_container) { // meanwhile: descriptor offsets from block-local to file order
         size_t b = 0;
@@ -1749,7 +1798,7 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
                     t.descs[i].refl_offset += b;
                     t.descs[i].res_offset += b;
                 }
-            b += p.used;
+            b += p.res.words;
         }
     }
     int rc2 = 0;
@@ -1765,52 +1814,28 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
     return rc2;
 }
 
-// Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.
-// `ref_words`: the order search, and the reference encoder's words of all blocks.  `pairing`: the channel pairing, and
-// its totals over all blocks.
+// Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.  r: the
+// results of all blocks.
 static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                         size_t *words_used, std::vector<selab200_verify_entry> *report,
-                         std::vector<selab200_lossless_entry> *recoded, unsigned long long *ref_words = nullptr,
-                         PairingTotals *pairing = nullptr)
+                         EncodeMode mode, Result &r)
 {
     const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
     Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
         EncodeTarget block = t;
-        if (split) // the block stays on its device; its words are counted from its own start
-            block = EncodeTarget{t.form, true, t.descs ? t.descs + (size_t)p.f0 * channels : nullptr, nullptr, nullptr,
-                                 selab200_encode_words_bound(p.nf, channels)};
-        PairingTotals pt;
-        const int rc = encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, &p.used, p.f0,
-                                   report ? &p.report : nullptr, recoded ? &p.recoded : nullptr,
-                                   ref_words ? &p.ref_words : nullptr, pairing ? &pt : nullptr);
-        p.base_words = pt.base_words;
-        p.n_difference = pt.n_difference;
-        return rc;
-    });
-    if (report)
-        *report = std::move(b.report);
-    if (recoded)
-        *recoded = std::move(b.recoded);
-    size_t total = 0;
-    for (const DevicePart &p : b.parts)
-        total += p.used;
-    *words_used = total;
-    if (ref_words) {
-        *ref_words = 0;
-        for (const DevicePart &p : b.parts)
-            *ref_words += p.ref_words;
-    }
-    if (pairing) {
-        *pairing = PairingTotals();
-        for (const DevicePart &p : b.parts) {
-            pairing->base_words += p.base_words;
-            pairing->n_difference += p.n_difference;
+        if (split) { // the block stays on its device; its words are counted from its own start
+            block.defer = true;
+            block.descs = t.descs ? t.descs + (size_t)p.f0 * channels : nullptr;
+            block.words = nullptr;
+            block.container = nullptr;
+            block.words_capacity = selab200_encode_words_bound(p.nf, channels);
         }
-    }
+        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, mode, p.f0, p.res);
+    });
+    r = std::move(b.total);
     if (b.rc || !split)
         return b.rc;
-    return place_blocks(b.parts, channels, t, total);
+    return place_blocks(b.parts, channels, t, r.words);
 }
 
 extern "C" {
@@ -1826,8 +1851,11 @@ int selab200_encode_frames(const int16_t *pcm, uint32_t n_frames, uint32_t chann
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     if (int rc = check_channels(channels))
         return rc;
-    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
-    return encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr);
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::plain, r);
+    *words_used = r.words;
+    return rc;
 }
 
 int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
@@ -1843,11 +1871,11 @@ int selab200_encode_frames_lossless(const int16_t *pcm, uint32_t n_frames, uint3
     if (int rc = check_channels(channels))
         return rc;
     *n_entries = 0;
-    std::vector<selab200_lossless_entry> rec;
-    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
-    if (int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, &rec))
-        return rc;
-    return deliver_records(rec, entries, capacity, n_entries);
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::lossless, r);
+    *words_used = r.words;
+    return rc ? rc : deliver_records(r.recoded, entries, capacity, n_entries);
 }
 
 int selab200_encode_frames_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
@@ -1861,10 +1889,11 @@ int selab200_encode_frames_search(const int16_t *pcm, uint32_t n_frames, uint32_
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     if (int rc = check_channels(channels))
         return rc;
-    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
-    unsigned long long ref = 0;
-    const int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr, &ref);
-    *ref_words = (size_t)ref;
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::search, r);
+    *words_used = r.words;
+    *ref_words = (size_t)r.ref_words;
     return rc;
 }
 
@@ -1879,11 +1908,12 @@ int selab200_encode_frames_pairing(const int16_t *pcm, uint32_t n_frames, uint32
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     if (int rc = check_channels(channels))
         return rc;
-    const EncodeTarget t{EncodeForm::arena, false, descs, words, nullptr, words_capacity};
-    PairingTotals pt;
-    const int rc = encode_blocks(pcm, n_frames, channels, t, words_used, nullptr, nullptr, nullptr, &pt);
-    *base_words = (size_t)pt.base_words;
-    *n_difference = (size_t)pt.n_difference;
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::pairing, r);
+    *words_used = r.words;
+    *base_words = (size_t)r.base_words;
+    *n_difference = (size_t)r.n_difference;
     return rc;
 }
 
@@ -1894,14 +1924,10 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 
 } // extern "C"
 
-// selab200_encode_container, and with `report` its verified form, with `recoded` its lossless form, with `ref_bytes`
-// its order-search form, with `pairing` its channel-pairing form, where *ref_bytes is the size of the lossless
-// form's output (g_mutex held by the caller).
+// selab200_encode_container in every mode, and with `verify` its verified form (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
-                                 std::vector<selab200_verify_entry> *report,
-                                 std::vector<selab200_lossless_entry> *recoded, size_t *ref_bytes = nullptr,
-                                 PairingTotals *pairing = nullptr)
+                                 EncodeMode mode, bool verify, Result &r)
 {
     if (int rc = require_ready())
         return rc;
@@ -1919,16 +1945,12 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
                                 (uint8_t)bits_per_sample, (uint8_t)(bits_per_sample >> 8), (uint8_t)channels,
                                 (uint8_t)n_frames, (uint8_t)(n_frames >> 8), (uint8_t)(n_frames >> 16), (uint8_t)(n_frames >> 24)};
     memcpy(container, header, sizeof header);
-    size_t words_used = 0;
-    const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4)};
-    unsigned long long ref_words = 0;
-    const int rc = encode_blocks(pcm, n_frames, channels, t, &words_used, report, recoded,
-                                 ref_bytes && !pairing ? &ref_words : nullptr, pairing);
-    if (pairing)
-        ref_words = pairing->base_words;
-    *bytes_used = (size_t)container_frame_byte(n_frames, channels, words_used);
-    if (ref_bytes)
-        *ref_bytes = (size_t)container_frame_byte(n_frames, channels, ref_words);
+    const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4),
+                         verify};
+    const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r);
+    *bytes_used = (size_t)container_frame_byte(n_frames, channels, r.words);
+    r.ref_bytes = (size_t)container_frame_byte(n_frames, channels,
+                                               mode == EncodeMode::pairing ? r.base_words : r.ref_words);
     return rc;
 }
 
@@ -1938,8 +1960,9 @@ int selab200_encode_container(const int16_t *pcm, uint32_t n_frames, uint32_t ch
                               uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used)
 {
     std::lock_guard<std::mutex> lock(g_mutex);
+    Result r;
     return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
-                                 nullptr, nullptr);
+                                 EncodeMode::plain, false, r);
 }
 
 int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -1953,11 +1976,11 @@ int selab200_encode_container_verified(const int16_t *pcm, uint32_t n_frames, ui
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     }
     *n_entries = 0;
-    std::vector<selab200_verify_entry> report;
+    Result r;
     if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
-                                       bytes_used, &report, nullptr))
+                                       bytes_used, EncodeMode::plain, true, r))
         return rc;
-    return deliver_records(report, entries, entries_capacity, n_entries);
+    return deliver_records(r.report, entries, entries_capacity, n_entries);
 }
 
 int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -1971,11 +1994,11 @@ int selab200_encode_container_lossless(const int16_t *pcm, uint32_t n_frames, ui
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     }
     *n_entries = 0;
-    std::vector<selab200_lossless_entry> rec;
+    Result r;
     if (int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
-                                       bytes_used, nullptr, &rec))
+                                       bytes_used, EncodeMode::lossless, false, r))
         return rc;
-    return deliver_records(rec, entries, entries_capacity, n_entries);
+    return deliver_records(r.recoded, entries, entries_capacity, n_entries);
 }
 
 int selab200_encode_container_search(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -1988,9 +2011,11 @@ int selab200_encode_container_search(const int16_t *pcm, uint32_t n_frames, uint
             return rc;
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     }
-    *ref_bytes = 0;
-    return encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity, bytes_used,
-                                 nullptr, nullptr, ref_bytes);
+    Result r;
+    const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                         bytes_used, EncodeMode::search, false, r);
+    *ref_bytes = r.ref_bytes;
+    return rc;
 }
 
 int selab200_encode_container_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
@@ -2003,12 +2028,11 @@ int selab200_encode_container_pairing(const int16_t *pcm, uint32_t n_frames, uin
             return rc;
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     }
-    *base_bytes = 0;
-    *n_difference = 0;
-    PairingTotals pt;
+    Result r;
     const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
-                                         bytes_used, nullptr, nullptr, base_bytes, &pt);
-    *n_difference = (size_t)pt.n_difference;
+                                         bytes_used, EncodeMode::pairing, false, r);
+    *base_bytes = r.ref_bytes;
+    *n_difference = (size_t)r.n_difference;
     return rc;
 }
 
@@ -2042,11 +2066,11 @@ int selab200_verify_frames(const selab200_subframe_desc *descs, uint32_t n_frame
     *n_entries = 0;
     const CodedInput in{descs, words, n_words, nullptr};
     const Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
-        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.report);
+        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.res.report);
     });
     if (b.rc)
         return b.rc;
-    return deliver_records(b.report, entries, capacity, n_entries);
+    return deliver_records(b.total.report, entries, capacity, n_entries);
 }
 
 // ---- .sela container, decode side ----------------------------------------------------------
@@ -2291,11 +2315,11 @@ int selab200_container_verify(selab200_container *h, const int16_t *pcm, selab20
         return rc;
     const CodedInput in{h->buf.h_descs, nullptr, (size_t)h->info.n_words, h};
     const Blocks b = run_blocks(n_frames, [&](DevicePart &p) {
-        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.report);
+        return decode_pipeline(in, p.f0, p.nf, channels, nullptr, pcm, &p.res.report);
     });
     if (b.rc)
         return b.rc;
-    return deliver_records(b.report, entries, capacity, n_entries);
+    return deliver_records(b.total.report, entries, capacity, n_entries);
 }
 
 int selab200_selftest(uint32_t *mismatches)
@@ -2305,62 +2329,14 @@ int selab200_selftest(uint32_t *mismatches)
         return rc;
     if (!mismatches)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    uint32_t *d = reinterpret_cast<uint32_t *>(static_cast<char *>(g.small.ptr) + 32);
-    CUDA_TRY(cudaMemsetAsync(d, 0, 4, g.stream));
+    uint32_t *d = &device_counters()->selftest;
+    CUDA_TRY(cudaMemsetAsync(d, 0, sizeof *d, g.stream));
     k_selftest_scaling<<<(131071 + 255) / 256, 256, 0, g.stream>>>(d);
     if (int rc = launch_check("k_selftest_scaling"))
         return rc;
-    CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d, 4, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(&g.h_small->selftest, d, sizeof *d, cudaMemcpyDeviceToHost, g.stream));
     CUDA_TRY(cudaStreamSynchronize(g.stream));
-    *mismatches = (uint32_t)g.h_small[8];
-    return 0;
-}
-
-// For tests: one unpipelined batch through encode_device with the tracing unit kernel (include/sela_b200.h).
-int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
-                          uint32_t *words, size_t words_capacity, size_t *words_used, selab200_analysis_trace *trace)
-{
-    std::lock_guard<std::mutex> lock(g_mutex);
-    if (int rc = require_ready())
-        return rc;
-    if (!pcm || !descs || !words || !words_used || !trace)
-        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    *words_used = 0;
-    if (n_frames == 0)
-        return 0;
-    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    const size_t ws_bytes = selab200_encode_workspace_bytes(n_frames, channels);
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
-    if (int rc = g.work.ensure(ws_bytes)) return rc;
-    if (int rc = g.aux.ensure(n_units * sizeof(selab200_analysis_trace))) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
-    selab200_analysis_trace *d_trace = static_cast<selab200_analysis_trace *>(g.aux.ptr);
-    CUDA_TRY(cudaMemsetAsync(d_trace, 0, n_units * sizeof(selab200_analysis_trace), g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
-    EncodeOptions o;
-    o.d_trace = d_trace;
-    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
-                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
-                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
-        return rc;
-    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(trace, d_trace, n_units * sizeof(selab200_analysis_trace), cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    uint64_t used;
-    memcpy(&used, g.h_small + 2, 8);
-    *words_used = (size_t)used;
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (used > words_capacity)
-        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
-    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    *mismatches = g.h_small->selftest;
     return 0;
 }
 
@@ -2387,6 +2363,150 @@ int selab200_quantise_probe(const double *k, size_t n, int32_t *out)
     return 0;
 }
 
+static_assert(sizeof(selab200_search_trace) == 32, "selab200_search_trace layout (include/sela_b200.h)");
+static_assert(sizeof(selab200_search_unit) == sizeof(SearchUnit) &&
+                  offsetof(selab200_search_unit, ref_order) == offsetof(SearchUnit, ref_order) &&
+                  offsetof(selab200_search_unit, best) == offsetof(SearchUnit, best),
+              "selab200_search_unit mirrors SearchUnit");
+
+// What a test hook returns besides descriptors and words (encode_batch): host pointers, null where the hook has none.
+struct BatchOutputs {
+    size_t *words_used = nullptr;
+    size_t *ref_words = nullptr;                           // search
+    size_t *base_words = nullptr, *n_difference = nullptr; // pairing
+    selab200_lossless_entry *entries = nullptr;            // lossless: the re-coded pairs
+    size_t entries_capacity = 0, *n_entries = nullptr;
+    selab200_analysis_trace *analysis = nullptr;           // plain: the tracing unit kernel's records
+    selab200_search_trace *trace = nullptr;                // search, pairing: the tracing kernels' records ...
+    selab200_search_unit *units = nullptr;                 // ... and the search records
+    uint8_t *par = nullptr;                                // ... and the pairing's choice
+};
+
+// A test hook's predictors: every order in min_order..kMaxOrder, every q in [-64, 63], and with zero_past, every q
+// past the order zero.  noun: what a predictor is called in the messages.
+static int check_predictors(const selab200_predictor *pred, size_t n, int min_order, bool zero_past, const char *noun)
+{
+    for (size_t u = 0; u < n; u++) {
+        const int o = pred[u].order;
+        if (o < min_order || o > kMaxOrder)
+            return fail(SELAB200_ERR_RANGE, "order %d of %s %zu outside %d..%d", o, noun, u, min_order, kMaxOrder);
+        for (int i = 0; i < kMaxOrder; i++) {
+            const int q = pred[u].q[i];
+            if (zero_past && (i < o ? q < -64 || q > 63 : q != 0))
+                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of %s %zu (order %d) outside [-64, 63], or not zero "
+                            "past the order", i, q, noun, u, o);
+            if (!zero_past && (q < -64 || q > 63))
+                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of %s %zu outside [-64, 63]", i, q, noun, u);
+        }
+    }
+    return 0;
+}
+
+// For tests: one unpipelined batch of `mode` through encode_device on g.stream.  pred (lossless: required): every
+// unit's predictor, for the pairing followed by the candidates' (include/sela_b200.h).
+static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                        const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
+                        size_t words_capacity, const BatchOutputs &out)
+{
+    if (int rc = require_ready())
+        return rc;
+    const bool lossless = mode == EncodeMode::lossless, search = mode == EncodeMode::search,
+               pairing = mode == EncodeMode::pairing;
+    if (!pcm || !descs || !words || !out.words_used || (mode == EncodeMode::plain && !out.analysis) ||
+        (lossless && (!pred || (!out.entries && out.entries_capacity) || !out.n_entries)) ||
+        (search && !out.ref_words) || (pairing && (!out.base_words || !out.n_difference)))
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    *out.words_used = 0;
+    if (lossless)
+        *out.n_entries = 0;
+    if (search)
+        *out.ref_words = 0;
+    if (pairing)
+        *out.base_words = *out.n_difference = 0;
+    if (n_frames == 0)
+        return 0;
+    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
+    const size_t n_pred = pairing ? n_units + n_sub * (channels - 1) : n_units;
+    if (pred)
+        if (int rc = check_predictors(pred, n_pred, search ? 1 : 0, !search, pairing ? "predictor" : "unit"))
+            return rc;
+    const EncodeLayout l = encode_layout(mode, n_frames, channels);
+    const size_t pred_bytes = pred ? align256(n_pred * sizeof(selab200_predictor)) : 0;
+    const size_t trace_bytes = out.analysis ? n_units * sizeof(selab200_analysis_trace)
+                               : out.trace  ? (pairing ? n_sub * channels : n_units * kMaxOrder) * sizeof(selab200_search_trace)
+                                            : 0;
+    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
+    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
+    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
+    if (int rc = g.work.ensure(l.bytes)) return rc;
+    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
+    Counters *d_ctr = device_counters();
+    const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
+    void *d_trace = static_cast<char *>(g.aux.ptr) + pred_bytes;
+    EncodeOptions o; // fresh: encode_device resets the counters and records
+    o.mode = mode;
+    if (lossless)
+        if (int rc = lossless_area(n_sub, o.lossless)) return rc;
+    o.d_ref_words = &d_ctr->ref_words;
+    o.d_base_words = &d_ctr->base_words;
+    o.d_n_difference = &d_ctr->n_difference;
+    o.d_pred = pred ? d_pred : nullptr;
+    o.d_pair_pred = pred && pairing ? d_pred + n_units : nullptr;
+    o.d_trace = out.analysis ? static_cast<selab200_analysis_trace *>(d_trace) : nullptr;
+    o.d_search_trace = out.trace ? static_cast<selab200_search_trace *>(d_trace) : nullptr;
+    if (trace_bytes)
+        CUDA_TRY(cudaMemsetAsync(d_trace, 0, trace_bytes, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
+    if (pred)
+        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_pred * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
+                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
+                               words_capacity, &d_ctr->used, &d_ctr->status, g.work.ptr, g.work.bytes, g.stream, o))
+        return rc;
+    const char *ws = static_cast<const char *>(g.work.ptr);
+    if (out.units)
+        CUDA_TRY(cudaMemcpyAsync(out.units, ws + l.search, n_units * sizeof(SearchUnit), cudaMemcpyDeviceToHost, g.stream));
+    if (out.par)
+        CUDA_TRY(cudaMemcpyAsync(out.par, ws + l.par, n_sub, cudaMemcpyDeviceToHost, g.stream));
+    if (trace_bytes)
+        CUDA_TRY(cudaMemcpyAsync(out.analysis ? static_cast<void *>(out.analysis) : static_cast<void *>(out.trace),
+                                 d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
+    Result r;
+    const int status = read_counters(g.stream, r);
+    *out.words_used = r.words;
+    if (search)
+        *out.ref_words = (size_t)r.ref_words;
+    if (pairing) {
+        *out.base_words = (size_t)r.base_words;
+        *out.n_difference = (size_t)r.n_difference;
+    }
+    if (status)
+        return status;
+    if (r.words > words_capacity)
+        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
+    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, r.words * 4, cudaMemcpyDeviceToHost, g.stream));
+    CUDA_TRY(cudaStreamSynchronize(g.stream));
+    if (!lossless)
+        return 0;
+    if (int rc = collect_records(o.lossless.n_entries, nullptr, o.lossless.entries, n_sub, g.stream, r.recoded))
+        return rc;
+    return deliver_records(r.recoded, out.entries, out.entries_capacity, out.n_entries);
+}
+
+// For tests: one unpipelined batch through encode_device with the tracing unit kernel (include/sela_b200.h).
+int selab200_encode_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *descs,
+                          uint32_t *words, size_t words_capacity, size_t *words_used, selab200_analysis_trace *trace)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.analysis = trace;
+    return encode_batch(EncodeMode::plain, pcm, n_frames, channels, nullptr, descs, words, words_capacity, out);
+}
+
 // For tests: one unpipelined lossless batch through encode_device, every unit coded with its predictor from pred.
 int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                     const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
@@ -2394,149 +2514,16 @@ int selab200_encode_lossless_forced(const int16_t *pcm, uint32_t n_frames, uint3
                                     size_t entries_capacity, size_t *n_entries)
 {
     std::lock_guard<std::mutex> lock(g_mutex);
-    if (int rc = require_ready())
-        return rc;
-    if (!pcm || !pred || !descs || !words || !words_used || (!entries && entries_capacity) || !n_entries)
-        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    *words_used = 0;
-    *n_entries = 0;
-    if (n_frames == 0)
-        return 0;
-    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    for (size_t u = 0; u < n_units; u++) {
-        const int o = pred[u].order;
-        if (o < 0 || o > kMaxOrder)
-            return fail(SELAB200_ERR_RANGE, "order %d of unit %zu outside 0..%d", o, u, kMaxOrder);
-        for (int i = 0; i < kMaxOrder; i++)
-            if (i < o ? pred[u].q[i] < -64 || pred[u].q[i] > 63 : pred[u].q[i] != 0)
-                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of unit %zu (order %d) outside [-64, 63], or not zero "
-                            "past the order", i, pred[u].q[i], u, o);
-    }
-    const size_t ws_bytes = selab200_encode_lossless_workspace_bytes(n_frames, channels);
-    const size_t rec_bytes = 256 + n_sub * sizeof(selab200_lossless_entry);
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
-    if (int rc = g.work.ensure(ws_bytes)) return rc;
-    if (int rc = g.aux.ensure(n_units * sizeof(selab200_predictor))) return rc;
-    if (int rc = g.lossless.ensure(rec_bytes)) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
-    const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
-    unsigned long long *d_count = static_cast<unsigned long long *>(g.lossless.ptr);
-    selab200_lossless_entry *d_entries =
-        reinterpret_cast<selab200_lossless_entry *>(static_cast<char *>(g.lossless.ptr) + 256);
-    CUDA_TRY(cudaMemsetAsync(g.lossless.ptr, 0, rec_bytes, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
-    const LosslessArgs la{d_entries, d_count, 0};
-    EncodeOptions o;
-    o.lossless = &la;
-    o.d_pred = d_pred;
-    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
-                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
-                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
-        return rc;
-    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    uint64_t used;
-    memcpy(&used, g.h_small + 2, 8);
-    *words_used = (size_t)used;
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (used > words_capacity)
-        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
-    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
-    std::vector<selab200_lossless_entry> rec;
-    if (int rc = collect_records(d_count, nullptr, d_entries, n_sub, g.stream, rec))
-        return rc;
-    return deliver_records(rec, entries, entries_capacity, n_entries);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.entries = entries;
+    out.entries_capacity = entries_capacity;
+    out.n_entries = n_entries;
+    return encode_batch(EncodeMode::lossless, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
-static_assert(sizeof(selab200_search_trace) == 32, "selab200_search_trace layout (include/sela_b200.h)");
-static_assert(sizeof(selab200_search_unit) == sizeof(SearchUnit) &&
-                  offsetof(selab200_search_unit, ref_order) == offsetof(SearchUnit, ref_order) &&
-                  offsetof(selab200_search_unit, best) == offsetof(SearchUnit, best),
-              "selab200_search_unit mirrors SearchUnit");
-
-// For tests: one unpipelined order-search batch through encode_device.  pred (required when `forced`): every unit's
-// q[0..99] and reference order.  units, trace (both or neither): the search records and the tracing kernels' records.
-static int encode_search_batch(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const selab200_predictor *pred,
-                               selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
-                               size_t *words_used, size_t *ref_words, selab200_search_unit *units,
-                               selab200_search_trace *trace)
-{
-    if (int rc = require_ready())
-        return rc;
-    if (!pcm || !descs || !words || !words_used || !ref_words)
-        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    *words_used = 0;
-    *ref_words = 0;
-    if (n_frames == 0)
-        return 0;
-    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    for (size_t u = 0; pred && u < n_units; u++) {
-        const int o = pred[u].order;
-        if (o < 1 || o > kMaxOrder)
-            return fail(SELAB200_ERR_RANGE, "order %d of unit %zu outside 1..%d", o, u, kMaxOrder);
-        for (int i = 0; i < kMaxOrder; i++)
-            if (pred[u].q[i] < -64 || pred[u].q[i] > 63)
-                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of unit %zu outside [-64, 63]", i, pred[u].q[i], u);
-    }
-    const size_t ws_bytes = selab200_encode_search_workspace_bytes(n_frames, channels);
-    const size_t pred_bytes = pred ? align256(n_units * sizeof(selab200_predictor)) : 0;
-    const size_t trace_bytes = trace ? n_units * kMaxOrder * sizeof(selab200_search_trace) : 0;
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
-    if (int rc = g.work.ensure(ws_bytes)) return rc;
-    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
-    unsigned long long *d_ref = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 16);
-    selab200_search_trace *d_trace =
-        trace ? reinterpret_cast<selab200_search_trace *>(static_cast<char *>(g.aux.ptr) + pred_bytes) : nullptr;
-    CUDA_TRY(cudaMemsetAsync(d_ref, 0, 8, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
-    if (pred)
-        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_units * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
-    if (trace)
-        CUDA_TRY(cudaMemsetAsync(d_trace, 0, trace_bytes, g.stream));
-    EncodeOptions o;
-    o.d_ref_words = d_ref;
-    o.d_pred = pred ? static_cast<const selab200_predictor *>(g.aux.ptr) : nullptr;
-    o.d_search_trace = d_trace;
-    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
-                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
-                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
-        return rc;
-    if (trace) { // the search records lie behind the encode workspace (encode_device)
-        const char *su = static_cast<const char *>(g.work.ptr) + align256(selab200_encode_workspace_bytes(n_frames, channels));
-        CUDA_TRY(cudaMemcpyAsync(units, su, n_units * sizeof(SearchUnit), cudaMemcpyDeviceToHost, g.stream));
-        CUDA_TRY(cudaMemcpyAsync(trace, d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
-    }
-    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 24, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    uint64_t used, ref;
-    memcpy(&used, g.h_small + 2, 8);
-    memcpy(&ref, g.h_small + 4, 8);
-    *words_used = (size_t)used;
-    *ref_words = (size_t)ref;
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (used > words_capacity)
-        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
-    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    return 0;
-}
-
+// For tests: one unpipelined order-search batch through encode_device, every unit's q[0..99] and reference order
+// from pred.
 int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                   size_t words_capacity, size_t *words_used, size_t *ref_words)
@@ -2544,10 +2531,14 @@ int selab200_encode_search_forced(const int16_t *pcm, uint32_t n_frames, uint32_
     std::lock_guard<std::mutex> lock(g_mutex);
     if (!pred)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    return encode_search_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, ref_words,
-                               nullptr, nullptr);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.ref_words = ref_words;
+    return encode_batch(EncodeMode::search, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
+// For tests: selab200_encode_search_forced (or, without pred, the unforced search) through the tracing search
+// kernels, with the search records and the tracing kernels' records.
 int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                  const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                  size_t words_capacity, size_t *words_used, size_t *ref_words,
@@ -2556,93 +2547,16 @@ int selab200_encode_search_trace(const int16_t *pcm, uint32_t n_frames, uint32_t
     std::lock_guard<std::mutex> lock(g_mutex);
     if (!units || !trace)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    return encode_search_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, ref_words,
-                               units, trace);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.ref_words = ref_words;
+    out.units = units;
+    out.trace = trace;
+    return encode_batch(EncodeMode::search, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
 // For tests: one unpipelined pairing batch through encode_device.  pred: the base's units' predictors, then the
-// candidates'.  par, table, trace (all or none): the choice, the candidate records and their trace records.
-static int encode_pairing_batch(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const selab200_predictor *pred,
-                                selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
-                                size_t *words_used, size_t *base_words, size_t *n_difference, uint8_t *par,
-                                selab200_search_trace *trace)
-{
-    if (int rc = require_ready())
-        return rc;
-    if (!pcm || !descs || !words || !words_used || !base_words || !n_difference)
-        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    if (int rc = check_channels(channels))
-        return rc;
-    *words_used = *base_words = *n_difference = 0;
-    if (n_frames == 0)
-        return 0;
-    const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    const size_t n_pairs = n_sub * channels, n_pred = n_units + n_sub * (channels - 1);
-    for (size_t u = 0; pred && u < n_pred; u++) {
-        const int o = pred[u].order;
-        if (o < 0 || o > kMaxOrder)
-            return fail(SELAB200_ERR_RANGE, "order %d of predictor %zu outside 0..%d", o, u, kMaxOrder);
-        for (int i = 0; i < kMaxOrder; i++)
-            if (i < o ? pred[u].q[i] < -64 || pred[u].q[i] > 63 : pred[u].q[i] != 0)
-                return fail(SELAB200_ERR_RANGE, "q[%d] = %d of predictor %zu (order %d) outside [-64, 63], or not "
-                            "zero past the order", i, pred[u].q[i], u, o);
-    }
-    const size_t pred_bytes = pred ? align256(n_pred * sizeof(selab200_predictor)) : 0;
-    const size_t trace_bytes = trace ? n_pairs * sizeof(selab200_search_trace) : 0;
-    if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
-    if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
-    if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
-    if (int rc = g.work.ensure(selab200_encode_pairing_workspace_bytes(n_frames, channels))) return rc;
-    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
-    uint64_t *d_used = reinterpret_cast<uint64_t *>(static_cast<char *>(g.small.ptr) + 8);
-    unsigned long long *d_totals = reinterpret_cast<unsigned long long *>(static_cast<char *>(g.small.ptr) + 64);
-    const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
-    selab200_search_trace *d_trace =
-        trace ? reinterpret_cast<selab200_search_trace *>(static_cast<char *>(g.aux.ptr) + pred_bytes) : nullptr;
-    CUDA_TRY(cudaMemsetAsync(d_totals, 0, 16, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
-    if (pred)
-        CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_pred * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
-    if (trace)
-        CUDA_TRY(cudaMemsetAsync(d_trace, 0, trace_bytes, g.stream));
-    PairingArgs pa{d_totals, d_totals + 1};
-    pa.d_pred = pred ? d_pred + n_units : nullptr;
-    pa.d_trace = d_trace;
-    EncodeOptions o;
-    o.pairing = &pa;
-    o.d_pred = pred ? d_pred : nullptr;
-    if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
-                               static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
-                               words_capacity, d_used, d_status, g.work.ptr, g.work.bytes, g.stream, o))
-        return rc;
-    if (trace) { // par[] lies behind the candidate table and the means (encode_device)
-        const char *d_par = static_cast<const char *>(g.work.ptr) +
-                            align256(selab200_encode_lossless_workspace_bytes(n_frames, channels)) +
-                            align256(n_pairs * sizeof(PairRecord)) + align256(n_pairs * sizeof(double));
-        CUDA_TRY(cudaMemcpyAsync(par, d_par, n_sub, cudaMemcpyDeviceToHost, g.stream));
-        CUDA_TRY(cudaMemcpyAsync(trace, d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
-    }
-    CUDA_TRY(cudaMemcpyAsync(descs, g.descs.ptr, n_sub * sizeof(selab200_subframe_desc), cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small, g.small.ptr, 16, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaMemcpyAsync(g.h_small + 8, d_totals, 16, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    uint64_t used, base, n_diff;
-    memcpy(&used, g.h_small + 2, 8);
-    memcpy(&base, g.h_small + 8, 8);
-    memcpy(&n_diff, g.h_small + 10, 8);
-    *words_used = (size_t)used;
-    *base_words = (size_t)base;
-    *n_difference = (size_t)n_diff;
-    if (g.h_small[0] != 0)
-        return fail(g.h_small[0], "%s", status_text(g.h_small[0]));
-    if (used > words_capacity)
-        return fail(SELAB200_ERR_CAPACITY, "%s", status_text(SELAB200_ERR_CAPACITY));
-    CUDA_TRY(cudaMemcpyAsync(words, g.words.ptr, used * 4, cudaMemcpyDeviceToHost, g.stream));
-    CUDA_TRY(cudaStreamSynchronize(g.stream));
-    return 0;
-}
-
+// candidates'.
 int selab200_encode_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                    const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                    size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference)
@@ -2650,10 +2564,15 @@ int selab200_encode_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32
     std::lock_guard<std::mutex> lock(g_mutex);
     if (!pred)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    return encode_pairing_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, base_words,
-                                n_difference, nullptr, nullptr);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_difference = n_difference;
+    return encode_batch(EncodeMode::pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
+// For tests: selab200_encode_pairing_forced (or, without pred, the unforced pairing) with the choice, par, and the
+// candidates' trace records.
 int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                   size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference,
@@ -2662,8 +2581,13 @@ int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_
     std::lock_guard<std::mutex> lock(g_mutex);
     if (!par || !trace)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
-    return encode_pairing_batch(pcm, n_frames, channels, pred, descs, words, words_capacity, words_used, base_words,
-                                n_difference, par, trace);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_difference = n_difference;
+    out.par = par;
+    out.trace = trace;
+    return encode_batch(EncodeMode::pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).
@@ -2815,7 +2739,7 @@ int selab200_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t
     if (int rc = g.aux.ensure((size_t)n_streams * 12 + 256)) return rc;
     uint32_t *d_counts = static_cast<uint32_t *>(g.aux.ptr);
     uint32_t *d_k = d_counts + n_streams, *d_nw = d_k + n_streams;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    int32_t *d_status = &device_counters()->status;
     CUDA_TRY(cudaMemsetAsync(d_status, 0, 4, g.stream));
     if (stride)
         CUDA_TRY(cudaMemcpy2DAsync(g.in.ptr, (size_t)pitch * 4, values, (size_t)stride * 4, (size_t)stride * 4, n_streams,
@@ -2848,7 +2772,7 @@ int selab200_rice_decode(const uint32_t *words, const uint32_t *n_words, uint32_
     if (int rc = g.aux.ensure((size_t)n_streams * 12 + 256)) return rc;
     uint32_t *d_nw = static_cast<uint32_t *>(g.aux.ptr);
     uint32_t *d_k = d_nw + n_streams, *d_counts = d_k + n_streams;
-    int32_t *d_status = static_cast<int32_t *>(g.small.ptr);
+    int32_t *d_status = &device_counters()->status;
     CUDA_TRY(cudaMemsetAsync(d_status, 0, 4, g.stream));
     CUDA_TRY(cudaMemsetAsync(g.work.ptr, 0, obytes, g.stream));
     CUDA_TRY(cudaMemcpyAsync(g.words.ptr, words, wbytes, cudaMemcpyHostToDevice, g.stream));

@@ -30,14 +30,6 @@ struct RepairParams {
 
 __host__ __device__ inline uint32_t units_per_frame(uint32_t channels) { return channels == 2 ? 3u : channels; }
 
-// Bytes of repair lists behind the encode workspace (selab200_encode_lossless_workspace_bytes).
-__host__ __device__ inline size_t repair_lists_bytes(uint32_t n_frames, uint32_t channels)
-{
-    const size_t n_units = encode_units(n_frames, channels);
-    auto a256 = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    return 256 + a256((size_t)n_frames * 4) + a256(n_units * sizeof(UnitRecord)) + a256(n_units * sizeof(RepairUnit));
-}
-
 __global__ void __launch_bounds__(256) k_lossless_select(EncodeParams p, RepairParams r)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;

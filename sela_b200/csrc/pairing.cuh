@@ -39,15 +39,6 @@ struct PairingParams {
     selab200_search_trace *trace;       // tests only: [n_frames][C][C] records of the candidates as they were sized
 };
 
-// Bytes of pairing tables behind the lossless workspace (selab200_encode_pairing_workspace_bytes).
-__host__ __device__ inline size_t pairing_tables_bytes(uint32_t n_frames, uint32_t channels)
-{
-    const size_t n_pairs = (size_t)n_frames * channels * channels;
-    auto a256 = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    return a256(n_pairs * sizeof(PairRecord)) + a256(n_pairs * sizeof(double)) + a256((size_t)n_frames * channels) +
-           a256((size_t)n_frames * 4);
-}
-
 __device__ __forceinline__ bool pairing_is_candidate(uint32_t channels, uint32_t p, uint32_t c)
 {
     return p != c && !(channels == 2 && p == 0); // stereo (0, 1): the base's unit 2
