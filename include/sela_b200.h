@@ -379,6 +379,40 @@ int selab200_encode_frames_pairing_device(const int16_t *d_pcm, uint32_t n_frame
                                           uint64_t *d_words_used, uint64_t *d_base_words, uint64_t *d_n_difference,
                                           int32_t *d_status, void *d_workspace, size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------ order search + pairing -- */
+
+/* The smallest files of these encodes, at the highest encode cost (DESIGN.md 7.5): the order search and the channel
+ * pairing together, like the "maximum" setting of other lossless codecs.  The base is selab200_encode_frames_search's
+ * encode of the frame; then every ordered pair (p, c), p != c, of a frame is the difference ch_p - ch_c coded at its
+ * searched order (the order 1..100 with the fewest words whose FIR has no tie; between equal words the reference
+ * encoder's order, else the lowest), and the pairing's choice runs on these words: the assignment with the fewest
+ * words in total, then the fewest difference subframes, then the lexicographically smallest parent vector.  Every
+ * frame takes at most the words of selab200_encode_frames_search on it, and every output decodes back to its source
+ * under this decoder and the unmodified reference decoder.  channels == 1 is the order search.  *base_words receives
+ * the words_used of selab200_encode_frames_search for the same frames (words_used <= base_words always),
+ * *n_difference the number of difference subframes emitted.  Frames are split over devices as for the other batch
+ * calls. */
+int selab200_encode_frames_search_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                          selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                          size_t *words_used, size_t *base_words, size_t *n_difference);
+
+/* selab200_encode_container, with the search + pairing; *base_bytes receives the size of
+ * selab200_encode_container_search's output for the same frames. */
+int selab200_encode_container_search_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                             uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                             size_t capacity, size_t *bytes_used, size_t *base_bytes,
+                                             size_t *n_difference);
+
+/* Device-resident form of selab200_encode_frames_search_pairing: arguments as selab200_encode_frames_device, with
+ * selab200_encode_search_pairing_workspace_bytes() of workspace; *d_base_words and *d_n_difference (uint64, device)
+ * receive the two totals.  Stream-ordered, no synchronisation. */
+size_t selab200_encode_search_pairing_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_encode_frames_search_pairing_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                 selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                 size_t words_capacity, uint64_t *d_words_used, uint64_t *d_base_words,
+                                                 uint64_t *d_n_difference, int32_t *d_status, void *d_workspace,
+                                                 size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------ stage level (host buffers) -- */
 
 /* lpc::ResidueGenerator::process (src/lpc/residue_generator.cpp:121-134) for
@@ -545,6 +579,29 @@ int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_
                                   const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                                   size_t words_capacity, size_t *words_used, size_t *base_words, size_t *n_difference,
                                   uint8_t *par, selab200_search_trace *trace);
+
+/* For tests: selab200_encode_frames_search_pairing on one device and one batch, except that every unit and every
+ * candidate takes its q[0..99] and reference order from pred, as selab200_encode_search_forced takes them.  pred holds
+ * the base's analysis units first, in selab200_encode_trace's order, then one record per candidate in (frame, p, c)
+ * order with the p = c entries skipped, as selab200_encode_pairing_forced orders them (stereo (0, 1) is the base's
+ * searched difference unit and its record is not read).  An order outside 1..100 or a q outside [-64, 63] ->
+ * SELAB200_ERR_RANGE. */
+int selab200_encode_search_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                          const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                          uint32_t *words, size_t words_capacity, size_t *words_used,
+                                          size_t *base_words, size_t *n_difference);
+
+/* For tests: selab200_encode_frames_search_pairing on one device and one batch
+ * (selab200_encode_search_pairing_forced's when pred is not NULL), through the tracing instantiations of the
+ * candidate kernels.  trace[((frame * channels + p) * channels + c) * 100 + order - 1] receives the record of the
+ * candidate ch_p - ch_c at every order 1..100: the reference order's from the analysis kernel, every other order's
+ * from the search kernel.  Stereo (0, 1), which is the base's unit, and the p = c records keep visits 0.
+ * par[frame * channels + c] receives the parent chosen for channel c (c itself: coded alone). */
+int selab200_encode_search_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                         const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                         uint32_t *words, size_t words_capacity, size_t *words_used,
+                                         size_t *base_words, size_t *n_difference, uint8_t *par,
+                                         selab200_search_trace *trace);
 
 #ifdef __cplusplus
 }

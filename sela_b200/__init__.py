@@ -7,5 +7,6 @@ Python mirror used by the tests and bench.py.  No CPU fallback.
 from .codec import (DESC_DTYPE, FRAME, LOSSLESS_DTYPE, VERIFY_DTYPE, SelaB200Error, container_info,  # noqa: F401
                     decode_container, decode_frames, encode_container, encode_container_lossless,
                     encode_container_search, encode_container_verified, encode_frames, encode_frames_lossless,
-                    encode_frames_search, encode_container_pairing, encode_frames_pairing, init,
+                    encode_frames_search, encode_container_pairing, encode_frames_pairing,
+                    encode_container_search_pairing, encode_frames_search_pairing, init,
                     lpc_residues, lpc_samples, rice_decode, rice_encode, verify_container, verify_frames)

@@ -27,6 +27,9 @@ error behaviour as in include/sela_b200.h):
     encode_frames_pairing / encode_container_pairing
                                     the encoder with the channel pairing (DESIGN.md 7.4), and its tests-only
                                     forms encode_pairing_forced / encode_pairing_trace
+    encode_frames_search_pairing / encode_container_search_pairing
+                                    the order search and the channel pairing together (DESIGN.md 7.5), and its
+                                    tests-only forms encode_search_pairing_forced / encode_search_pairing_trace
     encode_lossless_forced          encode with chosen predictors, and the order search with chosen
     / encode_search_forced          coefficients
 
@@ -495,7 +498,8 @@ def encode_container_pairing(pcm, channels, sample_rate, bits_per_sample=16, cap
     return out[:used.value], base.value, nd.value
 
 
-def _pairing_predictors(predictors, n_frames, channels):
+def _pairing_predictors(predictors, n_frames, channels, every_q=False):
+    """every_q: the search's form, q[0..99] whatever the order."""
     n = n_frames * ((3 if channels == 2 else channels) + channels * (channels - 1))
     if isinstance(predictors, np.ndarray) and predictors.dtype == PREDICTOR_DTYPE:
         pred = _c(predictors, PREDICTOR_DTYPE)
@@ -503,7 +507,8 @@ def _pairing_predictors(predictors, n_frames, channels):
         pred = np.zeros(len(predictors), PREDICTOR_DTYPE)
         for rec, (order, q) in zip(pred, predictors):
             rec["order"] = order
-            rec["q"][:order] = np.asarray(q)[:order]
+            n_q = MAX_ORDER if every_q else order
+            rec["q"][:n_q] = np.asarray(q)[:n_q]
     if pred.size != n:
         raise ValueError("%d predictors for %d units and candidates" % (pred.size, n))
     return pred
@@ -548,4 +553,78 @@ def encode_pairing_forced(pcm, channels, predictors, device=0):
     check(L.selab200_encode_pairing_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data, descs.ctypes.data,
                                            words.ctypes.data, cap, C.addressof(used), C.addressof(base),
                                            C.addressof(nd)))
+    return descs, words[:used.value].copy(), base.value, nd.value
+
+
+def encode_frames_search_pairing(pcm, channels, words_capacity=None, device=0):
+    """encode_frames with the order search and the channel pairing together (DESIGN.md 7.5) -> (descs, words,
+    base_words, n_difference): base_words is the number of words encode_frames_search writes for the same frames,
+    n_difference the number of difference subframes emitted."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_frames_search_pairing(pcm.ctypes.data, n_frames, channels, descs.ctypes.data,
+                                                  words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                                  C.addressof(nd)))
+    return descs, words[:used.value].copy(), base.value, nd.value
+
+
+def encode_container_search_pairing(pcm, channels, sample_rate, bits_per_sample=16, capacity=None, device=0):
+    """encode_container with the order search and the channel pairing -> (bytes, base_bytes, n_difference):
+    base_bytes is the size of encode_container_search's output for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_container_search_pairing(pcm.ctypes.data, n_frames, channels, sample_rate,
+                                                     bits_per_sample, out.ctypes.data, cap, C.addressof(used),
+                                                     C.addressof(base), C.addressof(nd)))
+    return out[:used.value], base.value, nd.value
+
+
+def encode_search_pairing_trace(pcm, channels, predictors=None, device=0):
+    """encode_frames_search_pairing on one batch through the tracing candidate kernels -> (descs, words, base_words,
+    n_difference, par, trace).
+
+    predictors (None: analyse): PREDICTOR_DTYPE records or (order, q[100]) pairs, as encode_search_forced takes
+    them: the base's analysis units in encode_trace's order, then one per candidate in (frame, p, c) order without
+    p = c.  par: uint8 [n_frames, channels], the parent chosen per channel.  trace: SEARCH_TRACE_DTYPE [n_frames,
+    channels, channels, 100], entry [f, p, c, order - 1] the candidate ch_p - ch_c at that order."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    pred = None if predictors is None else _pairing_predictors(predictors, n_frames, channels, every_q=True)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    par = np.zeros((n_frames, channels), np.uint8)
+    trace = np.zeros((n_frames, channels, channels, MAX_ORDER), SEARCH_TRACE_DTYPE)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_pairing_trace(pcm.ctypes.data, n_frames, channels,
+                                                 None if pred is None else pred.ctypes.data, descs.ctypes.data,
+                                                 words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                                 C.addressof(nd), par.ctypes.data, trace.ctypes.data))
+    return descs, words[:used.value].copy(), base.value, nd.value, par, trace
+
+
+def encode_search_pairing_forced(pcm, channels, predictors, device=0):
+    """encode_frames_search_pairing on one batch with every unit and candidate taking its q[0..99] and reference
+    order from `predictors` (as encode_search_pairing_trace takes them) -> (descs, words, base_words, n_difference)."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    pred = _pairing_predictors(predictors, n_frames, channels, every_q=True)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nd = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_pairing_forced(pcm.ctypes.data, n_frames, channels, pred.ctypes.data,
+                                                  descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
+                                                  C.addressof(base), C.addressof(nd)))
     return descs, words[:used.value].copy(), base.value, nd.value

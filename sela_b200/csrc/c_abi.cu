@@ -17,6 +17,7 @@
 #include "lossless.cuh"
 #include "pairing.cuh"
 #include "search.cuh"
+#include "search_pairing.cuh"
 #include "verify.cuh"
 
 using namespace selab200;
@@ -76,8 +77,8 @@ struct Counters {
     int32_t status;                  // the device status of the call
     uint64_t used;                   // encode: the word arena's fill level
     unsigned long long ref_words;    // search: the words the reference encoder's choice takes
-    unsigned long long base_words;   // pairing: the words of its base, the lossless encode
-    unsigned long long n_difference; // pairing: the difference subframes chosen
+    unsigned long long base_words;   // pairing: the words of its base, the lossless encode (search_pairing: the search)
+    unsigned long long n_difference; // pairing, search_pairing: the difference subframes chosen
     uint32_t selftest;               // selab200_selftest: the mismatches
     // host side only (collect_records): a count of set records, and the decode status that follows a verify count
     unsigned long long n_records;
@@ -380,7 +381,8 @@ int launch_lossless(const EncodeParams &p, const RepairParams &r, size_t n_frame
 
 // The order search (search.cuh) in place of k_encode_units: analysis, candidates, repack, and the reference encoder's
 // words added to *d_ref_words.  The warp kernels have grids of a fixed size, at most one residue row per unit of the
-// batch.  FORCE: the units' q and reference orders are d_pred's (selab200_encode_search_forced).  d_trace: the
+// batch.  d_ref_words null (the base of a search + pairing): k_search_ref_words is not run.  FORCE: the units' q and
+// reference orders are d_pred's (selab200_encode_search_forced).  d_trace: the
 // analysis and candidate kernels are their tracing instantiations, which write every (unit, order) record there
 // (selab200_encode_search_trace).
 template <bool STEREO, bool FORCE = false>
@@ -413,9 +415,11 @@ int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t
         k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
     if (int rc = launch_check("k_search_candidates"))
         return rc;
-    k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
-    if (int rc = launch_check("k_search_ref_words"))
-        return rc;
+    if (d_ref_words) {
+        k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
+        if (int rc = launch_check("k_search_ref_words"))
+            return rc;
+    }
     k_search_repack<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
     return launch_check("k_search_repack");
 }
@@ -445,18 +449,64 @@ int launch_pairing(const EncodeParams &p, const PairingParams &q, size_t n_frame
     return launch_check("k_pairing_repack");
 }
 
+// The search + pairing (search_pairing.cuh) between the order search and the scan: means, the candidates' analysis
+// and search, the table, the choice, and the winning differences packed at their searched orders in place of their
+// channels.  The warp kernels have grids of a fixed size, at most one residue row per unit of the batch.  d_trace:
+// the candidates' analysis and search kernels are their tracing instantiations (q.trace is d_trace).
+int launch_search_pairing(const EncodeParams &p, const PairingParams &q, SearchUnit *cand, size_t n_frames,
+                          size_t n_units, cudaStream_t stream, bool trace)
+{
+    constexpr size_t smem = encode_smem_bytes<true>(), smem_orders = search_smem_bytes<true>();
+    if (int rc = set_smem(trace ? k_search_pairing_units_trace : k_search_pairing_units, smem))
+        return rc;
+    if (int rc = trace ? set_smem(k_search_pairing_candidates_trace, smem_orders)
+                       : set_smem(k_search_pairing_candidates, smem_orders))
+        return rc;
+    if (int rc = set_smem(k_search_pairing_repack, smem_orders))
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(q.stale, 0, n_frames * sizeof(uint32_t), stream)); // every searched unit is tie-free
+    const size_t n_pairs = n_frames * p.channels * p.channels;
+    k_pairing_means<<<(unsigned)((n_pairs + 127) / 128), 128, 0, stream>>>(p, q);
+    if (int rc = launch_check("k_pairing_means"))
+        return rc;
+    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
+    if (trace)
+        k_search_pairing_units_trace<<<warps, 32, smem, stream>>>(p, q, cand);
+    else
+        k_search_pairing_units<<<warps, 32, smem, stream>>>(p, q, cand);
+    if (int rc = launch_check("k_search_pairing_units"))
+        return rc;
+    if (trace)
+        k_search_pairing_candidates_trace<<<warps, 32, smem_orders, stream>>>(p, cand, q.trace);
+    else
+        k_search_pairing_candidates<<<warps, 32, smem_orders, stream>>>(p, cand);
+    if (int rc = launch_check("k_search_pairing_candidates"))
+        return rc;
+    k_search_pairing_table<<<(unsigned)((n_pairs + 255) / 256), 256, 0, stream>>>(p, q, cand);
+    if (int rc = launch_check("k_search_pairing_table"))
+        return rc;
+    k_pairing_select<<<(unsigned)std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream>>>(p, q);
+    if (int rc = launch_check("k_pairing_select"))
+        return rc;
+    k_search_pairing_repack<<<warps, 32, smem_orders, stream>>>(p, q, cand);
+    return launch_check("k_search_pairing_repack");
+}
+
 // Which encoder an encode call runs.  lossless: re-code every subframe the reference decoder would not reproduce
 // (DESIGN.md 7.2).  search: code every subframe at the predictor order with the fewest words (7.3).  pairing: code
-// channels as differences wherever that takes fewer words, on top of the lossless encode (7.4).
-enum class EncodeMode { plain, lossless, search, pairing };
+// channels as differences wherever that takes fewer words, on top of the lossless encode (7.4).  search_pairing: the
+// pairing on top of the search, every channel and every difference at its cheapest order (7.5).
+enum class EncodeMode { plain, lossless, search, pairing, search_pairing };
 
 // Where every region of an encode workspace lies, as byte offsets from its base, and its size.  Every mode has the
 // plain encode's regions; lossless and pairing add the repair lists, search the SearchUnits, and pairing the pairing
-// tables behind the repair lists.  The offsets of the regions a mode lacks are 0.
+// tables behind the repair lists.  search_pairing has the SearchUnits (every region padded), the pairing tables and
+// the candidates' SearchUnits.  The offsets of the regions a mode lacks are 0.
 struct EncodeLayout {
     size_t units, slots, means, residues;                       // EncodeParams
     size_t repair_count, repair_frames, repair_orig, repair_units; // RepairParams
     size_t search;                                              // SearchUnit[n_units]
+    size_t pair_search;                                         // search_pairing: SearchUnit[n_frames][C][C]
     size_t pair_table, pair_means, par, stale;                  // PairingParams
     size_t bytes;                                               // selab200_encode_*_workspace_bytes
 };
@@ -487,12 +537,16 @@ EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels
         l.repair_orig = region(n_units * sizeof(UnitRecord));
         l.repair_units = region(n_units * sizeof(RepairUnit));
     }
-    if (mode == EncodeMode::pairing) {
+    if (mode == EncodeMode::search_pairing)
+        l.search = region(n_units * sizeof(SearchUnit));
+    if (mode == EncodeMode::pairing || mode == EncodeMode::search_pairing) {
         l.pair_table = region(n_pairs * sizeof(PairRecord));
         l.pair_means = region(n_pairs * sizeof(double));
         l.par = region(n_sub);
         l.stale = region((size_t)n_frames * 4);
     }
+    if (mode == EncodeMode::search_pairing)
+        l.pair_search = region(n_pairs * sizeof(SearchUnit));
     l.bytes = at;
     return l;
 }
@@ -521,15 +575,17 @@ struct EncodeOptions {
     unsigned long long sub_base = 0;            // ... where the batch's first subframe is subframe sub_base
     LosslessArgs lossless{};                    // lossless: where the re-coded pairs are reported
     unsigned long long *d_ref_words = nullptr;  // search: += the reference encoder's words
-    unsigned long long *d_base_words = nullptr; // pairing: += the words of its base, the lossless encode ...
+    unsigned long long *d_base_words = nullptr; // pairing, search_pairing: += the words of its base, the lossless
+                                                // encode or the search ...
     unsigned long long *d_n_difference = nullptr; // ... and the difference subframes chosen
     // tests only
     selab200_analysis_trace *d_trace = nullptr;      // plain: the tracing unit kernel writes every unit's analysis here
-    const selab200_predictor *d_pred = nullptr;      // lossless, search, pairing: every unit's predictor (pairing: its
-                                                     // base's units)
-    const selab200_predictor *d_pair_pred = nullptr; // pairing: the candidates' predictors (PairingParams::pred)
-    selab200_search_trace *d_search_trace = nullptr; // search, pairing: the tracing kernels write every (unit, order) /
-                                                     // candidate record here
+    const selab200_predictor *d_pred = nullptr;      // lossless, search, pairing, search_pairing: every unit's
+                                                     // predictor (pairing, search_pairing: its base's units)
+    const selab200_predictor *d_pair_pred = nullptr; // pairing, search_pairing: the candidates' predictors
+                                                     // (PairingParams::pred)
+    selab200_search_trace *d_search_trace = nullptr; // search, pairing, search_pairing: the tracing kernels write every
+                                                     // (unit, order) / candidate / (candidate, order) record here
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -543,7 +599,8 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
         return fail(SELAB200_ERR_ARGUMENT, "stereo PCM must be 16-byte aligned on the device");
-    const bool pairing = o.mode == EncodeMode::pairing;
+    const bool search_pairing = o.mode == EncodeMode::search_pairing;
+    const bool pairing = o.mode == EncodeMode::pairing || search_pairing; // the pairing tables, counters and patch
     const size_t n_sub = (size_t)n_frames * channels;
     if (o.fresh) {
         CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(int32_t), stream));
@@ -593,7 +650,7 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         q.trace = o.d_search_trace;
     }
     const PairingParams *pq = pairing ? &q : nullptr;
-    if (o.mode == EncodeMode::lossless || pairing) {
+    if (o.mode == EncodeMode::lossless || o.mode == EncodeMode::pairing) {
         const LosslessArgs la = pairing ? LosslessArgs{} : o.lossless; // the pairing's base takes no report
         RepairParams r;
         r.count = reinterpret_cast<uint32_t *>(ws + l.repair_count);
@@ -614,16 +671,21 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         if (pairing)
             if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
                 return rc;
-    } else if (o.mode == EncodeMode::search) {
+    } else if (o.mode == EncodeMode::search || search_pairing) {
+        // the base of a search + pairing takes no reference words and no trace (its candidates are traced)
         SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
-        unsigned long long *rw = o.d_ref_words;
-        selab200_search_trace *tr = o.d_search_trace;
+        unsigned long long *rw = search_pairing ? nullptr : o.d_ref_words;
+        selab200_search_trace *tr = search_pairing ? nullptr : o.d_search_trace;
         const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr)
                                           : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr))
                                 : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr)
                                           : launch_search<false>(p, su, n_frames, n_units, rw, stream, nullptr, tr));
         if (rc)
             return rc;
+        if (search_pairing)
+            if (int rc = launch_search_pairing(p, q, reinterpret_cast<SearchUnit *>(ws + l.pair_search), n_frames,
+                                               n_units, stream, o.d_search_trace != nullptr))
+                return rc;
     } else {
         const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
                                                  : launch_encode_units<true, false>(p, n_units, nullptr, stream))
@@ -1116,6 +1178,11 @@ size_t selab200_encode_search_workspace_bytes(uint32_t n_frames, uint32_t channe
     return encode_layout(EncodeMode::search, n_frames, channels).bytes;
 }
 
+size_t selab200_encode_search_pairing_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    return encode_layout(EncodeMode::search_pairing, n_frames, channels).bytes;
+}
+
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_sub = (size_t)n_frames * channels;
@@ -1190,6 +1257,25 @@ int selab200_encode_frames_pairing_device(const int16_t *d_pcm, uint32_t n_frame
         return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
     EncodeOptions o;
     o.mode = EncodeMode::pairing;
+    o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
+    o.d_n_difference = reinterpret_cast<unsigned long long *>(d_n_difference);
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
+}
+
+int selab200_encode_frames_search_pairing_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                 selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                 size_t words_capacity, uint64_t *d_words_used, uint64_t *d_base_words,
+                                                 uint64_t *d_n_difference, int32_t *d_status, void *d_workspace,
+                                                 size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_base_words || !d_n_difference || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    EncodeOptions o;
+    o.mode = EncodeMode::search_pairing;
     o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
     o.d_n_difference = reinterpret_cast<unsigned long long *>(d_n_difference);
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
@@ -1324,9 +1410,10 @@ struct EncodeTarget {
 struct Result {
     size_t words = 0;                  // encode: the words used (for CAPACITY: the size the caller needs)
     unsigned long long ref_words = 0;  // search: the words the reference encoder's choice takes
-    unsigned long long base_words = 0; // pairing: the words of its base, the lossless encode
-    unsigned long long n_difference = 0; // pairing: the difference subframes chosen
-    size_t ref_bytes = 0;              // container search / pairing: the size of the output it is measured against
+    unsigned long long base_words = 0; // pairing: the words of its base, the lossless encode (search_pairing: the search)
+    unsigned long long n_difference = 0; // pairing, search_pairing: the difference subframes chosen
+    size_t ref_bytes = 0;              // container search / pairing / search_pairing: the size of the output it is
+                                       // measured against
     std::vector<selab200_lossless_entry> recoded; // lossless: the re-coded (frame, channel) pairs
     std::vector<selab200_verify_entry> report;    // verify: the (frame, channel) pairs that do not decode back
     void add(const Result &b)
@@ -1917,6 +2004,26 @@ int selab200_encode_frames_pairing(const int16_t *pcm, uint32_t n_frames, uint32
     return rc;
 }
 
+int selab200_encode_frames_search_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                          selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                          size_t *words_used, size_t *base_words, size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !base_words || !n_difference)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::search_pairing, r);
+    *words_used = r.words;
+    *base_words = (size_t)r.base_words;
+    *n_difference = (size_t)r.n_difference;
+    return rc;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -1950,7 +2057,9 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, r.words);
     r.ref_bytes = (size_t)container_frame_byte(n_frames, channels,
-                                               mode == EncodeMode::pairing ? r.base_words : r.ref_words);
+                                               mode == EncodeMode::pairing || mode == EncodeMode::search_pairing
+                                                   ? r.base_words
+                                                   : r.ref_words);
     return rc;
 }
 
@@ -2031,6 +2140,25 @@ int selab200_encode_container_pairing(const int16_t *pcm, uint32_t n_frames, uin
     Result r;
     const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
                                          bytes_used, EncodeMode::pairing, false, r);
+    *base_bytes = r.ref_bytes;
+    *n_difference = (size_t)r.n_difference;
+    return rc;
+}
+
+int selab200_encode_container_search_pairing(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                             uint32_t sample_rate, uint16_t bits_per_sample, uint8_t *container,
+                                             size_t capacity, size_t *bytes_used, size_t *base_bytes,
+                                             size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!base_bytes || !n_difference) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    Result r;
+    const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                         bytes_used, EncodeMode::search_pairing, false, r);
     *base_bytes = r.ref_bytes;
     *n_difference = (size_t)r.n_difference;
     return rc;
@@ -2373,13 +2501,14 @@ static_assert(sizeof(selab200_search_unit) == sizeof(SearchUnit) &&
 struct BatchOutputs {
     size_t *words_used = nullptr;
     size_t *ref_words = nullptr;                           // search
-    size_t *base_words = nullptr, *n_difference = nullptr; // pairing
+    size_t *base_words = nullptr, *n_difference = nullptr; // pairing, search_pairing
     selab200_lossless_entry *entries = nullptr;            // lossless: the re-coded pairs
     size_t entries_capacity = 0, *n_entries = nullptr;
     selab200_analysis_trace *analysis = nullptr;           // plain: the tracing unit kernel's records
-    selab200_search_trace *trace = nullptr;                // search, pairing: the tracing kernels' records ...
-    selab200_search_unit *units = nullptr;                 // ... and the search records
-    uint8_t *par = nullptr;                                // ... and the pairing's choice
+    selab200_search_trace *trace = nullptr;                // search, pairing, search_pairing: the tracing kernels'
+                                                           // records ...
+    selab200_search_unit *units = nullptr;                 // ... and the search records (search)
+    uint8_t *par = nullptr;                                // ... and the pairing's choice (pairing, search_pairing)
 };
 
 // A test hook's predictors: every order in min_order..kMaxOrder, every q in [-64, 63], and with zero_past, every q
@@ -2403,7 +2532,7 @@ static int check_predictors(const selab200_predictor *pred, size_t n, int min_or
 }
 
 // For tests: one unpipelined batch of `mode` through encode_device on g.stream.  pred (lossless: required): every
-// unit's predictor, for the pairing followed by the candidates' (include/sela_b200.h).
+// unit's predictor, for the pairing and the search + pairing followed by the candidates' (include/sela_b200.h).
 static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                         const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
                         size_t words_capacity, const BatchOutputs &out)
@@ -2411,7 +2540,9 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     if (int rc = require_ready())
         return rc;
     const bool lossless = mode == EncodeMode::lossless, search = mode == EncodeMode::search,
-               pairing = mode == EncodeMode::pairing;
+               search_pairing = mode == EncodeMode::search_pairing,
+               pairing = mode == EncodeMode::pairing || search_pairing;
+    const bool every_q = search || search_pairing; // predictors are q[0..99] and a reference order 1..100
     if (!pcm || !descs || !words || !out.words_used || (mode == EncodeMode::plain && !out.analysis) ||
         (lossless && (!pred || (!out.entries && out.entries_capacity) || !out.n_entries)) ||
         (search && !out.ref_words) || (pairing && (!out.base_words || !out.n_difference)))
@@ -2430,12 +2561,14 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
     const size_t n_pred = pairing ? n_units + n_sub * (channels - 1) : n_units;
     if (pred)
-        if (int rc = check_predictors(pred, n_pred, search ? 1 : 0, !search, pairing ? "predictor" : "unit"))
+        if (int rc = check_predictors(pred, n_pred, every_q ? 1 : 0, !every_q, pairing ? "predictor" : "unit"))
             return rc;
     const EncodeLayout l = encode_layout(mode, n_frames, channels);
     const size_t pred_bytes = pred ? align256(n_pred * sizeof(selab200_predictor)) : 0;
+    const size_t n_records = search_pairing ? n_sub * channels * kMaxOrder : pairing ? n_sub * channels
+                                                                                    : n_units * kMaxOrder;
     const size_t trace_bytes = out.analysis ? n_units * sizeof(selab200_analysis_trace)
-                               : out.trace  ? (pairing ? n_sub * channels : n_units * kMaxOrder) * sizeof(selab200_search_trace)
+                               : out.trace  ? n_records * sizeof(selab200_search_trace)
                                             : 0;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
@@ -2588,6 +2721,43 @@ int selab200_encode_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_
     out.par = par;
     out.trace = trace;
     return encode_batch(EncodeMode::pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
+}
+
+// For tests: one unpipelined search + pairing batch through encode_device.  pred: the base's units' q[0..99] and
+// reference orders, then the candidates'.
+int selab200_encode_search_pairing_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                          const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                          uint32_t *words, size_t words_capacity, size_t *words_used,
+                                          size_t *base_words, size_t *n_difference)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!pred)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_difference = n_difference;
+    return encode_batch(EncodeMode::search_pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
+}
+
+// For tests: selab200_encode_search_pairing_forced (or, without pred, the unforced search + pairing) through the
+// tracing candidate kernels, with the choice, par, and every (candidate, order) record.
+int selab200_encode_search_pairing_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                         const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                         uint32_t *words, size_t words_capacity, size_t *words_used,
+                                         size_t *base_words, size_t *n_difference, uint8_t *par,
+                                         selab200_search_trace *trace)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!par || !trace)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_difference = n_difference;
+    out.par = par;
+    out.trace = trace;
+    return encode_batch(EncodeMode::search_pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

@@ -344,6 +344,38 @@ __device__ __forceinline__ Signal stage_unit(const EncodeParams &p, const uint32
     return sig;
 }
 
+// Stages d = ch_par - ch_c of `frame` (17 bits) at smem as stage_unit stages the stereo difference: d >> 1 in the
+// int16 row, d & 1 in the bit array behind it, kHistoryPad zeros in front of both.  The channel pairing's candidates
+// (pairing.cuh, search_pairing.cuh).
+__device__ __forceinline__ Signal stage_pair(const EncodeParams &p, uint32_t frame, uint32_t par, uint32_t c,
+                                             unsigned char *smem)
+{
+    constexpr int kRow = kHistoryPad + kFrame;
+    int16_t *s16 = reinterpret_cast<int16_t *>(smem);
+    uint32_t *lo_bits = reinterpret_cast<uint32_t *>(smem + kRow * 2);
+    const int lane = lane_id();
+    const int16_t *src = p.pcm + (size_t)frame * kFrame * p.channels;
+    for (int j = lane; j < kHistoryPad / 2; j += 32)
+        reinterpret_cast<uint32_t *>(s16)[j] = 0;
+    if (lane < kHistoryPad / 32)
+        lo_bits[lane] = 0;
+    int16_t *row = s16 + kHistoryPad;
+    uint32_t *lo = lo_bits + kHistoryPad / 32;
+    for (int it = 0; it < kFrame / 32; it++) {
+        const size_t j = (size_t)(it * 32 + lane) * p.channels;
+        const int d = (int)src[j + par] - (int)src[j + c];
+        row[it * 32 + lane] = (int16_t)(d >> 1);
+        const uint32_t bits = __ballot_sync(kFull, d & 1);
+        if (lane == 0)
+            lo[it] = bits;
+    }
+    __syncwarp();
+    Signal sig;
+    sig.a = row;
+    sig.lo = lo;
+    return sig;
+}
+
 // Shared memory of the signal staged by stage_unit.
 template <bool STEREO>
 __host__ __device__ constexpr size_t unit_signal_bytes()

@@ -22,7 +22,11 @@
 
 namespace selab200 {
 
-struct __align__(16) PairRecord { // one candidate (p, c) of a frame
+// One candidate (p, c) of a frame.  In the search + pairing (search_pairing.cuh) k_search_pairing_table fills it from
+// the candidate's searched key: res_words the searched words (reflection + residue), order the searched order,
+// refl_words, refl_k and res_k 0, tie 0 (every searched order is tie-free).  k_pairing_select reads only the sum of
+// the two word counts and tie.
+struct __align__(16) PairRecord {
     uint32_t refl_words, res_words;
     uint8_t order, refl_k, res_k, tie;
     uint32_t pad;
@@ -87,45 +91,18 @@ __global__ void __launch_bounds__(128) k_pairing_means(EncodeParams p, PairingPa
     q.means[i] = chain.mean();
 }
 
-// Stages d = ch_par - ch_c of `frame` (17 bits) at smem as stage_unit stages the stereo difference: d >> 1 in the
-// int16 row, d & 1 in the bit array behind it, kHistoryPad zeros in front of both.
-__device__ __forceinline__ Signal stage_pair(const EncodeParams &p, uint32_t frame, uint32_t par, uint32_t c,
-                                             unsigned char *smem)
-{
-    constexpr int kRow = kHistoryPad + kFrame;
-    int16_t *s16 = reinterpret_cast<int16_t *>(smem);
-    uint32_t *lo_bits = reinterpret_cast<uint32_t *>(smem + kRow * 2);
-    const int lane = lane_id();
-    const int16_t *src = p.pcm + (size_t)frame * kFrame * p.channels;
-    for (int j = lane; j < kHistoryPad / 2; j += 32)
-        reinterpret_cast<uint32_t *>(s16)[j] = 0;
-    if (lane < kHistoryPad / 32)
-        lo_bits[lane] = 0;
-    int16_t *row = s16 + kHistoryPad;
-    uint32_t *lo = lo_bits + kHistoryPad / 32;
-    for (int it = 0; it < kFrame / 32; it++) {
-        const size_t j = (size_t)(it * 32 + lane) * p.channels;
-        const int d = (int)src[j + par] - (int)src[j + c];
-        row[it * 32 + lane] = (int16_t)(d >> 1);
-        const uint32_t bits = __ballot_sync(kFull, d & 1);
-        if (lane == 0)
-            lo[it] = bits;
-    }
-    __syncwarp();
-    Signal sig;
-    sig.a = row;
-    sig.lo = lo;
-    return sig;
-}
-
-// Candidate (par, c) of `frame` by one warp, with the steps of encode_unit on a stereo difference.  res: the warp's
-// residue row.
+// Candidate (par, c) of `frame` by one warp, with the steps of encode_unit on a stereo difference (stage_pair in
+// kernels.cuh stages it).  res: the warp's residue row.
 //   PACK = false  FIR with the tie check, Rice sizes, the candidate's record into the table
 //   PACK = true   FIR, Rice, pack into the slot of unit `out` and rewrite its record
-template <bool PACK>
+//   SEARCH        (PACK = false; search + pairing, search_pairing.cuh) as kUnitSearch does for a unit: every q and
+//                 the reference order's words and key into su[(frame, par, c)], nothing into the table.  TRACE: the
+//                 reference order's search record into q.trace
+template <bool PACK, bool SEARCH = false, bool TRACE = false>
 __device__ __forceinline__ void pair_unit(const EncodeParams &p, const PairingParams &q, uint32_t frame, uint32_t par,
-                                          uint32_t c, int32_t *res, uint32_t out)
+                                          uint32_t c, int32_t *res, uint32_t out, SearchUnit *su = nullptr)
 {
+    static_assert(!SEARCH || !PACK, "the search packs through search_orders");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<true>();
     AnalysisScratch &scratch = *reinterpret_cast<AnalysisScratch *>(smem_raw + kSigBytes);
@@ -145,11 +122,25 @@ __device__ __forceinline__ void pair_unit(const EncodeParams &p, const PairingPa
         __syncwarp();
     }
     warp_coefficients(cf, scratch.t(), order);
+    if constexpr (SEARCH) { // every q, from k[] (still intact) or as forced
+        for (int i = lane; i < kMaxOrder; i += 32)
+            su[idx].q[i] = q.pred ? cf.q[i] : quantise_reflection(i, scratch.kk()[i]);
+        __syncwarp();
+    }
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring); // over k[] and the step-up row, dead now
     const bool tie = warp_fir_residual<true, !PACK>(sig, cf, order, planes, res);
     const RiceChoice cq = warp_rice_choose(cf.q, order);
     const RiceChoice cr = warp_rice_choose(res, kFrame);
-    if constexpr (!PACK) {
+    if constexpr (SEARCH) {
+        if constexpr (TRACE)
+            search_trace_record(q.trace, (uint32_t)idx, order, cf, res, tie, cq, cr);
+        if (lane == 0) {
+            SearchUnit &s = su[idx];
+            s.ref_order = order;
+            s.ref_words = cq.words + cr.words;
+            s.best = tie ? kNoCandidate : (unsigned long long)(cq.words + cr.words) << 8;
+        }
+    } else if constexpr (!PACK) {
         if (q.trace) {
             search_trace_record(q.trace + idx, 0, 1, cf, res, tie, cq, cr);
             if (lane == 0)

@@ -68,9 +68,13 @@ __device__ __forceinline__ void step_up(double *t, int i, int q)
 //                 check, Rice sizes, a tie-free order into su[unit].best
 //   PACK = true   (o_lo = o_hi) FIR, Rice, pack into the unit's slot and rewrite its record
 // TRACE (PACK = false, tests only, selab200_encode_search_trace): each order's record into trace as well.
-template <bool STEREO, bool PACK, bool TRACE = false>
+// PAIR (search + pairing, search_pairing.cuh; STEREO = true for its shared memory layout): `unit` is the candidate
+// (frame, par, c) at ((frame * C + par) * C + c) of su and trace, its signal ch_par - ch_c from stage_pair, its FIR
+// always the wide one, and PACK packs into unit `out`.  Without PAIR, PACK packs into `unit` and `out` is unused.
+template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false>
 __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
-                                              int o_hi, int32_t *res, selab200_search_trace *trace = nullptr)
+                                              int o_hi, int32_t *res, selab200_search_trace *trace = nullptr,
+                                              uint32_t out = 0)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
@@ -78,10 +82,17 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kSearchStepBytes);
     uint32_t *planes = reinterpret_cast<uint32_t *>(smem_raw + kSigBytes + kSearchStepBytes + sizeof(CoefSmem));
     static_assert(kSearchStepBytes % 16 == 0 && sizeof(CoefSmem) % 16 == 0, "search shared memory layout");
+    static_assert(!PAIR || STEREO, "a pair is staged as the stereo difference is");
 
     const int lane = lane_id();
-    const bool wide = STEREO && unit % 3 == 2;
-    const Signal sig = stage_unit<STEREO>(p, unit, smem_raw);
+    const bool wide = PAIR || (STEREO && unit % 3 == 2);
+    const uint32_t dst = PAIR ? out : unit;
+    Signal sig;
+    if constexpr (PAIR)
+        sig = stage_pair(p, unit / (p.channels * p.channels), unit / p.channels % p.channels, unit % p.channels,
+                         smem_raw);
+    else
+        sig = stage_unit<STEREO>(p, unit, smem_raw);
     SearchUnit &s = su[unit];
     const int ref = (int)s.ref_order;
     for (int i = lane; i < 104; i += 32)
@@ -119,7 +130,7 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
         } else {
             const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
             if (!too_large) {
-                uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
+                uint32_t *slot = p.slots + (size_t)dst * kSlotWords;
                 warp_rice_pack(cf.q, o, cq, slot);
                 warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
             }
@@ -132,7 +143,7 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
                 u.res_words = cr.words;
                 u.flags = too_large ? 1u : 0u;
                 u.pad[0] = u.pad[1] = 0;
-                p.units[unit] = u;
+                p.units[dst] = u;
             }
         }
         __syncwarp();

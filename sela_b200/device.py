@@ -99,6 +99,26 @@ class DeviceCodec:
             self.capacity, self.words_used.data_ptr(), self.base_words.data_ptr(), self.n_difference.data_ptr(),
             self.status.data_ptr(), self.pairing_ws.data_ptr(), self.pairing_ws_bytes, C.c_void_p(stream)))
 
+    def encode_search_pairing(self, pcm):
+        """encode with the order search and the channel pairing together (DESIGN.md 7.5).  Asynchronous;
+        self.base_words and self.n_difference (int64 cuda tensors) receive the words encode_search() writes for the
+        same frames and the number of difference subframes.  The workspace is allocated on first use."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.numel() == self.n_sub * FRAME
+        L = lib()
+        if not hasattr(self, "search_pairing_ws"):
+            self.search_pairing_ws_bytes = L.selab200_encode_search_pairing_workspace_bytes(self.n_frames,
+                                                                                            self.channels)
+            self.search_pairing_ws = torch.zeros(self.search_pairing_ws_bytes, dtype=torch.uint8, device=self.device)
+        if not hasattr(self, "base_words"):
+            self.base_words = torch.zeros(1, dtype=torch.int64, device=self.device)
+            self.n_difference = torch.zeros(1, dtype=torch.int64, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_encode_frames_search_pairing_device(
+            pcm.data_ptr(), self.n_frames, self.channels, self.descs.data_ptr(), self.words.data_ptr(),
+            self.capacity, self.words_used.data_ptr(), self.base_words.data_ptr(), self.n_difference.data_ptr(),
+            self.status.data_ptr(), self.search_pairing_ws.data_ptr(), self.search_pairing_ws_bytes,
+            C.c_void_p(stream)))
+
     def decode(self, pcm_out, n_words):
         """Decode self.descs / self.words[:n_words] into pcm_out (int16 cuda tensor). Asynchronous."""
         assert pcm_out.dtype == torch.int16 and pcm_out.is_cuda and pcm_out.numel() == self.n_sub * FRAME

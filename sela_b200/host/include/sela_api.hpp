@@ -123,7 +123,7 @@ class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
     void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                  size_t *refBytes = nullptr, size_t *differences = nullptr);
+                  size_t *refBytes = nullptr, size_t *differences = nullptr, bool searchBase = false);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -152,6 +152,11 @@ public:
     // fewest words (selab200_encode_container_pairing).  Returns the bytes written; `losslessBytes` receives the
     // bytes processLosslessTo() writes for the same input, `differences` the number of difference subframes.
     size_t processPairingTo(std::ofstream &outputFile, size_t &losslessBytes, size_t &differences);
+    // Not in the reference: the smallest of these files, at the highest encode cost: processPairingTo() on top of
+    // processSearchTo(), every channel and every channel difference at the order with the fewest words
+    // (selab200_encode_container_search_pairing).  Returns the bytes written; `searchBytes` receives the bytes
+    // processSearchTo() writes for the same input, `differences` the number of difference subframes.
+    size_t processSearchPairingTo(std::ofstream &outputFile, size_t &searchBytes, size_t &differences);
 };
 class Decoder {
     void readFrames();

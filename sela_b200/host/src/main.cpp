@@ -14,6 +14,9 @@
 // alone or as its difference from another, whichever takes the fewest words, for any channel count, and decoding back
 // to the WAV under the reference decoder), one line with the bytes written, the bytes -L writes and the number of
 // difference subframes.
+// `-B in.wav out.sela` ("best"): -S and -P together, every channel and every channel difference at the order with the
+// fewest words; the smallest file of these modes at the highest encode cost, decoding back to the WAV under the
+// reference decoder.  One line with the bytes written, the bytes -S writes and the number of difference subframes.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -109,6 +112,8 @@ int usage(const std::string &prog)
               << " -S path/to/input.wav path/to/output.sela\n\n"
               << "Encoding a file smaller, pairing the channels of every frame (H100 build):\n" << prog
               << " -P path/to/input.wav path/to/output.sela\n\n"
+              << "Encoding a file smallest, searching the predictor orders and pairing the channels (H100 build):\n"
+              << prog << " -B path/to/input.wav path/to/output.sela\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -189,6 +194,14 @@ int main(int argc, char **argv)
             size_t losslessBytes = 0, differences = 0;
             const size_t written = sela::Encoder(in).processPairingTo(out, losslessBytes, differences);
             std::cout << "Wrote " << written << " bytes (-L: " << losslessBytes << " bytes), " << differences
+                      << " difference subframes" << std::endl;
+        } else if (mode == "-B" && argc == 4) {
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Encoding with the order search and the channel pairing: " << argv[2] << std::endl;
+            size_t searchBytes = 0, differences = 0;
+            const size_t written = sela::Encoder(in).processSearchPairingTo(out, searchBytes, differences);
+            std::cout << "Wrote " << written << " bytes (-S: " << searchBytes << " bytes), " << differences
                       << " difference subframes" << std::endl;
         } else if (mode == "-t" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);

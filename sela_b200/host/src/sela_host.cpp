@@ -810,11 +810,19 @@ size_t Encoder::processPairingTo(std::ofstream &outputFile, size_t &losslessByte
     return (size_t)(outputFile.tellp() - at);
 }
 
+size_t Encoder::processSearchPairingTo(std::ofstream &outputFile, size_t &searchBytes, size_t &differences)
+{
+    const std::streampos at = outputFile.tellp();
+    encodeTo(outputFile, nullptr, nullptr, &searchBytes, &differences, true);
+    return (size_t)(outputFile.tellp() - at);
+}
+
 // processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
 // selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search, with `differences`
-// as well through selab200_encode_container_pairing.
+// as well through selab200_encode_container_pairing, and with `searchBase` too through
+// selab200_encode_container_search_pairing.
 void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                       size_t *refBytes, size_t *differences)
+                       size_t *refBytes, size_t *differences, bool searchBase)
 {
     if (differences)
         *differences = 0;
@@ -871,6 +879,11 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         for (size_t i = 0; i < n && i < raw.size(); i++)
             recoded->push_back(RecodedEntry{raw[i].frame, raw[i].channel, raw[i].ref_order, raw[i].order,
                                             raw[i].ref_words, raw[i].words});
+    } else if (differences && searchBase) {
+        Phase p("order-search + pairing encode (device)");
+        check(selab200_encode_container_search_pairing(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                       (uint32_t)n_frames, channels, w.fmt.sampleRate,
+                                                       w.fmt.bitsPerSample, out, cap, &used, refBytes, differences));
     } else if (differences) {
         Phase p("pairing encode (device)");
         check(selab200_encode_container_pairing(reinterpret_cast<const int16_t *>(file.data + dat.body),

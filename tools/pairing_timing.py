@@ -1,4 +1,4 @@
-"""What the channel pairing (DESIGN.md 7.4) costs and saves, on three workloads:
+"""What the channel pairing (DESIGN.md 7.4) and the search + pairing (7.5) cost and save, on three workloads:
 
   BASELINE config 2/3     44.1 kHz stereo, 10 minutes, seed 1: 12 919 frames
   config-4-shaped file    48 kHz, 8 channels of independent sine + noise, 10 minutes, seed 2: 14 062 frames
@@ -6,9 +6,9 @@
   correlated 8 channels   one source in every channel with a gain per channel and small independent noise
                           (tests/exact_pairing.common_source), 2 000 frames: cost and gain
 
-For each: device time of DeviceCodec.encode and encode_lossless against DeviceCodec.encode_pairing (CUDA events, runs
-alternated in one process so that drift on a shared card hits all alike), device time per kernel (torch.profiler, a
-pass of its own), and the words each writes.  The card's name and power limit are read in the same call.
+For each: device time of DeviceCodec.encode, encode_lossless, encode_search, encode_pairing and encode_search_pairing
+(CUDA events, runs alternated in one process so that drift on a shared card hits all alike), device time per kernel
+(torch.profiler, a pass of its own), and the words each writes.  The card's name and power limit are read in the same call.
 Usage: python tools/pairing_timing.py [reps] [out.json]   (prints one JSON line; also writes it to out.json if named)"""
 import json
 import os
@@ -86,7 +86,20 @@ def measure(name, pcm, ch):
     out["words_pairing"] = words_pairing
     out["difference_subframes"] = int(codec.n_difference.item())
     out["saving"] = round(1 - words_pairing / words_lossless, 5)
-    forms = (("encode", codec.encode), ("encode_lossless", codec.encode_lossless), ("encode_pairing", codec.encode_pairing))
+    codec.encode_search(t)
+    codec.check_status()
+    words_search = int(codec.words_used.item())
+    codec.encode_search_pairing(t)
+    codec.check_status()
+    words_sp, base_words = int(codec.words_used.item()), int(codec.base_words.item())
+    assert base_words == words_search and words_sp <= words_search
+    out["words_search"] = words_search
+    out["words_search_pairing"] = words_sp
+    out["search_pairing_difference_subframes"] = int(codec.n_difference.item())
+    out["search_pairing_saving_vs_search"] = round(1 - words_sp / words_search, 5)
+    out["search_pairing_saving_vs_default"] = round(1 - words_sp / out["words_default"], 5)
+    forms = (("encode", codec.encode), ("encode_lossless", codec.encode_lossless), ("encode_search", codec.encode_search),
+             ("encode_pairing", codec.encode_pairing), ("encode_search_pairing", codec.encode_search_pairing))
     runs = [[event_ms(lambda: fn(t), REPS) for _, fn in forms] for _ in range(3)]  # alternated
     codec.check_status()
     for i, (name_, fn) in enumerate(forms):
