@@ -413,6 +413,50 @@ int selab200_encode_frames_search_pairing_device(const int16_t *d_pcm, uint32_t 
                                                  uint64_t *d_n_difference, int32_t *d_status, void *d_workspace,
                                                  size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------------ window search -- */
+
+/* The order search with apodised analyses (DESIGN.md 7.6), like the apodisation option of other lossless codecs.
+ * Each analysis unit is coded as selab200_encode_frames_search codes it, unless one of the selected windows does
+ * strictly better: the unit's signal minus its mean, multiplied by the window, is analysed as the reference analyses
+ * the plain signal (autocorrelation, Schur recursion, all 100 quantised coefficients, each clamped to [-64, 63]),
+ * and searched over orders 1..100 as the order search does (the FIR of every order with its tie check, both Rice
+ * sizes; an order whose predictor leaves the domain of the Q35 conversion counts as tied).  The unit takes the
+ * tie-free window candidate with the fewest words if that is strictly fewer than the order search's winner (between
+ * equal words the lower window bit, then the lower order).  The stereo decision then runs as always.  So every frame
+ * takes at most the words of selab200_encode_frames_search, a file no window improves is byte-identical to it, and
+ * every output decodes back to its source under this decoder and the unmodified reference decoder.
+ *
+ * windows: a mask over the rows of the fixed window table (selab200_analysis_window): bit 0 Tukey(0.5), 1 Tukey(0.25),
+ * 2 Hann, 3 Tukey(0.5) over samples 0..1023 and zero after, 4 Tukey(0.5) over samples 1024..2047 and zero before.  A
+ * mask of 0 or with a bit above 4 -> SELAB200_ERR_ARGUMENT.  Each window costs about one more order search.
+ * *base_words receives the words_used of selab200_encode_frames_search for the same frames, *n_window the number of
+ * analysis units (channels; for stereo ch0, ch1 and ch0 - ch1) coded from a window.  Frames are split over devices
+ * as for the other batch calls. */
+int selab200_encode_frames_search_windows(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t windows,
+                                          selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                          size_t *words_used, size_t *base_words, size_t *n_window);
+
+/* selab200_encode_container, with the window search; *base_bytes receives the size of
+ * selab200_encode_container_search's output for the same frames. */
+int selab200_encode_container_search_windows(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                             uint32_t windows, uint32_t sample_rate, uint16_t bits_per_sample,
+                                             uint8_t *container, size_t capacity, size_t *bytes_used,
+                                             size_t *base_bytes, size_t *n_window);
+
+/* Device-resident form of selab200_encode_frames_search_windows: arguments as selab200_encode_frames_device, with
+ * selab200_encode_search_windows_workspace_bytes() of workspace (it grows with the number of windows in the mask);
+ * *d_base_words and *d_n_window (uint64, device) receive the two totals.  Stream-ordered, no synchronisation. */
+size_t selab200_encode_search_windows_workspace_bytes(uint32_t n_frames, uint32_t channels, uint32_t windows);
+int selab200_encode_frames_search_windows_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                 uint32_t windows, selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                 size_t words_capacity, uint64_t *d_words_used, uint64_t *d_base_words,
+                                                 uint64_t *d_n_window, int32_t *d_status, void *d_workspace,
+                                                 size_t workspace_bytes, void *stream);
+
+/* Row `index` (0..4) of the window table into out[2048]: the exact doubles the window search multiplies by.  Needs
+ * no device and no selab200_init.  Another index or a null out -> SELAB200_ERR_ARGUMENT. */
+int selab200_analysis_window(int index, double *out);
+
 /* ------------------------------------------ stage level (host buffers) -- */
 
 /* lpc::ResidueGenerator::process (src/lpc/residue_generator.cpp:121-134) for
@@ -602,6 +646,27 @@ int selab200_encode_search_pairing_trace(const int16_t *pcm, uint32_t n_frames, 
                                          uint32_t *words, size_t words_capacity, size_t *words_used,
                                          size_t *base_words, size_t *n_difference, uint8_t *par,
                                          selab200_search_trace *trace);
+
+/* For tests: selab200_encode_frames_search_windows on one device and one batch, except that every analysis unit and
+ * every (unit, window) record takes its q[0..99] from pred.  pred holds the units first, as
+ * selab200_encode_search_forced takes them (q[0..99] and a reference order 1..100), then n_units * popcount(windows)
+ * records in (unit, window) order, windows in increasing bit order, whose q[0..99] are the window analyses' (their
+ * order, 0..100, is not read).  A value out of range -> SELAB200_ERR_RANGE. */
+int selab200_encode_search_windows_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t windows,
+                                          const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                          uint32_t *words, size_t words_capacity, size_t *words_used,
+                                          size_t *base_words, size_t *n_window);
+
+/* For tests: selab200_encode_frames_search_windows on one device and one batch with the n_windows (1..5) windows
+ * windows[n_windows][2048] in place of the table's (selab200_encode_search_windows_forced's q when pred is not NULL),
+ * through the tracing candidate kernel.  trace[((unit * n_windows) + w) * 100 + order - 1] receives the record of
+ * unit `unit` (selab200_encode_trace's order) coded from window w at every order 1..100; keys[unit] receives the
+ * unit's best window candidate as words << 16 | w << 8 | order (all ones: none). */
+int selab200_encode_search_windows_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                         const double *windows, uint32_t n_windows, const selab200_predictor *pred,
+                                         selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                         size_t *words_used, size_t *base_words, size_t *n_window,
+                                         selab200_search_trace *trace, uint64_t *keys);
 
 #ifdef __cplusplus
 }

@@ -30,6 +30,9 @@ error behaviour as in include/sela_b200.h):
     encode_frames_search_pairing / encode_container_search_pairing
                                     the order search and the channel pairing together (DESIGN.md 7.5), and its
                                     tests-only forms encode_search_pairing_forced / encode_search_pairing_trace
+    encode_frames_search_windows / encode_container_search_windows / analysis_window
+                                    the order search over apodised analyses (DESIGN.md 7.6), its window table, and
+                                    its tests-only forms encode_search_windows_forced / encode_search_windows_trace
     encode_lossless_forced          encode with chosen predictors, and the order search with chosen
     / encode_search_forced          coefficients
 
@@ -628,3 +631,103 @@ def encode_search_pairing_forced(pcm, channels, predictors, device=0):
                                                   descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
                                                   C.addressof(base), C.addressof(nd)))
     return descs, words[:used.value].copy(), base.value, nd.value
+
+
+def analysis_window(index):
+    """Row `index` (0..4) of the window search's table (DESIGN.md 7.6) -> float64 [2048], the exact doubles the
+    encoder multiplies by: 0 Tukey(0.5), 1 Tukey(0.25), 2 Hann, 3 and 4 Tukey(0.5) over the first and the second half
+    of the frame.  Needs no device."""
+    out = np.zeros(FRAME, np.float64)
+    check(lib().selab200_analysis_window(int(index), out.ctypes.data))
+    return out
+
+
+def encode_frames_search_windows(pcm, channels, windows=1, words_capacity=None, device=0):
+    """encode_frames with the window search (DESIGN.md 7.6) -> (descs, words, base_words, n_window).  windows: a mask
+    over analysis_window's rows (1: Tukey(0.5)).  base_words is the number of words encode_frames_search writes for
+    the same frames, n_window the number of analysis units coded from a window."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nw = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_frames_search_windows(pcm.ctypes.data, n_frames, channels, windows, descs.ctypes.data,
+                                                  words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                                  C.addressof(nw)))
+    return descs, words[:used.value].copy(), base.value, nw.value
+
+
+def encode_container_search_windows(pcm, channels, sample_rate, windows=1, bits_per_sample=16, capacity=None,
+                                    device=0):
+    """encode_container with the window search -> (bytes, base_bytes, n_window): base_bytes is the size of
+    encode_container_search's output for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used, base, nw = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_container_search_windows(pcm.ctypes.data, n_frames, channels, windows, sample_rate,
+                                                     bits_per_sample, out.ctypes.data, cap, C.addressof(used),
+                                                     C.addressof(base), C.addressof(nw)))
+    return out[:used.value], base.value, nw.value
+
+
+def _window_predictors(predictors, n_units, n_windows):
+    """(order, q[100]) pairs: the units' as encode_search_forced takes them, then the (unit, window) records'."""
+    pred = np.zeros(len(predictors), PREDICTOR_DTYPE)
+    for rec, (order, q) in zip(pred, predictors):
+        rec["order"] = order
+        rec["q"][:] = np.asarray(q)[:MAX_ORDER]
+    if pred.size != n_units * (1 + n_windows):
+        raise ValueError("%d predictors for %d units and %d windows" % (pred.size, n_units, n_windows))
+    return pred
+
+
+def encode_search_windows_forced(pcm, channels, windows, predictors, device=0):
+    """encode_frames_search_windows on one batch with every unit's q[0..99] and reference order, then every
+    (unit, window) record's q[0..99] (windows in increasing bit order; its order is not read), from `predictors`
+    ((order, q[100]) pairs) -> (descs, words, base_words, n_window)."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    n_units = n_frames * (3 if channels == 2 else channels)
+    pred = _window_predictors(predictors, n_units, bin(windows & 31).count("1"))
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, base, nw = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_windows_forced(pcm.ctypes.data, n_frames, channels, windows, pred.ctypes.data,
+                                                  descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
+                                                  C.addressof(base), C.addressof(nw)))
+    return descs, words[:used.value].copy(), base.value, nw.value
+
+
+def encode_search_windows_trace(pcm, channels, tables, predictors=None, device=0):
+    """The window search on one batch with the windows `tables` (float64 [n, 2048], 1 <= n <= 5) in place of the
+    table's (encode_search_windows_forced's q with `predictors`), through the tracing candidate kernel -> (descs,
+    words, base_words, n_window, trace, keys): trace SEARCH_TRACE_DTYPE [n_units, n, 100], entry [u, w, order - 1]
+    unit u (encode_trace's order) coded from window w at that order; keys uint64 [n_units], unit u's best window
+    candidate as words << 16 | w << 8 | order."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    tables = np.ascontiguousarray(np.atleast_2d(tables), np.float64)
+    n_windows = tables.shape[0]
+    if tables.shape[1] != FRAME:
+        raise ValueError("a window has 2048 values")
+    n_units = n_frames * (3 if channels == 2 else channels)
+    pred = None if predictors is None else _window_predictors(predictors, n_units, n_windows)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    trace = np.zeros((n_units, n_windows, MAX_ORDER), SEARCH_TRACE_DTYPE)
+    keys = np.zeros(n_units, np.uint64)
+    used, base, nw = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_windows_trace(pcm.ctypes.data, n_frames, channels, tables.ctypes.data, n_windows,
+                                                 None if pred is None else pred.ctypes.data, descs.ctypes.data,
+                                                 words.ctypes.data, cap, C.addressof(used), C.addressof(base),
+                                                 C.addressof(nw), trace.ctypes.data, keys.ctypes.data))
+    return descs, words[:used.value].copy(), base.value, nw.value, trace, keys

@@ -5,6 +5,7 @@
 // CUDA device every compute entry point returns SELAB200_ERR_NO_DEVICE.
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -19,6 +20,7 @@
 #include "search.cuh"
 #include "search_pairing.cuh"
 #include "verify.cuh"
+#include "window.cuh"
 
 using namespace selab200;
 
@@ -72,13 +74,14 @@ struct DeviceBuffer {
 };
 
 // The counters of the host-buffer, test and stage calls: at the front of g.small on the device, and in the pinned
-// g.h_small they come down to.  The encode counters (status .. n_difference) are reset and read back as one block.
+// g.h_small they come down to.  The encode counters (status .. n_window) are reset and read back as one block.
 struct Counters {
     int32_t status;                  // the device status of the call
     uint64_t used;                   // encode: the word arena's fill level
     unsigned long long ref_words;    // search: the words the reference encoder's choice takes
     unsigned long long base_words;   // pairing: the words of its base, the lossless encode (search_pairing: the search)
     unsigned long long n_difference; // pairing, search_pairing: the difference subframes chosen
+    unsigned long long n_window;     // search_windows: the units coded from a window
     uint32_t selftest;               // selab200_selftest: the mismatches
     // host side only (collect_records): a count of set records, and the decode status that follows a verify count
     unsigned long long n_records;
@@ -109,6 +112,7 @@ struct Context {
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
     cudaStream_t last_rice_stream = nullptr;
     std::vector<struct ContainerBuffers> *spare = nullptr; // recycled container buffers of this device
+    const double *windows = nullptr;               // d_analysis_windows on `device`, filled by init_slot
 };
 
 // One context per device the library was initialised for (selab200_init / selab200_init_devices), slot 0 the
@@ -492,26 +496,102 @@ int launch_search_pairing(const EncodeParams &p, const PairingParams &q, SearchU
     return launch_check("k_search_pairing_repack");
 }
 
+// The window table of the window search (DESIGN.md 7.6), computed once on the host: row i is the window of mask bit
+// i.  Tukey(p) over n samples: L = floor(p (n - 1) / 2) samples 0.5 (1 - cos(pi i / L)) at each end, 1 between.
+const double *analysis_window_table()
+{
+    static const std::vector<double> table = [] {
+        std::vector<double> t((size_t)kAnalysisWindows * kFrame, 1.0);
+        const auto tukey = [](double *w, int n, double frac) {
+            const int L = (int)std::floor(frac * (n - 1) / 2);
+            for (int i = 0; i < L; i++) {
+                const double v = 0.5 * (1.0 - std::cos(M_PI * i / L));
+                w[i] = v;
+                w[n - 1 - i] = v;
+            }
+        };
+        double *row = t.data();
+        tukey(row, kFrame, 0.5);                                    // 0: Tukey(0.5)
+        tukey(row + kFrame, kFrame, 0.25);                          // 1: Tukey(0.25)
+        for (int i = 0; i < kFrame; i++)                            // 2: Hann
+            row[2 * kFrame + i] = 0.5 - 0.5 * std::cos(2 * M_PI * i / (kFrame - 1));
+        std::fill(row + 3 * kFrame + kFrame / 2, row + 4 * kFrame, 0.0); // 3: Tukey(0.5) over the first half
+        tukey(row + 3 * kFrame, kFrame / 2, 0.5);
+        std::fill(row + 4 * kFrame, row + 4 * kFrame + kFrame / 2, 0.0); // 4: Tukey(0.5) over the second half
+        tukey(row + 4 * kFrame + kFrame / 2, kFrame / 2, 0.5);
+        return t;
+    }();
+    return table.data();
+}
+
+// A window mask names at least one window and none past the table.
+int check_windows(uint32_t windows)
+{
+    if (windows == 0 || (windows >> kAnalysisWindows) != 0)
+        return fail(SELAB200_ERR_ARGUMENT, "window mask 0x%x must select windows among bits 0..%d", windows,
+                    kAnalysisWindows - 1);
+    return 0;
+}
+
+// The window search (window.cuh) after the order search and before the scan: the order search's words added to
+// *d_base_words, the window analyses, their candidates, and the units whose best window candidate has strictly fewer
+// words repacked.  su: the order search's SearchUnits.  The warp kernels have grids of a fixed size, the candidate
+// and repack kernels at most one residue row per unit of the batch.  trace: the candidate kernel is its tracing
+// instantiation (wp.trace).
+template <bool STEREO>
+int launch_windows(const EncodeParams &p, const WindowParams &wp, const SearchUnit *su, size_t n_frames,
+                   size_t n_units, unsigned long long *d_base_words, cudaStream_t stream, bool trace)
+{
+    constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
+    if (int rc = set_smem(k_window_units<STEREO>, smem))
+        return rc;
+    if (int rc = trace ? set_smem(k_window_candidates<STEREO, true>, smem_orders)
+                       : set_smem(k_window_candidates<STEREO, false>, smem_orders))
+        return rc;
+    if (int rc = set_smem(k_window_repack<STEREO>, smem_orders))
+        return rc;
+    k_window_base_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, d_base_words);
+    if (int rc = launch_check("k_window_base_words"))
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(wp.key, 0xff, n_units * sizeof(unsigned long long), stream));
+    const size_t cap = (size_t)g.sms * 32;
+    k_window_units<STEREO><<<(unsigned)std::min(n_units * wp.n, cap), 32, smem, stream>>>(p, wp);
+    if (int rc = launch_check("k_window_units"))
+        return rc;
+    const unsigned warps = (unsigned)std::min(n_units, cap);
+    if (trace)
+        k_window_candidates<STEREO, true><<<warps, 32, smem_orders, stream>>>(p, wp);
+    else
+        k_window_candidates<STEREO, false><<<warps, 32, smem_orders, stream>>>(p, wp);
+    if (int rc = launch_check("k_window_candidates"))
+        return rc;
+    k_window_repack<STEREO><<<warps, 32, smem_orders, stream>>>(p, wp, su);
+    return launch_check("k_window_repack");
+}
+
 // Which encoder an encode call runs.  lossless: re-code every subframe the reference decoder would not reproduce
 // (DESIGN.md 7.2).  search: code every subframe at the predictor order with the fewest words (7.3).  pairing: code
 // channels as differences wherever that takes fewer words, on top of the lossless encode (7.4).  search_pairing: the
-// pairing on top of the search, every channel and every difference at its cheapest order (7.5).
-enum class EncodeMode { plain, lossless, search, pairing, search_pairing };
+// pairing on top of the search, every channel and every difference at its cheapest order (7.5).  search_windows: the
+// search, and every unit also searched from the analysis of each selected window (7.6).
+enum class EncodeMode { plain, lossless, search, pairing, search_pairing, search_windows };
 
 // Where every region of an encode workspace lies, as byte offsets from its base, and its size.  Every mode has the
 // plain encode's regions; lossless and pairing add the repair lists, search the SearchUnits, and pairing the pairing
 // tables behind the repair lists.  search_pairing has the SearchUnits (every region padded), the pairing tables and
-// the candidates' SearchUnits.  The offsets of the regions a mode lacks are 0.
+// the candidates' SearchUnits.  search_windows has the SearchUnits, one per (unit, window) and the units' window keys.
+// The offsets of the regions a mode lacks are 0.
 struct EncodeLayout {
     size_t units, slots, means, residues;                       // EncodeParams
     size_t repair_count, repair_frames, repair_orig, repair_units; // RepairParams
     size_t search;                                              // SearchUnit[n_units]
     size_t pair_search;                                         // search_pairing: SearchUnit[n_frames][C][C]
     size_t pair_table, pair_means, par, stale;                  // PairingParams
+    size_t window_search, window_keys;                          // search_windows: WindowParams::su and ::key
     size_t bytes;                                               // selab200_encode_*_workspace_bytes
 };
 
-EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels)
+EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels, uint32_t n_windows = 0)
 {
     const size_t n_units = encode_units(n_frames, channels), n_sub = (size_t)n_frames * channels;
     const size_t n_pairs = n_sub * channels;
@@ -530,6 +610,11 @@ EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels
         l.search = at;
         l.bytes = at + n_units * sizeof(SearchUnit);
         return l;
+    }
+    if (mode == EncodeMode::search_windows) {
+        l.search = region(n_units * sizeof(SearchUnit));
+        l.window_search = region(n_units * n_windows * sizeof(SearchUnit));
+        l.window_keys = region(n_units * sizeof(unsigned long long));
     }
     if (mode == EncodeMode::lossless || mode == EncodeMode::pairing) {
         l.repair_count = region(256);
@@ -578,14 +663,19 @@ struct EncodeOptions {
     unsigned long long *d_base_words = nullptr; // pairing, search_pairing: += the words of its base, the lossless
                                                 // encode or the search ...
     unsigned long long *d_n_difference = nullptr; // ... and the difference subframes chosen
+    uint32_t windows = 0;                         // search_windows: the window mask ...
+    unsigned long long *d_n_window = nullptr;     // ... += the units coded from a window
     // tests only
     selab200_analysis_trace *d_trace = nullptr;      // plain: the tracing unit kernel writes every unit's analysis here
     const selab200_predictor *d_pred = nullptr;      // lossless, search, pairing, search_pairing: every unit's
                                                      // predictor (pairing, search_pairing: its base's units)
     const selab200_predictor *d_pair_pred = nullptr; // pairing, search_pairing: the candidates' predictors
                                                      // (PairingParams::pred)
-    selab200_search_trace *d_search_trace = nullptr; // search, pairing, search_pairing: the tracing kernels write every
-                                                     // (unit, order) / candidate / (candidate, order) record here
+    selab200_search_trace *d_search_trace = nullptr; // search, pairing, search_pairing, search_windows: the tracing
+                                                     // kernels write every (unit, order) / candidate / (candidate,
+                                                     // order) / (unit, window, order) record here
+    const selab200_predictor *d_window_pred = nullptr; // search_windows: the (unit, window) records' q
+    const double *d_windows = nullptr;               // search_windows: the table the mask indexes (null: the fixed one)
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -594,7 +684,12 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
 {
     if (int rc = check_channels(channels))
         return rc;
-    const EncodeLayout l = encode_layout(o.mode, n_frames, channels);
+    const bool search_windows = o.mode == EncodeMode::search_windows;
+    if (search_windows && !o.d_windows)
+        if (int rc = check_windows(o.windows))
+            return rc;
+    const uint32_t n_windows = search_windows ? (uint32_t)__builtin_popcount(o.windows) : 0;
+    const EncodeLayout l = encode_layout(o.mode, n_frames, channels, n_windows);
     if (ws_bytes < l.bytes)
         return fail(SELAB200_ERR_ARGUMENT, "encode workspace too small");
     if (channels == 2 && (reinterpret_cast<uintptr_t>(d_pcm) & 15) != 0) // the stereo kernel reads 16 bytes (4 sample pairs) at a time
@@ -615,6 +710,10 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         if (pairing) {
             CUDA_TRY(cudaMemsetAsync(o.d_base_words, 0, sizeof(unsigned long long), stream));
             CUDA_TRY(cudaMemsetAsync(o.d_n_difference, 0, sizeof(unsigned long long), stream));
+        }
+        if (search_windows) {
+            CUDA_TRY(cudaMemsetAsync(o.d_base_words, 0, sizeof(unsigned long long), stream));
+            CUDA_TRY(cudaMemsetAsync(o.d_n_window, 0, sizeof(unsigned long long), stream));
         }
     }
     if (n_frames == 0)
@@ -671,11 +770,13 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         if (pairing)
             if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
                 return rc;
-    } else if (o.mode == EncodeMode::search || search_pairing) {
-        // the base of a search + pairing takes no reference words and no trace (its candidates are traced)
+    } else if (o.mode == EncodeMode::search || search_pairing || search_windows) {
+        // the base of a search + pairing or a window search takes no reference words and no trace (its candidates
+        // are traced)
         SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
-        unsigned long long *rw = search_pairing ? nullptr : o.d_ref_words;
-        selab200_search_trace *tr = search_pairing ? nullptr : o.d_search_trace;
+        const bool base = search_pairing || search_windows;
+        unsigned long long *rw = base ? nullptr : o.d_ref_words;
+        selab200_search_trace *tr = base ? nullptr : o.d_search_trace;
         const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr)
                                           : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr))
                                 : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr)
@@ -686,6 +787,21 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
             if (int rc = launch_search_pairing(p, q, reinterpret_cast<SearchUnit *>(ws + l.pair_search), n_frames,
                                                n_units, stream, o.d_search_trace != nullptr))
                 return rc;
+        if (search_windows) {
+            WindowParams wp;
+            wp.table = o.d_windows ? o.d_windows : g.windows;
+            wp.mask = o.windows;
+            wp.n = n_windows;
+            wp.su = reinterpret_cast<SearchUnit *>(ws + l.window_search);
+            wp.key = reinterpret_cast<unsigned long long *>(ws + l.window_keys);
+            wp.n_window = o.d_n_window;
+            wp.pred = o.d_window_pred;
+            wp.trace = o.d_search_trace;
+            const bool trace = o.d_search_trace != nullptr;
+            if (int rc = stereo ? launch_windows<true>(p, wp, su, n_frames, n_units, o.d_base_words, stream, trace)
+                                : launch_windows<false>(p, wp, su, n_frames, n_units, o.d_base_words, stream, trace))
+                return rc;
+        }
     } else {
         const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
                                                  : launch_encode_units<true, false>(p, n_units, nullptr, stream))
@@ -1008,6 +1124,13 @@ static int init_slot(int device, int slot)
     CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_totals), (kMaxChunks + 1) * 8));
     if (int rc = g.small.ensure(256))
         return rc;
+    // The window search's table, copied before any stream of the context can launch a kernel that reads it: a
+    // pageable copy may still be in flight when cudaMemcpyToSymbol returns, and the streams above do not wait for it.
+    CUDA_TRY(cudaMemcpyToSymbol(d_analysis_windows, analysis_window_table(), sizeof(d_analysis_windows)));
+    CUDA_TRY(cudaDeviceSynchronize());
+    void *table = nullptr;
+    CUDA_TRY(cudaGetSymbolAddress(&table, d_analysis_windows));
+    g.windows = static_cast<const double *>(table);
     g.spare = &g_spare_store[slot];
     g.device = device;
     g.sms = prop.multiProcessorCount;
@@ -1062,6 +1185,7 @@ static void shutdown_slot()
     g.events = false;
     g.ready = false;
     g.device = -1;
+    g.windows = nullptr; // the address belongs to this device; a slot set up again may get another
     g.last_rice_n_sub = 0;
     if (g_last_rice_ctx == tl_ctx)
         g_last_rice_ctx = nullptr;
@@ -1183,6 +1307,21 @@ size_t selab200_encode_search_pairing_workspace_bytes(uint32_t n_frames, uint32_
     return encode_layout(EncodeMode::search_pairing, n_frames, channels).bytes;
 }
 
+size_t selab200_encode_search_windows_workspace_bytes(uint32_t n_frames, uint32_t channels, uint32_t windows)
+{
+    return encode_layout(EncodeMode::search_windows, n_frames, channels, (uint32_t)__builtin_popcount(windows)).bytes;
+}
+
+int selab200_analysis_window(int index, double *out)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (index < 0 || index >= kAnalysisWindows || !out)
+        return fail(SELAB200_ERR_ARGUMENT, "window %d is not in the table (0..%d), or out is null", index,
+                    kAnalysisWindows - 1);
+    memcpy(out, analysis_window_table() + (size_t)index * kFrame, kFrame * sizeof(double));
+    return 0;
+}
+
 size_t selab200_decode_workspace_bytes(uint32_t n_frames, uint32_t channels)
 {
     const size_t n_sub = (size_t)n_frames * channels;
@@ -1278,6 +1417,28 @@ int selab200_encode_frames_search_pairing_device(const int16_t *d_pcm, uint32_t 
     o.mode = EncodeMode::search_pairing;
     o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
     o.d_n_difference = reinterpret_cast<unsigned long long *>(d_n_difference);
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
+}
+
+int selab200_encode_frames_search_windows_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                uint32_t windows, selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                size_t words_capacity, uint64_t *d_words_used, uint64_t *d_base_words,
+                                                uint64_t *d_n_window, int32_t *d_status, void *d_workspace,
+                                                size_t workspace_bytes, void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_base_words || !d_n_window || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    if (int rc = check_windows(windows))
+        return rc;
+    EncodeOptions o;
+    o.mode = EncodeMode::search_windows;
+    o.windows = windows;
+    o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
+    o.d_n_window = reinterpret_cast<unsigned long long *>(d_n_window);
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
@@ -1412,6 +1573,7 @@ struct Result {
     unsigned long long ref_words = 0;  // search: the words the reference encoder's choice takes
     unsigned long long base_words = 0; // pairing: the words of its base, the lossless encode (search_pairing: the search)
     unsigned long long n_difference = 0; // pairing, search_pairing: the difference subframes chosen
+    unsigned long long n_window = 0;   // search_windows: the units coded from a window
     size_t ref_bytes = 0;              // container search / pairing / search_pairing: the size of the output it is
                                        // measured against
     std::vector<selab200_lossless_entry> recoded; // lossless: the re-coded (frame, channel) pairs
@@ -1422,6 +1584,7 @@ struct Result {
         ref_words += b.ref_words;
         base_words += b.base_words;
         n_difference += b.n_difference;
+        n_window += b.n_window;
         recoded.insert(recoded.end(), b.recoded.begin(), b.recoded.end());
         report.insert(report.end(), b.report.begin(), b.report.end());
     }
@@ -1437,6 +1600,7 @@ static int read_counters(cudaStream_t stream, Result &r)
     r.ref_words = c.ref_words;
     r.base_words = c.base_words;
     r.n_difference = c.n_difference;
+    r.n_window = c.n_window;
     return c.status ? fail(c.status, "%s", status_text(c.status)) : 0;
 }
 
@@ -1453,7 +1617,7 @@ static int lossless_area(size_t n_sub, LosslessArgs &la)
 // The pipelined encoder over host buffers, running `mode`, into r; frames numbered from frame_base in what it
 // reports.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                       EncodeMode mode, uint32_t frame_base, Result &r)
+                       EncodeMode mode, uint32_t windows, uint32_t frame_base, Result &r)
 {
     const size_t words_capacity = t.words_capacity;
     const bool to_container = t.form == EncodeForm::container;
@@ -1466,7 +1630,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
     const bool verify = t.verify && to_container;
     const bool lossless = mode == EncodeMode::lossless;
-    const size_t ws_bytes = encode_layout(mode, plan.max_frames, channels).bytes;
+    const size_t ws_bytes = encode_layout(mode, plan.max_frames, channels, (uint32_t)__builtin_popcount(windows)).bytes;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(container_frame_byte(n_frames, channels, words_capacity) + 64)) return rc;
@@ -1518,6 +1682,8 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         o.d_ref_words = &d_ctr->ref_words;
         o.d_base_words = &d_ctr->base_words;
         o.d_n_difference = &d_ctr->n_difference;
+        o.windows = windows;
+        o.d_n_window = &d_ctr->n_window;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
                                    d_words, words_capacity, &d_ctr->used, &d_ctr->status, ws.ptr, ws.bytes, cs, o))
             return rc;
@@ -1902,9 +2068,9 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
 }
 
 // Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.  r: the
-// results of all blocks.
+// results of all blocks.  windows: the window search's mask.
 static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                         EncodeMode mode, Result &r)
+                         EncodeMode mode, Result &r, uint32_t windows = 0)
 {
     const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
@@ -1917,7 +2083,7 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
             block.container = nullptr;
             block.words_capacity = selab200_encode_words_bound(p.nf, channels);
         }
-        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, mode, p.f0, p.res);
+        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, mode, windows, p.f0, p.res);
     });
     r = std::move(b.total);
     if (b.rc || !split)
@@ -2024,6 +2190,29 @@ int selab200_encode_frames_search_pairing(const int16_t *pcm, uint32_t n_frames,
     return rc;
 }
 
+int selab200_encode_frames_search_windows(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t windows,
+                                         selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                         size_t *words_used, size_t *base_words, size_t *n_window)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !base_words || !n_window)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    if (int rc = check_windows(windows))
+        return rc;
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::search_windows, r,
+                                 windows);
+    *words_used = r.words;
+    *base_words = (size_t)r.base_words;
+    *n_window = (size_t)r.n_window;
+    return rc;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -2034,7 +2223,7 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 // selab200_encode_container in every mode, and with `verify` its verified form (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
-                                 EncodeMode mode, bool verify, Result &r)
+                                 EncodeMode mode, bool verify, Result &r, uint32_t windows = 0)
 {
     if (int rc = require_ready())
         return rc;
@@ -2054,10 +2243,11 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     memcpy(container, header, sizeof header);
     const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4),
                          verify};
-    const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r);
+    const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r, windows);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, r.words);
     r.ref_bytes = (size_t)container_frame_byte(n_frames, channels,
-                                               mode == EncodeMode::pairing || mode == EncodeMode::search_pairing
+                                               mode == EncodeMode::pairing || mode == EncodeMode::search_pairing ||
+                                                       mode == EncodeMode::search_windows
                                                    ? r.base_words
                                                    : r.ref_words);
     return rc;
@@ -2161,6 +2351,27 @@ int selab200_encode_container_search_pairing(const int16_t *pcm, uint32_t n_fram
                                          bytes_used, EncodeMode::search_pairing, false, r);
     *base_bytes = r.ref_bytes;
     *n_difference = (size_t)r.n_difference;
+    return rc;
+}
+
+int selab200_encode_container_search_windows(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                            uint32_t windows, uint32_t sample_rate, uint16_t bits_per_sample,
+                                            uint8_t *container, size_t capacity, size_t *bytes_used,
+                                            size_t *base_bytes, size_t *n_window)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!base_bytes || !n_window) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    if (int rc = check_windows(windows))
+        return rc;
+    Result r;
+    const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                         bytes_used, EncodeMode::search_windows, false, r, windows);
+    *base_bytes = r.ref_bytes;
+    *n_window = (size_t)r.n_window;
     return rc;
 }
 
@@ -2501,7 +2712,9 @@ static_assert(sizeof(selab200_search_unit) == sizeof(SearchUnit) &&
 struct BatchOutputs {
     size_t *words_used = nullptr;
     size_t *ref_words = nullptr;                           // search
-    size_t *base_words = nullptr, *n_difference = nullptr; // pairing, search_pairing
+    size_t *base_words = nullptr, *n_difference = nullptr; // pairing, search_pairing (base_words: search_windows)
+    size_t *n_window = nullptr;                            // search_windows ...
+    uint64_t *window_keys = nullptr;                       // ... and its units' window keys
     selab200_lossless_entry *entries = nullptr;            // lossless: the re-coded pairs
     size_t entries_capacity = 0, *n_entries = nullptr;
     selab200_analysis_trace *analysis = nullptr;           // plain: the tracing unit kernel's records
@@ -2532,23 +2745,31 @@ static int check_predictors(const selab200_predictor *pred, size_t n, int min_or
 }
 
 // For tests: one unpipelined batch of `mode` through encode_device on g.stream.  pred (lossless: required): every
-// unit's predictor, for the pairing and the search + pairing followed by the candidates' (include/sela_b200.h).
+// unit's predictor, for the pairing and the search + pairing followed by the candidates', for the window search by
+// the (unit, window) records' (include/sela_b200.h).  windows: the window search's mask; with window_table (host,
+// popcount(windows) rows of 2048) the mask selects that table's rows in place of the fixed table's.
 static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                         const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
-                        size_t words_capacity, const BatchOutputs &out)
+                        size_t words_capacity, const BatchOutputs &out, uint32_t windows = 0,
+                        const double *window_table = nullptr)
 {
     if (int rc = require_ready())
         return rc;
     const bool lossless = mode == EncodeMode::lossless, search = mode == EncodeMode::search,
                search_pairing = mode == EncodeMode::search_pairing,
+               search_windows = mode == EncodeMode::search_windows,
                pairing = mode == EncodeMode::pairing || search_pairing;
-    const bool every_q = search || search_pairing; // predictors are q[0..99] and a reference order 1..100
+    const bool every_q = search || search_pairing || search_windows; // q[0..99] and a reference order 1..100
     if (!pcm || !descs || !words || !out.words_used || (mode == EncodeMode::plain && !out.analysis) ||
         (lossless && (!pred || (!out.entries && out.entries_capacity) || !out.n_entries)) ||
-        (search && !out.ref_words) || (pairing && (!out.base_words || !out.n_difference)))
+        (search && !out.ref_words) || (pairing && (!out.base_words || !out.n_difference)) ||
+        (search_windows && (!out.base_words || !out.n_window)))
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     if (int rc = check_channels(channels))
         return rc;
+    if (search_windows && !window_table)
+        if (int rc = check_windows(windows))
+            return rc;
     *out.words_used = 0;
     if (lossless)
         *out.n_entries = 0;
@@ -2556,28 +2777,40 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
         *out.ref_words = 0;
     if (pairing)
         *out.base_words = *out.n_difference = 0;
+    if (search_windows)
+        *out.base_words = *out.n_window = 0;
     if (n_frames == 0)
         return 0;
     const size_t n_sub = (size_t)n_frames * channels, n_units = encode_units(n_frames, channels);
-    const size_t n_pred = pairing ? n_units + n_sub * (channels - 1) : n_units;
-    if (pred)
-        if (int rc = check_predictors(pred, n_pred, every_q ? 1 : 0, !every_q, pairing ? "predictor" : "unit"))
+    const uint32_t n_windows = search_windows ? (uint32_t)__builtin_popcount(windows) : 0;
+    const size_t n_pred = pairing ? n_units + n_sub * (channels - 1) : n_units + n_units * n_windows;
+    if (pred) {
+        const size_t n_first = search_windows ? n_units : n_pred;
+        if (int rc = check_predictors(pred, n_first, every_q ? 1 : 0, !every_q, pairing ? "predictor" : "unit"))
             return rc;
-    const EncodeLayout l = encode_layout(mode, n_frames, channels);
+        if (search_windows) // the window records' order is not read
+            if (int rc = check_predictors(pred + n_units, n_pred - n_units, 0, false, "window record"))
+                return rc;
+    }
+    const EncodeLayout l = encode_layout(mode, n_frames, channels, n_windows);
     const size_t pred_bytes = pred ? align256(n_pred * sizeof(selab200_predictor)) : 0;
-    const size_t n_records = search_pairing ? n_sub * channels * kMaxOrder : pairing ? n_sub * channels
-                                                                                    : n_units * kMaxOrder;
+    const size_t n_records = search_pairing   ? n_sub * channels * kMaxOrder
+                             : pairing        ? n_sub * channels
+                             : search_windows ? n_units * n_windows * kMaxOrder
+                                              : n_units * kMaxOrder;
     const size_t trace_bytes = out.analysis ? n_units * sizeof(selab200_analysis_trace)
                                : out.trace  ? n_records * sizeof(selab200_search_trace)
                                             : 0;
+    const size_t table_bytes = window_table ? (size_t)n_windows * kFrame * sizeof(double) : 0;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
     if (int rc = g.work.ensure(l.bytes)) return rc;
-    if (int rc = g.aux.ensure(pred_bytes + trace_bytes)) return rc;
+    if (int rc = g.aux.ensure(pred_bytes + align256(trace_bytes) + table_bytes)) return rc;
     Counters *d_ctr = device_counters();
     const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
     void *d_trace = static_cast<char *>(g.aux.ptr) + pred_bytes;
+    double *d_table = reinterpret_cast<double *>(static_cast<char *>(g.aux.ptr) + pred_bytes + align256(trace_bytes));
     EncodeOptions o; // fresh: encode_device resets the counters and records
     o.mode = mode;
     if (lossless)
@@ -2585,8 +2818,12 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     o.d_ref_words = &d_ctr->ref_words;
     o.d_base_words = &d_ctr->base_words;
     o.d_n_difference = &d_ctr->n_difference;
+    o.windows = windows;
+    o.d_n_window = &d_ctr->n_window;
     o.d_pred = pred ? d_pred : nullptr;
     o.d_pair_pred = pred && pairing ? d_pred + n_units : nullptr;
+    o.d_window_pred = pred && search_windows ? d_pred + n_units : nullptr;
+    o.d_windows = window_table ? d_table : nullptr;
     o.d_trace = out.analysis ? static_cast<selab200_analysis_trace *>(d_trace) : nullptr;
     o.d_search_trace = out.trace ? static_cast<selab200_search_trace *>(d_trace) : nullptr;
     if (trace_bytes)
@@ -2594,6 +2831,8 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, pcm, n_sub * kFrame * 2, cudaMemcpyHostToDevice, g.stream));
     if (pred)
         CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, pred, n_pred * sizeof(selab200_predictor), cudaMemcpyHostToDevice, g.stream));
+    if (table_bytes)
+        CUDA_TRY(cudaMemcpyAsync(d_table, window_table, table_bytes, cudaMemcpyHostToDevice, g.stream));
     if (int rc = encode_device(static_cast<const int16_t *>(g.in.ptr), n_frames, channels,
                                static_cast<selab200_subframe_desc *>(g.descs.ptr), static_cast<uint32_t *>(g.words.ptr),
                                words_capacity, &d_ctr->used, &d_ctr->status, g.work.ptr, g.work.bytes, g.stream, o))
@@ -2603,6 +2842,9 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
         CUDA_TRY(cudaMemcpyAsync(out.units, ws + l.search, n_units * sizeof(SearchUnit), cudaMemcpyDeviceToHost, g.stream));
     if (out.par)
         CUDA_TRY(cudaMemcpyAsync(out.par, ws + l.par, n_sub, cudaMemcpyDeviceToHost, g.stream));
+    if (out.window_keys)
+        CUDA_TRY(cudaMemcpyAsync(out.window_keys, ws + l.window_keys, n_units * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                                 g.stream));
     if (trace_bytes)
         CUDA_TRY(cudaMemcpyAsync(out.analysis ? static_cast<void *>(out.analysis) : static_cast<void *>(out.trace),
                                  d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
@@ -2615,6 +2857,10 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     if (pairing) {
         *out.base_words = (size_t)r.base_words;
         *out.n_difference = (size_t)r.n_difference;
+    }
+    if (search_windows) {
+        *out.base_words = (size_t)r.base_words;
+        *out.n_window = (size_t)r.n_window;
     }
     if (status)
         return status;
@@ -2758,6 +3004,47 @@ int selab200_encode_search_pairing_trace(const int16_t *pcm, uint32_t n_frames, 
     out.par = par;
     out.trace = trace;
     return encode_batch(EncodeMode::search_pairing, pcm, n_frames, channels, pred, descs, words, words_capacity, out);
+}
+
+// For tests: one unpipelined window-search batch through encode_device.  pred: the units' q[0..99] and reference
+// orders, then the q of every (unit, window) record.
+int selab200_encode_search_windows_forced(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t windows,
+                                          const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                          uint32_t *words, size_t words_capacity, size_t *words_used,
+                                          size_t *base_words, size_t *n_window)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!pred)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_window = n_window;
+    return encode_batch(EncodeMode::search_windows, pcm, n_frames, channels, pred, descs, words, words_capacity, out,
+                        windows);
+}
+
+// For tests: the window search with the given window rows (or, with pred, selab200_encode_search_windows_forced's)
+// through the tracing candidate kernel, with every (unit, window, order) record and every unit's window key.
+int selab200_encode_search_windows_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                         const double *windows, uint32_t n_windows, const selab200_predictor *pred,
+                                         selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                         size_t *words_used, size_t *base_words, size_t *n_window,
+                                         selab200_search_trace *trace, uint64_t *keys)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!windows || !trace || !keys)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (n_windows < 1 || n_windows > (uint32_t)kAnalysisWindows)
+        return fail(SELAB200_ERR_ARGUMENT, "%u windows: must be 1..%d", n_windows, kAnalysisWindows);
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.base_words = base_words;
+    out.n_window = n_window;
+    out.trace = trace;
+    out.window_keys = keys;
+    return encode_batch(EncodeMode::search_windows, pcm, n_frames, channels, pred, descs, words, words_capacity, out,
+                        (1u << n_windows) - 1, windows);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

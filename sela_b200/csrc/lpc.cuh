@@ -85,9 +85,12 @@ struct MeanChain {
 //    `ac[i] += d[j]*d[j-i]` with the multiply rounded before the add;
 //  - j < i terms are fed as d[negative] = +0.0: acc + (+-0) leaves a +0.0
 //    accumulator unchanged, so starting the chain at j = 0 instead of j = i is
-//    bit-identical.
-template <typename Sig>
-__device__ void warp_autocorrelation(const Sig &sig, LpcSmem &sm, const double mean)
+//    bit-identical;
+//  - WINDOW (the window search, DESIGN.md 7.6): d[j] = (x[j] - mean) * win[j], one more
+//    rounded multiply per staged value.  The 32 lanes read 32 different j, so win is read
+//    through L1 (a __constant__ table would serialise them).
+template <typename Sig, bool WINDOW = false>
+__device__ void warp_autocorrelation(const Sig &sig, LpcSmem &sm, const double mean, const double *win = nullptr)
 {
     const int lane = lane_id();
 
@@ -116,7 +119,10 @@ __device__ void warp_autocorrelation(const Sig &sig, LpcSmem &sm, const double m
 #pragma unroll
         for (int r = 0; r < 4; r++) {
             int j = tile * 128 + r * 32 + lane;
-            sm.ring[ring_index(j)] = dsub(sample_to_x(sig.at(j)), mean);
+            if constexpr (WINDOW)
+                sm.ring[ring_index(j)] = dmul(dsub(sample_to_x(sig.at(j)), mean), __ldg(win + j));
+            else
+                sm.ring[ring_index(j)] = dsub(sample_to_x(sig.at(j)), mean);
         }
         __syncwarp();
         for (int blk = 0; blk < 4; blk++) {

@@ -71,10 +71,15 @@ __device__ __forceinline__ void step_up(double *t, int i, int q)
 // PAIR (search + pairing, search_pairing.cuh; STEREO = true for its shared memory layout): `unit` is the candidate
 // (frame, par, c) at ((frame * C + par) * C + c) of su and trace, its signal ch_par - ch_c from stage_pair, its FIR
 // always the wide one, and PACK packs into unit `out`.  Without PAIR, PACK packs into `unit` and `out` is unused.
-template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false>
+// WINDOW (window search, window.cuh): `unit` is the record (analysis unit u, window w) at u * n_win + w of su and
+// trace, its signal unit u's; a tie-free order enters wkey[u] as words << 16 | w << 8 | order, and PACK packs into u.
+// An order whose predictor leaves the domain of the int64 conversion (|2^35 t| >= 2^62, undefined in the reference;
+// a window's clamped q can get there) counts as tied: it is never eligible.
+template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false, bool WINDOW = false>
 __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
                                               int o_hi, int32_t *res, selab200_search_trace *trace = nullptr,
-                                              uint32_t out = 0)
+                                              uint32_t out = 0, uint32_t n_win = 1,
+                                              unsigned long long *wkey = nullptr)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
@@ -83,16 +88,18 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     uint32_t *planes = reinterpret_cast<uint32_t *>(smem_raw + kSigBytes + kSearchStepBytes + sizeof(CoefSmem));
     static_assert(kSearchStepBytes % 16 == 0 && sizeof(CoefSmem) % 16 == 0, "search shared memory layout");
     static_assert(!PAIR || STEREO, "a pair is staged as the stereo difference is");
+    static_assert(!(PAIR && WINDOW), "one kind of record");
 
     const int lane = lane_id();
-    const bool wide = PAIR || (STEREO && unit % 3 == 2);
-    const uint32_t dst = PAIR ? out : unit;
+    const uint32_t src = WINDOW ? unit / n_win : unit; // the analysis unit whose signal is coded
+    const bool wide = PAIR || (STEREO && src % 3 == 2);
+    const uint32_t dst = PAIR ? out : src;
     Signal sig;
     if constexpr (PAIR)
         sig = stage_pair(p, unit / (p.channels * p.channels), unit / p.channels % p.channels, unit % p.channels,
                          smem_raw);
     else
-        sig = stage_unit<STEREO>(p, unit, smem_raw);
+        sig = stage_unit<STEREO>(p, src, smem_raw);
     SearchUnit &s = su[unit];
     const int ref = (int)s.ref_order;
     for (int i = lane; i < 104; i += 32)
@@ -107,26 +114,37 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     for (int o = o_lo; o <= o_hi; o++) {
         if (!PACK && o == ref)
             continue;
+        bool outside = false; // WINDOW: the predictor leaves the conversion's domain
         if (o >= 2) {
             for (; done < o; done++)
                 step_up(t, done, cf.q[done]);
             for (int m = lane; m < o; m += 32) {
+                if constexpr (WINDOW)
+                    outside |= !(fabs(dmul(scale, -t[m])) < 4611686018427387904.0); // 2^62
                 const long long v = __double2ll_rz(dmul(scale, -t[m]));
                 cf.clo[m] = (uint32_t)v;
                 cf.chi[m] = (int32_t)(v >> 32);
             }
             __syncwarp();
+            if constexpr (WINDOW)
+                outside = __any_sync(kFull, outside);
         }
-        const bool tie = wide ? warp_fir_residual<true, !PACK>(sig, cf, o, planes, res)
-                              : warp_fir_residual<false, !PACK>(sig, cf, o, planes, res);
+        const bool tie = (wide ? warp_fir_residual<true, !PACK>(sig, cf, o, planes, res)
+                               : warp_fir_residual<false, !PACK>(sig, cf, o, planes, res)) ||
+                         outside;
         const RiceChoice cq = warp_rice_choose(cf.q, o);
         const RiceChoice cr = warp_rice_choose(res, kFrame);
         if constexpr (!PACK) {
             if constexpr (TRACE)
                 search_trace_record(trace, unit, o, cf, res, tie, cq, cr);
             const unsigned long long words = cq.words + cr.words;
-            if (lane == 0 && !tie)
-                atomicMin(&s.best, words << 8 | (unsigned long long)o);
+            if constexpr (WINDOW) {
+                if (lane == 0 && !tie)
+                    atomicMin(&wkey[src], words << 16 | (unsigned long long)(unit % n_win) << 8 | (unsigned long long)o);
+            } else {
+                if (lane == 0 && !tie)
+                    atomicMin(&s.best, words << 8 | (unsigned long long)o);
+            }
         } else {
             const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
             if (!too_large) {

@@ -119,6 +119,27 @@ class DeviceCodec:
             self.status.data_ptr(), self.search_pairing_ws.data_ptr(), self.search_pairing_ws_bytes,
             C.c_void_p(stream)))
 
+    def encode_search_windows(self, pcm, windows=1):
+        """encode with the window search (DESIGN.md 7.6) over the window mask `windows`.  Asynchronous;
+        self.base_words and self.n_window (int64 cuda tensors) receive the words encode_search() writes for the same
+        frames and the number of analysis units coded from a window.  The workspace of the largest mask used so far
+        is allocated on first use."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.numel() == self.n_sub * FRAME
+        L = lib()
+        need = L.selab200_encode_search_windows_workspace_bytes(self.n_frames, self.channels, windows)
+        if getattr(self, "windows_ws_bytes", 0) < need:
+            self.windows_ws_bytes = need
+            self.windows_ws = torch.zeros(need, dtype=torch.uint8, device=self.device)
+        if not hasattr(self, "base_words"):
+            self.base_words = torch.zeros(1, dtype=torch.int64, device=self.device)
+        if not hasattr(self, "n_window"):
+            self.n_window = torch.zeros(1, dtype=torch.int64, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_encode_frames_search_windows_device(
+            pcm.data_ptr(), self.n_frames, self.channels, windows, self.descs.data_ptr(), self.words.data_ptr(),
+            self.capacity, self.words_used.data_ptr(), self.base_words.data_ptr(), self.n_window.data_ptr(),
+            self.status.data_ptr(), self.windows_ws.data_ptr(), self.windows_ws_bytes, C.c_void_p(stream)))
+
     def decode(self, pcm_out, n_words):
         """Decode self.descs / self.words[:n_words] into pcm_out (int16 cuda tensor). Asynchronous."""
         assert pcm_out.dtype == torch.int16 and pcm_out.is_cuda and pcm_out.numel() == self.n_sub * FRAME

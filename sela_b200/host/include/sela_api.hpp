@@ -123,7 +123,8 @@ class Encoder {
     void readFrames();
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
     void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                  size_t *refBytes = nullptr, size_t *differences = nullptr, bool searchBase = false);
+                  size_t *refBytes = nullptr, size_t *differences = nullptr, bool searchBase = false,
+                  uint32_t windows = 0);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -157,6 +158,13 @@ public:
     // (selab200_encode_container_search_pairing).  Returns the bytes written; `searchBytes` receives the bytes
     // processSearchTo() writes for the same input, `differences` the number of difference subframes.
     size_t processSearchPairingTo(std::ofstream &outputFile, size_t &searchBytes, size_t &differences);
+    // Not in the reference: processSearchTo(), and every subframe also searched from the analysis of each window in
+    // the mask `windows` (bit 0 Tukey(0.5), 1 Tukey(0.25), 2 Hann, 3 and 4 Tukey(0.5) over each half frame), coded
+    // from whichever analysis and order takes the fewest words (selab200_encode_container_search_windows).  Returns
+    // the bytes written; `searchBytes` receives the bytes processSearchTo() writes for the same input, `windowUnits`
+    // the number of analysis units coded from a window.
+    size_t processSearchWindowsTo(std::ofstream &outputFile, uint32_t windows, size_t &searchBytes,
+                                  size_t &windowUnits);
 };
 class Decoder {
     void readFrames();

@@ -17,6 +17,9 @@
 // `-B in.wav out.sela` ("best"): -S and -P together, every channel and every channel difference at the order with the
 // fewest words; the smallest file of these modes at the highest encode cost, decoding back to the WAV under the
 // reference decoder.  One line with the bytes written, the bytes -S writes and the number of difference subframes.
+// `-W in.wav out.sela`: -S, and every subframe also searched from a Tukey(0.5)-windowed analysis, coded from whichever
+// analysis and order takes the fewest words; a file at most -S's size, decoding back to the WAV under the reference
+// decoder.  One line with the bytes written, the bytes -S writes and the number of units coded from the window.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -114,6 +117,8 @@ int usage(const std::string &prog)
               << " -P path/to/input.wav path/to/output.sela\n\n"
               << "Encoding a file smallest, searching the predictor orders and pairing the channels (H100 build):\n"
               << prog << " -B path/to/input.wav path/to/output.sela\n\n"
+              << "Encoding a file smaller, searching the predictor orders over windowed analyses (H100 build):\n"
+              << prog << " -W path/to/input.wav path/to/output.sela\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -203,6 +208,14 @@ int main(int argc, char **argv)
             const size_t written = sela::Encoder(in).processSearchPairingTo(out, searchBytes, differences);
             std::cout << "Wrote " << written << " bytes (-S: " << searchBytes << " bytes), " << differences
                       << " difference subframes" << std::endl;
+        } else if (mode == "-W" && argc == 4) {
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Encoding with the order search over Tukey(0.5)-windowed analyses: " << argv[2] << std::endl;
+            size_t searchBytes = 0, windowUnits = 0;
+            const size_t written = sela::Encoder(in).processSearchWindowsTo(out, 1u, searchBytes, windowUnits);
+            std::cout << "Wrote " << written << " bytes (-S: " << searchBytes << " bytes), " << windowUnits
+                      << " units coded from the window" << std::endl;
         } else if (mode == "-t" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ifstream wav(argv[3], std::ios::binary);

@@ -817,12 +817,21 @@ size_t Encoder::processSearchPairingTo(std::ofstream &outputFile, size_t &search
     return (size_t)(outputFile.tellp() - at);
 }
 
+size_t Encoder::processSearchWindowsTo(std::ofstream &outputFile, uint32_t windows, size_t &searchBytes,
+                                       size_t &windowUnits)
+{
+    const std::streampos at = outputFile.tellp();
+    encodeTo(outputFile, nullptr, nullptr, &searchBytes, &windowUnits, false, windows);
+    return (size_t)(outputFile.tellp() - at);
+}
+
 // processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
 // selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search, with `differences`
 // as well through selab200_encode_container_pairing, and with `searchBase` too through
-// selab200_encode_container_search_pairing.
+// selab200_encode_container_search_pairing.  With `windows` (and refBytes, differences) through
+// selab200_encode_container_search_windows, `differences` receiving the units coded from a window.
 void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                       size_t *refBytes, size_t *differences, bool searchBase)
+                       size_t *refBytes, size_t *differences, bool searchBase, uint32_t windows)
 {
     if (differences)
         *differences = 0;
@@ -879,6 +888,11 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         for (size_t i = 0; i < n && i < raw.size(); i++)
             recoded->push_back(RecodedEntry{raw[i].frame, raw[i].channel, raw[i].ref_order, raw[i].order,
                                             raw[i].ref_words, raw[i].words});
+    } else if (windows) {
+        Phase p("window-search encode (device)");
+        check(selab200_encode_container_search_windows(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                       (uint32_t)n_frames, channels, windows, w.fmt.sampleRate,
+                                                       w.fmt.bitsPerSample, out, cap, &used, refBytes, differences));
     } else if (differences && searchBase) {
         Phase p("order-search + pairing encode (device)");
         check(selab200_encode_container_search_pairing(reinterpret_cast<const int16_t *>(file.data + dat.body),
