@@ -347,6 +347,39 @@ int selab200_encode_frames_search_device(const int16_t *d_pcm, uint32_t n_frames
                                          uint64_t *d_words_used, uint64_t *d_ref_words, int32_t *d_status,
                                          void *d_workspace, size_t workspace_bytes, void *stream);
 
+/* ----------------------------------------------- guided order search -- */
+
+/* Most of the order search's saving at a fraction of its cost (DESIGN.md 7.7), like the middle presets of other
+ * lossless codecs.  Each analysis unit is searched as selab200_encode_frames_search searches it, but only over the
+ * `candidates` (K, 1..100) orders an estimate ranks best, order 1 and the reference encoder's order.  The estimate of
+ * order o is E_o = P_o * r^o, with P_1 = 1 and P_o = prod_{i<o} (1 - k_i^2) over the dequantised reflection
+ * coefficients k_i, and r = 2^(1/256) (4 bits per coefficient over a 2048-sample frame); orders rank by (E_o, o),
+ * lower first.  The winner and tie rules are the order search's, so every unit takes at least the order search's
+ * words, and at most the reference encoder's where its order has no tie; every output decodes back to its source
+ * under this decoder and the unmodified reference decoder; K = 100 is byte-identical to the order search.  A
+ * candidate count of 0 or above 100 -> SELAB200_ERR_ARGUMENT.  *ref_words as selab200_encode_frames_search's.  Frames
+ * are split over devices as for the other batch calls. */
+int selab200_encode_frames_search_guided(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t candidates,
+                                         selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                         size_t *words_used, size_t *ref_words);
+
+/* selab200_encode_container, with the guided order search; *ref_bytes receives the size of
+ * selab200_encode_container's output for the same frames. */
+int selab200_encode_container_search_guided(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                            uint32_t candidates, uint32_t sample_rate, uint16_t bits_per_sample,
+                                            uint8_t *container, size_t capacity, size_t *bytes_used,
+                                            size_t *ref_bytes);
+
+/* Device-resident form of selab200_encode_frames_search_guided: arguments as selab200_encode_frames_device, with
+ * selab200_encode_search_guided_workspace_bytes() of workspace; *d_ref_words (uint64, device) receives the reference
+ * encoder's words.  Stream-ordered, no synchronisation. */
+size_t selab200_encode_search_guided_workspace_bytes(uint32_t n_frames, uint32_t channels);
+int selab200_encode_frames_search_guided_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                uint32_t candidates, selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                size_t words_capacity, uint64_t *d_words_used, uint64_t *d_ref_words,
+                                                int32_t *d_status, void *d_workspace, size_t workspace_bytes,
+                                                void *stream);
+
 /* ---------------------------------------------------- channel pairing -- */
 
 /* Smaller files of correlated channels at a higher encode cost (DESIGN.md 7.4).  The format can code any channel of
@@ -667,6 +700,17 @@ int selab200_encode_search_windows_trace(const int16_t *pcm, uint32_t n_frames, 
                                          selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
                                          size_t *words_used, size_t *base_words, size_t *n_window,
                                          selab200_search_trace *trace, uint64_t *keys);
+
+/* For tests: selab200_encode_frames_search_guided on one device and one batch (with pred, every unit's q[0..99] and
+ * reference order from it, as selab200_encode_search_forced takes them), through the tracing instantiations of the
+ * search kernels.  trace[unit * 100 + order - 1] receives the record of every order sized (the reference order's
+ * from the analysis kernel, every other listed order's from the listed-order kernel); the records of unlisted orders
+ * keep visits 0.  estimates[unit * 100 + order - 1] receives E_order, masks[unit * 4 + (order - 1) / 32] bit
+ * (order - 1) % 32 whether the order is listed. */
+int selab200_encode_search_guided_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t candidates,
+                                        const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                        uint32_t *words, size_t words_capacity, size_t *words_used, size_t *ref_words,
+                                        selab200_search_trace *trace, double *estimates, uint32_t *masks);
 
 #ifdef __cplusplus
 }

@@ -9,5 +9,6 @@ from .codec import (DESC_DTYPE, FRAME, LOSSLESS_DTYPE, VERIFY_DTYPE, SelaB200Err
                     encode_container_search, encode_container_verified, encode_frames, encode_frames_lossless,
                     encode_frames_search, encode_container_pairing, encode_frames_pairing,
                     encode_container_search_pairing, encode_frames_search_pairing,
-                    encode_container_search_windows, encode_frames_search_windows, analysis_window, init,
+                    encode_container_search_windows, encode_frames_search_windows, analysis_window,
+                    encode_container_search_guided, encode_frames_search_guided, init,
                     lpc_residues, lpc_samples, rice_decode, rice_encode, verify_container, verify_frames)

@@ -134,6 +134,10 @@ _SIGNATURES = {
     "selab200_encode_frames_search_windows": (_I, [_V, _U32, _U32, _U32, _V, _V, _SZ, _V, _V, _V]),
     "selab200_encode_container_search_windows": (_I, [_V, _U32, _U32, _U32, _U32, C.c_uint16, _V, _SZ, _V, _V, _V]),
     "selab200_analysis_window": (_I, [_I, _V]),
+    "selab200_encode_search_guided_workspace_bytes": (_SZ, [_U32, _U32]),
+    "selab200_encode_frames_search_guided_device": (_I, [_V, _U32, _U32, _U32, _V, _V, _SZ, _V, _V, _V, _V, _SZ, _V]),
+    "selab200_encode_frames_search_guided": (_I, [_V, _U32, _U32, _U32, _V, _V, _SZ, _V, _V]),
+    "selab200_encode_container_search_guided": (_I, [_V, _U32, _U32, _U32, _U32, C.c_uint16, _V, _SZ, _V, _V]),
     "selab200_lpc_residues": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_lpc_samples": (_I, [_V, _U32, _V, _V, _V]),
     "selab200_rice_encode": (_I, [_V, _V, _U32, _U32, _V, _V, _V, _U32]),
@@ -151,6 +155,7 @@ _SIGNATURES = {
     "selab200_encode_search_pairing_trace": (_I, [_V, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _V, _V, _V]),
     "selab200_encode_search_windows_forced": (_I, [_V, _U32, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _V]),
     "selab200_encode_search_windows_trace": (_I, [_V, _U32, _U32, _V, _U32, _V, _V, _V, _SZ, _V, _V, _V, _V, _V]),
+    "selab200_encode_search_guided_trace": (_I, [_V, _U32, _U32, _U32, _V, _V, _V, _SZ, _V, _V, _V, _V, _V]),
 }
 
 

@@ -33,6 +33,9 @@ error behaviour as in include/sela_b200.h):
     encode_frames_search_windows / encode_container_search_windows / analysis_window
                                     the order search over apodised analyses (DESIGN.md 7.6), its window table, and
                                     its tests-only forms encode_search_windows_forced / encode_search_windows_trace
+    encode_frames_search_guided / encode_container_search_guided
+                                    the order search over the orders an estimate ranks best (DESIGN.md 7.7), and its
+                                    tests-only form encode_search_guided_trace
     encode_lossless_forced          encode with chosen predictors, and the order search with chosen
     / encode_search_forced          coefficients
 
@@ -468,6 +471,66 @@ def encode_search_trace(pcm, channels, predictors=None, device=0):
                                          descs.ctypes.data, words.ctypes.data, cap, C.addressof(used),
                                          C.addressof(ref), units.ctypes.data, trace.ctypes.data))
     return descs, words[:used.value].copy(), ref.value, units, trace
+
+
+def encode_frames_search_guided(pcm, channels, candidates=4, words_capacity=None, device=0):
+    """encode_frames with the guided order search (DESIGN.md 7.7) -> (descs, words, ref_words): the order search over
+    the `candidates` (1..100) orders a reflection-coefficient estimate ranks best, order 1 and the reference order.
+    ref_words is the number of words encode_frames writes for the same frames; candidates=100 gives
+    encode_frames_search's output."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = words_capacity if words_capacity is not None else L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_frames_search_guided(pcm.ctypes.data, n_frames, channels, candidates, descs.ctypes.data,
+                                                 words.ctypes.data, cap, C.addressof(used), C.addressof(ref)))
+    return descs, words[:used.value].copy(), ref.value
+
+
+def encode_container_search_guided(pcm, channels, sample_rate, candidates=4, bits_per_sample=16, capacity=None,
+                                   device=0):
+    """encode_container with the guided order search -> (bytes, ref_bytes): ref_bytes is the size of
+    encode_container's output for the same frames."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    L = lib()
+    cap = capacity if capacity is not None else L.selab200_container_bound(n_frames, channels)
+    out = np.empty(max(cap, 1), np.uint8)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_container_search_guided(pcm.ctypes.data, n_frames, channels, candidates, sample_rate,
+                                                    bits_per_sample, out.ctypes.data, cap, C.addressof(used),
+                                                    C.addressof(ref)))
+    return out[:used.value], ref.value
+
+
+def encode_search_guided_trace(pcm, channels, candidates, predictors=None, device=0):
+    """encode_frames_search_guided (with `predictors`, every unit's q[100] and reference order as encode_search_forced
+    takes them) on one batch through the tracing kernels -> (descs, words, ref_words, trace, estimates, masks).
+
+    trace: SEARCH_TRACE_DTYPE[n_units, 100], the record of every order sized (column order - 1; visits 0 where the
+    order was not sized); estimates: float64 [n_units, 100], E_order at order - 1; masks: bool [n_units, 100], the
+    listed orders.  Units in encode_trace's order."""
+    init(device)
+    pcm, n_frames = _whole_frames(pcm, channels)
+    n_units = n_frames * (3 if channels == 2 else channels)
+    pred = None if predictors is None else _search_predictors(predictors, n_units)
+    L = lib()
+    cap = L.selab200_encode_words_bound(n_frames, channels)
+    descs = np.zeros(n_frames * channels, DESC_DTYPE)
+    words = np.empty(max(cap, 1), np.uint32)
+    trace = np.zeros((n_units, MAX_ORDER), SEARCH_TRACE_DTYPE)
+    est = np.zeros((n_units, MAX_ORDER), np.float64)
+    masks = np.zeros((n_units, 4), np.uint32)
+    used, ref = C.c_size_t(0), C.c_size_t(0)
+    check(L.selab200_encode_search_guided_trace(pcm.ctypes.data, n_frames, channels, candidates,
+                                                None if pred is None else pred.ctypes.data, descs.ctypes.data,
+                                                words.ctypes.data, cap, C.addressof(used), C.addressof(ref),
+                                                trace.ctypes.data, est.ctypes.data, masks.ctypes.data))
+    listed = ((masks[:, np.arange(MAX_ORDER) // 32] >> (np.arange(MAX_ORDER) % 32).astype(np.uint32)) & 1).astype(bool)
+    return descs, words[:used.value].copy(), ref.value, trace, est, listed
 
 
 def encode_frames_pairing(pcm, channels, words_capacity=None, device=0):

@@ -18,6 +18,7 @@
 #include "lossless.cuh"
 #include "pairing.cuh"
 #include "search.cuh"
+#include "search_guided.cuh"
 #include "search_pairing.cuh"
 #include "verify.cuh"
 #include "window.cuh"
@@ -383,16 +384,40 @@ int launch_lossless(const EncodeParams &p, const RepairParams &r, size_t n_frame
     return launch_check("k_lossless_report");
 }
 
+// The guided order search's candidates (search_guided.cuh): the estimate and every unit's listed orders sized.  trace:
+// the tracing instantiations (gp.estimates is set).
+template <bool STEREO>
+int launch_guided(const EncodeParams &p, SearchUnit *su, const GuidedParams &gp, unsigned warps, cudaStream_t stream,
+                  selab200_search_trace *trace)
+{
+    constexpr size_t smem_orders = search_smem_bytes<STEREO>();
+    if (int rc = trace ? set_smem(k_search_listed<STEREO, true>, smem_orders)
+                       : set_smem(k_search_listed<STEREO, false>, smem_orders))
+        return rc;
+    if (trace)
+        k_search_estimate<true><<<warps, 32, 0, stream>>>(p, su, gp);
+    else
+        k_search_estimate<false><<<warps, 32, 0, stream>>>(p, su, gp);
+    if (int rc = launch_check("k_search_estimate"))
+        return rc;
+    if (trace)
+        k_search_listed<STEREO, true><<<warps, 32, smem_orders, stream>>>(p, su, gp, trace);
+    else
+        k_search_listed<STEREO, false><<<warps, 32, smem_orders, stream>>>(p, su, gp, nullptr);
+    return launch_check("k_search_listed");
+}
+
 // The order search (search.cuh) in place of k_encode_units: analysis, candidates, repack, and the reference encoder's
 // words added to *d_ref_words.  The warp kernels have grids of a fixed size, at most one residue row per unit of the
 // batch.  d_ref_words null (the base of a search + pairing): k_search_ref_words is not run.  FORCE: the units' q and
 // reference orders are d_pred's (selab200_encode_search_forced).  d_trace: the
 // analysis and candidate kernels are their tracing instantiations, which write every (unit, order) record there
-// (selab200_encode_search_trace).
+// (selab200_encode_search_trace).  gp (guided order search, DESIGN.md 7.7): k_search_estimate and k_search_listed
+// in place of k_search_candidates, their tracing instantiations with d_trace.
 template <bool STEREO, bool FORCE = false>
 int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t n_units,
                   unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred = nullptr,
-                  selab200_search_trace *d_trace = nullptr)
+                  selab200_search_trace *d_trace = nullptr, const GuidedParams *gp = nullptr)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
     if (int rc = set_smem(k_search_units<STEREO, FORCE>, smem))
@@ -413,12 +438,17 @@ int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t
     if (int rc = launch_check("k_search_units"))
         return rc;
     const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
-    if (d_trace)
-        k_search_candidates_trace<STEREO><<<warps, 32, smem_orders, stream>>>(p, su, d_trace);
-    else
-        k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
-    if (int rc = launch_check("k_search_candidates"))
-        return rc;
+    if (gp) {
+        if (int rc = launch_guided<STEREO>(p, su, *gp, warps, stream, d_trace))
+            return rc;
+    } else {
+        if (d_trace)
+            k_search_candidates_trace<STEREO><<<warps, 32, smem_orders, stream>>>(p, su, d_trace);
+        else
+            k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
+        if (int rc = launch_check("k_search_candidates"))
+            return rc;
+    }
     if (d_ref_words) {
         k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
         if (int rc = launch_check("k_search_ref_words"))
@@ -573,14 +603,24 @@ int launch_windows(const EncodeParams &p, const WindowParams &wp, const SearchUn
 // (DESIGN.md 7.2).  search: code every subframe at the predictor order with the fewest words (7.3).  pairing: code
 // channels as differences wherever that takes fewer words, on top of the lossless encode (7.4).  search_pairing: the
 // pairing on top of the search, every channel and every difference at its cheapest order (7.5).  search_windows: the
-// search, and every unit also searched from the analysis of each selected window (7.6).
-enum class EncodeMode { plain, lossless, search, pairing, search_pairing, search_windows };
+// search, and every unit also searched from the analysis of each selected window (7.6).  search_guided: the search
+// over the orders an estimate ranks best, order 1 and the reference order (7.7).
+enum class EncodeMode { plain, lossless, search, pairing, search_pairing, search_windows, search_guided };
+
+// The guided order search's candidate count names 1..100 orders.
+int check_candidates(uint32_t candidates)
+{
+    if (candidates == 0 || candidates > (uint32_t)kMaxOrder)
+        return fail(SELAB200_ERR_ARGUMENT, "%u candidates: must be 1..%d", candidates, kMaxOrder);
+    return 0;
+}
 
 // Where every region of an encode workspace lies, as byte offsets from its base, and its size.  Every mode has the
 // plain encode's regions; lossless and pairing add the repair lists, search the SearchUnits, and pairing the pairing
 // tables behind the repair lists.  search_pairing has the SearchUnits (every region padded), the pairing tables and
 // the candidates' SearchUnits.  search_windows has the SearchUnits, one per (unit, window) and the units' window keys.
-// The offsets of the regions a mode lacks are 0.
+// search_guided has the SearchUnits (padded) and a 16-byte order mask per unit.  The offsets of the regions a mode
+// lacks are 0.
 struct EncodeLayout {
     size_t units, slots, means, residues;                       // EncodeParams
     size_t repair_count, repair_frames, repair_orig, repair_units; // RepairParams
@@ -588,6 +628,7 @@ struct EncodeLayout {
     size_t pair_search;                                         // search_pairing: SearchUnit[n_frames][C][C]
     size_t pair_table, pair_means, par, stale;                  // PairingParams
     size_t window_search, window_keys;                          // search_windows: WindowParams::su and ::key
+    size_t masks;                                               // search_guided: GuidedParams::masks
     size_t bytes;                                               // selab200_encode_*_workspace_bytes
 };
 
@@ -615,6 +656,10 @@ EncodeLayout encode_layout(EncodeMode mode, uint32_t n_frames, uint32_t channels
         l.search = region(n_units * sizeof(SearchUnit));
         l.window_search = region(n_units * n_windows * sizeof(SearchUnit));
         l.window_keys = region(n_units * sizeof(unsigned long long));
+    }
+    if (mode == EncodeMode::search_guided) {
+        l.search = region(n_units * sizeof(SearchUnit));
+        l.masks = region(n_units * sizeof(uint4));
     }
     if (mode == EncodeMode::lossless || mode == EncodeMode::pairing) {
         l.repair_count = region(256);
@@ -665,6 +710,7 @@ struct EncodeOptions {
     unsigned long long *d_n_difference = nullptr; // ... and the difference subframes chosen
     uint32_t windows = 0;                         // search_windows: the window mask ...
     unsigned long long *d_n_window = nullptr;     // ... += the units coded from a window
+    uint32_t candidates = 0;                      // search_guided: K, the orders listed by rank
     // tests only
     selab200_analysis_trace *d_trace = nullptr;      // plain: the tracing unit kernel writes every unit's analysis here
     const selab200_predictor *d_pred = nullptr;      // lossless, search, pairing, search_pairing: every unit's
@@ -676,6 +722,7 @@ struct EncodeOptions {
                                                      // order) / (unit, window, order) record here
     const selab200_predictor *d_window_pred = nullptr; // search_windows: the (unit, window) records' q
     const double *d_windows = nullptr;               // search_windows: the table the mask indexes (null: the fixed one)
+    double *d_estimates = nullptr;                   // search_guided, with d_search_trace: every unit's E[100]
 };
 
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
@@ -687,6 +734,10 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     const bool search_windows = o.mode == EncodeMode::search_windows;
     if (search_windows && !o.d_windows)
         if (int rc = check_windows(o.windows))
+            return rc;
+    const bool search_guided = o.mode == EncodeMode::search_guided;
+    if (search_guided)
+        if (int rc = check_candidates(o.candidates))
             return rc;
     const uint32_t n_windows = search_windows ? (uint32_t)__builtin_popcount(o.windows) : 0;
     const EncodeLayout l = encode_layout(o.mode, n_frames, channels, n_windows);
@@ -705,7 +756,7 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
             if (n_sub)
                 CUDA_TRY(cudaMemsetAsync(o.lossless.entries, 0, n_sub * sizeof(selab200_lossless_entry), stream));
         }
-        if (o.mode == EncodeMode::search)
+        if (o.mode == EncodeMode::search || search_guided)
             CUDA_TRY(cudaMemsetAsync(o.d_ref_words, 0, sizeof(unsigned long long), stream));
         if (pairing) {
             CUDA_TRY(cudaMemsetAsync(o.d_base_words, 0, sizeof(unsigned long long), stream));
@@ -770,17 +821,19 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         if (pairing)
             if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
                 return rc;
-    } else if (o.mode == EncodeMode::search || search_pairing || search_windows) {
+    } else if (o.mode == EncodeMode::search || search_pairing || search_windows || search_guided) {
         // the base of a search + pairing or a window search takes no reference words and no trace (its candidates
         // are traced)
         SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
         const bool base = search_pairing || search_windows;
         unsigned long long *rw = base ? nullptr : o.d_ref_words;
         selab200_search_trace *tr = base ? nullptr : o.d_search_trace;
-        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr)
-                                          : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr))
-                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr)
-                                          : launch_search<false>(p, su, n_frames, n_units, rw, stream, nullptr, tr));
+        GuidedParams gp{o.candidates, reinterpret_cast<uint4 *>(ws + l.masks), o.d_estimates};
+        const GuidedParams *pg = search_guided ? &gp : nullptr;
+        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr, pg)
+                                          : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr, pg))
+                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr, pg)
+                                          : launch_search<false>(p, su, n_frames, n_units, rw, stream, nullptr, tr, pg));
         if (rc)
             return rc;
         if (search_pairing)
@@ -1312,6 +1365,11 @@ size_t selab200_encode_search_windows_workspace_bytes(uint32_t n_frames, uint32_
     return encode_layout(EncodeMode::search_windows, n_frames, channels, (uint32_t)__builtin_popcount(windows)).bytes;
 }
 
+size_t selab200_encode_search_guided_workspace_bytes(uint32_t n_frames, uint32_t channels)
+{
+    return encode_layout(EncodeMode::search_guided, n_frames, channels).bytes;
+}
+
 int selab200_analysis_window(int index, double *out)
 {
     std::lock_guard<std::mutex> lock(g_mutex);
@@ -1439,6 +1497,27 @@ int selab200_encode_frames_search_windows_device(const int16_t *d_pcm, uint32_t 
     o.windows = windows;
     o.d_base_words = reinterpret_cast<unsigned long long *>(d_base_words);
     o.d_n_window = reinterpret_cast<unsigned long long *>(d_n_window);
+    return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
+                         d_workspace, workspace_bytes, (cudaStream_t)stream, o);
+}
+
+int selab200_encode_frames_search_guided_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
+                                                uint32_t candidates, selab200_subframe_desc *d_descs, uint32_t *d_words,
+                                                size_t words_capacity, uint64_t *d_words_used, uint64_t *d_ref_words,
+                                                int32_t *d_status, void *d_workspace, size_t workspace_bytes,
+                                                void *stream)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = d_pcm ? require_ready_for(d_pcm) : require_ready())
+        return rc;
+    if (!d_pcm || !d_descs || !d_words || !d_words_used || !d_ref_words || !d_status || !d_workspace)
+        return fail(SELAB200_ERR_ARGUMENT, "null device pointer");
+    if (int rc = check_candidates(candidates))
+        return rc;
+    EncodeOptions o;
+    o.mode = EncodeMode::search_guided;
+    o.candidates = candidates;
+    o.d_ref_words = reinterpret_cast<unsigned long long *>(d_ref_words);
     return encode_device(d_pcm, n_frames, channels, d_descs, d_words, words_capacity, d_words_used, d_status,
                          d_workspace, workspace_bytes, (cudaStream_t)stream, o);
 }
@@ -1615,9 +1694,9 @@ static int lossless_area(size_t n_sub, LosslessArgs &la)
 }
 
 // The pipelined encoder over host buffers, running `mode`, into r; frames numbered from frame_base in what it
-// reports.
+// reports.  arg: the mode's parameter, the window search's mask or the guided order search's candidate count.
 static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                       EncodeMode mode, uint32_t windows, uint32_t frame_base, Result &r)
+                       EncodeMode mode, uint32_t arg, uint32_t frame_base, Result &r)
 {
     const size_t words_capacity = t.words_capacity;
     const bool to_container = t.form == EncodeForm::container;
@@ -1630,6 +1709,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
     const size_t frame_bytes = (size_t)channels * kFrame * 2;
     const bool verify = t.verify && to_container;
     const bool lossless = mode == EncodeMode::lossless;
+    const uint32_t windows = mode == EncodeMode::search_windows ? arg : 0;
     const size_t ws_bytes = encode_layout(mode, plan.max_frames, channels, (uint32_t)__builtin_popcount(windows)).bytes;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
@@ -1684,6 +1764,7 @@ static int encode_host(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
         o.d_n_difference = &d_ctr->n_difference;
         o.windows = windows;
         o.d_n_window = &d_ctr->n_window;
+        o.candidates = mode == EncodeMode::search_guided ? arg : 0;
         if (int rc = encode_device(d_pcm + (size_t)f0 * channels * kFrame, nf, channels, d_descs + (size_t)f0 * channels,
                                    d_words, words_capacity, &d_ctr->used, &d_ctr->status, ws.ptr, ws.bytes, cs, o))
             return rc;
@@ -2068,9 +2149,9 @@ static int place_blocks(const std::vector<DevicePart> &parts, uint32_t channels,
 }
 
 // Every host-buffer encode: encode_host on each block of run_blocks, then, with several blocks, place_blocks.  r: the
-// results of all blocks.  windows: the window search's mask.
+// results of all blocks.  arg: the mode's parameter (encode_host).
 static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channels, const EncodeTarget &t,
-                         EncodeMode mode, Result &r, uint32_t windows = 0)
+                         EncodeMode mode, Result &r, uint32_t arg = 0)
 {
     const bool split = use_all_devices(n_frames);
     const size_t per_frame = (size_t)channels * kFrame;
@@ -2083,7 +2164,7 @@ static int encode_blocks(const int16_t *pcm, uint32_t n_frames, uint32_t channel
             block.container = nullptr;
             block.words_capacity = selab200_encode_words_bound(p.nf, channels);
         }
-        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, mode, windows, p.f0, p.res);
+        return encode_host(pcm + p.f0 * per_frame, p.nf, channels, block, mode, arg, p.f0, p.res);
     });
     r = std::move(b.total);
     if (b.rc || !split)
@@ -2213,6 +2294,28 @@ int selab200_encode_frames_search_windows(const int16_t *pcm, uint32_t n_frames,
     return rc;
 }
 
+int selab200_encode_frames_search_guided(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t candidates,
+                                        selab200_subframe_desc *descs, uint32_t *words, size_t words_capacity,
+                                        size_t *words_used, size_t *ref_words)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!pcm || !descs || !words || !words_used || !ref_words)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (int rc = check_channels(channels))
+        return rc;
+    if (int rc = check_candidates(candidates))
+        return rc;
+    Result r;
+    const int rc = encode_blocks(pcm, n_frames, channels, EncodeTarget{EncodeForm::arena, false, descs, words, nullptr,
+                                                                       words_capacity}, EncodeMode::search_guided, r,
+                                 candidates);
+    *words_used = r.words;
+    *ref_words = (size_t)r.ref_words;
+    return rc;
+}
+
 size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 {
     return (size_t)container_frame_byte(n_frames, channels, selab200_encode_words_bound(n_frames, channels));
@@ -2223,7 +2326,7 @@ size_t selab200_container_bound(uint32_t n_frames, uint32_t channels)
 // selab200_encode_container in every mode, and with `verify` its verified form (g_mutex held by the caller).
 static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t sample_rate,
                                  uint16_t bits_per_sample, uint8_t *container, size_t capacity, size_t *bytes_used,
-                                 EncodeMode mode, bool verify, Result &r, uint32_t windows = 0)
+                                 EncodeMode mode, bool verify, Result &r, uint32_t arg = 0)
 {
     if (int rc = require_ready())
         return rc;
@@ -2243,7 +2346,7 @@ static int encode_container_impl(const int16_t *pcm, uint32_t n_frames, uint32_t
     memcpy(container, header, sizeof header);
     const EncodeTarget t{EncodeForm::container, false, nullptr, nullptr, container, (size_t)((capacity - fixed) / 4),
                          verify};
-    const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r, windows);
+    const int rc = encode_blocks(pcm, n_frames, channels, t, mode, r, arg);
     *bytes_used = (size_t)container_frame_byte(n_frames, channels, r.words);
     r.ref_bytes = (size_t)container_frame_byte(n_frames, channels,
                                                mode == EncodeMode::pairing || mode == EncodeMode::search_pairing ||
@@ -2372,6 +2475,25 @@ int selab200_encode_container_search_windows(const int16_t *pcm, uint32_t n_fram
                                          bytes_used, EncodeMode::search_windows, false, r, windows);
     *base_bytes = r.ref_bytes;
     *n_window = (size_t)r.n_window;
+    return rc;
+}
+
+int selab200_encode_container_search_guided(const int16_t *pcm, uint32_t n_frames, uint32_t channels,
+                                           uint32_t candidates, uint32_t sample_rate, uint16_t bits_per_sample,
+                                           uint8_t *container, size_t capacity, size_t *bytes_used, size_t *ref_bytes)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!ref_bytes) {
+        if (int rc = require_ready())
+            return rc;
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    }
+    if (int rc = check_candidates(candidates))
+        return rc;
+    Result r;
+    const int rc = encode_container_impl(pcm, n_frames, channels, sample_rate, bits_per_sample, container, capacity,
+                                         bytes_used, EncodeMode::search_guided, false, r, candidates);
+    *ref_bytes = r.ref_bytes;
     return rc;
 }
 
@@ -2722,6 +2844,8 @@ struct BatchOutputs {
                                                            // records ...
     selab200_search_unit *units = nullptr;                 // ... and the search records (search)
     uint8_t *par = nullptr;                                // ... and the pairing's choice (pairing, search_pairing)
+    double *estimates = nullptr;                           // search_guided, with trace: every unit's E[100] ...
+    uint32_t *masks = nullptr;                             // ... and its order mask, 4 words
 };
 
 // A test hook's predictors: every order in min_order..kMaxOrder, every q in [-64, 63], and with zero_past, every q
@@ -2746,16 +2870,19 @@ static int check_predictors(const selab200_predictor *pred, size_t n, int min_or
 
 // For tests: one unpipelined batch of `mode` through encode_device on g.stream.  pred (lossless: required): every
 // unit's predictor, for the pairing and the search + pairing followed by the candidates', for the window search by
-// the (unit, window) records' (include/sela_b200.h).  windows: the window search's mask; with window_table (host,
-// popcount(windows) rows of 2048) the mask selects that table's rows in place of the fixed table's.
+// the (unit, window) records' (include/sela_b200.h).  arg: the window search's mask, or the guided order search's
+// candidate count; with window_table (host, popcount(mask) rows of 2048) the mask selects that table's rows in place
+// of the fixed table's.
 static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, uint32_t channels,
                         const selab200_predictor *pred, selab200_subframe_desc *descs, uint32_t *words,
-                        size_t words_capacity, const BatchOutputs &out, uint32_t windows = 0,
+                        size_t words_capacity, const BatchOutputs &out, uint32_t arg = 0,
                         const double *window_table = nullptr)
 {
     if (int rc = require_ready())
         return rc;
-    const bool lossless = mode == EncodeMode::lossless, search = mode == EncodeMode::search,
+    const bool search_guided = mode == EncodeMode::search_guided;
+    const uint32_t windows = mode == EncodeMode::search_windows ? arg : 0;
+    const bool lossless = mode == EncodeMode::lossless, search = mode == EncodeMode::search || search_guided,
                search_pairing = mode == EncodeMode::search_pairing,
                search_windows = mode == EncodeMode::search_windows,
                pairing = mode == EncodeMode::pairing || search_pairing;
@@ -2769,6 +2896,9 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
         return rc;
     if (search_windows && !window_table)
         if (int rc = check_windows(windows))
+            return rc;
+    if (search_guided)
+        if (int rc = check_candidates(arg))
             return rc;
     *out.words_used = 0;
     if (lossless)
@@ -2802,15 +2932,17 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
                                : out.trace  ? n_records * sizeof(selab200_search_trace)
                                             : 0;
     const size_t table_bytes = window_table ? (size_t)n_windows * kFrame * sizeof(double) : 0;
+    const size_t est_bytes = out.estimates ? n_units * kMaxOrder * sizeof(double) : 0;
     if (int rc = g.in.ensure(n_sub * kFrame * 2)) return rc;
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
     if (int rc = g.work.ensure(l.bytes)) return rc;
-    if (int rc = g.aux.ensure(pred_bytes + align256(trace_bytes) + table_bytes)) return rc;
+    if (int rc = g.aux.ensure(pred_bytes + align256(trace_bytes) + align256(table_bytes) + est_bytes)) return rc;
     Counters *d_ctr = device_counters();
     const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
     void *d_trace = static_cast<char *>(g.aux.ptr) + pred_bytes;
     double *d_table = reinterpret_cast<double *>(static_cast<char *>(g.aux.ptr) + pred_bytes + align256(trace_bytes));
+    double *d_est = reinterpret_cast<double *>(reinterpret_cast<char *>(d_table) + align256(table_bytes));
     EncodeOptions o; // fresh: encode_device resets the counters and records
     o.mode = mode;
     if (lossless)
@@ -2820,6 +2952,8 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     o.d_n_difference = &d_ctr->n_difference;
     o.windows = windows;
     o.d_n_window = &d_ctr->n_window;
+    o.candidates = search_guided ? arg : 0;
+    o.d_estimates = est_bytes ? d_est : nullptr;
     o.d_pred = pred ? d_pred : nullptr;
     o.d_pair_pred = pred && pairing ? d_pred + n_units : nullptr;
     o.d_window_pred = pred && search_windows ? d_pred + n_units : nullptr;
@@ -2845,6 +2979,10 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     if (out.window_keys)
         CUDA_TRY(cudaMemcpyAsync(out.window_keys, ws + l.window_keys, n_units * sizeof(uint64_t), cudaMemcpyDeviceToHost,
                                  g.stream));
+    if (out.masks)
+        CUDA_TRY(cudaMemcpyAsync(out.masks, ws + l.masks, n_units * sizeof(uint4), cudaMemcpyDeviceToHost, g.stream));
+    if (est_bytes)
+        CUDA_TRY(cudaMemcpyAsync(out.estimates, d_est, est_bytes, cudaMemcpyDeviceToHost, g.stream));
     if (trace_bytes)
         CUDA_TRY(cudaMemcpyAsync(out.analysis ? static_cast<void *>(out.analysis) : static_cast<void *>(out.trace),
                                  d_trace, trace_bytes, cudaMemcpyDeviceToHost, g.stream));
@@ -3045,6 +3183,27 @@ int selab200_encode_search_windows_trace(const int16_t *pcm, uint32_t n_frames, 
     out.window_keys = keys;
     return encode_batch(EncodeMode::search_windows, pcm, n_frames, channels, pred, descs, words, words_capacity, out,
                         (1u << n_windows) - 1, windows);
+}
+
+// For tests: the guided order search on one unpipelined batch (with pred, every unit's q[0..99] and reference order
+// from it, as selab200_encode_search_forced takes them) through the tracing kernels, with every sized order's record,
+// every unit's E[100] and its order mask.
+int selab200_encode_search_guided_trace(const int16_t *pcm, uint32_t n_frames, uint32_t channels, uint32_t candidates,
+                                        const selab200_predictor *pred, selab200_subframe_desc *descs,
+                                        uint32_t *words, size_t words_capacity, size_t *words_used, size_t *ref_words,
+                                        selab200_search_trace *trace, double *estimates, uint32_t *masks)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (!trace || !estimates || !masks)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    BatchOutputs out;
+    out.words_used = words_used;
+    out.ref_words = ref_words;
+    out.trace = trace;
+    out.estimates = estimates;
+    out.masks = masks;
+    return encode_batch(EncodeMode::search_guided, pcm, n_frames, channels, pred, descs, words, words_capacity, out,
+                        candidates);
 }
 
 // selab200_fir_probe, and with `ties` selab200_fir_tie_probe (g_mutex held by the caller).

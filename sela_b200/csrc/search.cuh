@@ -75,11 +75,13 @@ __device__ __forceinline__ void step_up(double *t, int i, int q)
 // trace, its signal unit u's; a tie-free order enters wkey[u] as words << 16 | w << 8 | order, and PACK packs into u.
 // An order whose predictor leaves the domain of the int64 conversion (|2^35 t| >= 2^62, undefined in the reference;
 // a window's clamped q can get there) counts as tied: it is never eligible.
-template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false, bool WINDOW = false>
+// LISTED (PACK = false; guided order search, search_guided.cuh): only the orders whose bit o - 1 is set in
+// listed[unit] are sized; the step-up still runs through every order below the highest one sized.
+template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false, bool WINDOW = false, bool LISTED = false>
 __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
                                               int o_hi, int32_t *res, selab200_search_trace *trace = nullptr,
                                               uint32_t out = 0, uint32_t n_win = 1,
-                                              unsigned long long *wkey = nullptr)
+                                              unsigned long long *wkey = nullptr, const uint4 *listed = nullptr)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr size_t kSigBytes = unit_signal_bytes<STEREO>();
@@ -89,6 +91,7 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     static_assert(kSearchStepBytes % 16 == 0 && sizeof(CoefSmem) % 16 == 0, "search shared memory layout");
     static_assert(!PAIR || STEREO, "a pair is staged as the stereo difference is");
     static_assert(!(PAIR && WINDOW), "one kind of record");
+    static_assert(!LISTED || !(PACK || PAIR || WINDOW), "a list of a unit's orders to size");
 
     const int lane = lane_id();
     const uint32_t src = WINDOW ? unit / n_win : unit; // the analysis unit whose signal is coded
@@ -111,9 +114,18 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     __syncwarp();
     const double scale = 34359738368.0; // 2^35
     int done = 0;                       // step-up iterations applied to t
+    uint4 mask{};
+    if constexpr (LISTED)
+        mask = listed[unit];
     for (int o = o_lo; o <= o_hi; o++) {
         if (!PACK && o == ref)
             continue;
+        if constexpr (LISTED) {
+            const int b = o - 1;
+            const uint32_t m = b < 32 ? mask.x : b < 64 ? mask.y : b < 96 ? mask.z : mask.w;
+            if (!((m >> (b & 31)) & 1u))
+                continue;
+        }
         bool outside = false; // WINDOW: the predictor leaves the conversion's domain
         if (o >= 2) {
             for (; done < o; done++)

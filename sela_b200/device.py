@@ -82,6 +82,23 @@ class DeviceCodec:
             self.capacity, self.words_used.data_ptr(), self.ref_words.data_ptr(), self.status.data_ptr(),
             self.search_ws.data_ptr(), self.search_ws_bytes, C.c_void_p(stream)))
 
+    def encode_search_guided(self, pcm, candidates=4):
+        """encode with the guided order search (DESIGN.md 7.7) over `candidates` (1..100) ranked orders.
+        Asynchronous; self.ref_words (int64 cuda tensor) receives the words encode() writes for the same frames.  The
+        workspace is allocated on first use."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.numel() == self.n_sub * FRAME
+        L = lib()
+        if not hasattr(self, "guided_ws"):
+            self.guided_ws_bytes = L.selab200_encode_search_guided_workspace_bytes(self.n_frames, self.channels)
+            self.guided_ws = torch.zeros(self.guided_ws_bytes, dtype=torch.uint8, device=self.device)
+        if not hasattr(self, "ref_words"):
+            self.ref_words = torch.zeros(1, dtype=torch.int64, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(L.selab200_encode_frames_search_guided_device(
+            pcm.data_ptr(), self.n_frames, self.channels, candidates, self.descs.data_ptr(), self.words.data_ptr(),
+            self.capacity, self.words_used.data_ptr(), self.ref_words.data_ptr(), self.status.data_ptr(),
+            self.guided_ws.data_ptr(), self.guided_ws_bytes, C.c_void_p(stream)))
+
     def encode_pairing(self, pcm):
         """encode with the channel pairing (DESIGN.md 7.4).  Asynchronous; self.base_words and self.n_difference
         (int64 cuda tensors) receive the words encode_lossless() writes for the same frames and the number of

@@ -124,7 +124,7 @@ class Encoder {
     void processFrames(std::vector<data::SelaFrame> &encodedSelaFrames);
     void encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
                   size_t *refBytes = nullptr, size_t *differences = nullptr, bool searchBase = false,
-                  uint32_t windows = 0);
+                  uint32_t windows = 0, uint32_t candidates = 0);
     std::ifstream &ifStream;
     file::WavFile wavFile;
 
@@ -165,6 +165,10 @@ public:
     // the number of analysis units coded from a window.
     size_t processSearchWindowsTo(std::ofstream &outputFile, uint32_t windows, size_t &searchBytes,
                                   size_t &windowUnits);
+    // Not in the reference: processSearchTo() over only the `candidates` (1..100) orders a reflection-coefficient
+    // estimate ranks best, order 1 and the reference order (selab200_encode_container_search_guided).  Returns the
+    // bytes written; `refBytes` receives the bytes processTo() writes for the same input.
+    size_t processSearchGuidedTo(std::ofstream &outputFile, uint32_t candidates, size_t &refBytes);
 };
 class Decoder {
     void readFrames();

@@ -825,13 +825,21 @@ size_t Encoder::processSearchWindowsTo(std::ofstream &outputFile, uint32_t windo
     return (size_t)(outputFile.tellp() - at);
 }
 
+size_t Encoder::processSearchGuidedTo(std::ofstream &outputFile, uint32_t candidates, size_t &refBytes)
+{
+    const std::streampos at = outputFile.tellp();
+    encodeTo(outputFile, nullptr, nullptr, &refBytes, nullptr, false, 0, candidates);
+    return (size_t)(outputFile.tellp() - at);
+}
+
 // processTo(); with `report` through selab200_encode_container_verified (same bytes), with `recoded` through
 // selab200_encode_container_lossless, with `refBytes` through selab200_encode_container_search, with `differences`
 // as well through selab200_encode_container_pairing, and with `searchBase` too through
 // selab200_encode_container_search_pairing.  With `windows` (and refBytes, differences) through
-// selab200_encode_container_search_windows, `differences` receiving the units coded from a window.
+// selab200_encode_container_search_windows, `differences` receiving the units coded from a window.  With
+// `candidates` (and refBytes) through selab200_encode_container_search_guided.
 void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *report, std::vector<RecodedEntry> *recoded,
-                       size_t *refBytes, size_t *differences, bool searchBase, uint32_t windows)
+                       size_t *refBytes, size_t *differences, bool searchBase, uint32_t windows, uint32_t candidates)
 {
     if (differences)
         *differences = 0;
@@ -893,6 +901,11 @@ void Encoder::encodeTo(std::ofstream &outputFile, std::vector<VerifyEntry> *repo
         check(selab200_encode_container_search_windows(reinterpret_cast<const int16_t *>(file.data + dat.body),
                                                        (uint32_t)n_frames, channels, windows, w.fmt.sampleRate,
                                                        w.fmt.bitsPerSample, out, cap, &used, refBytes, differences));
+    } else if (candidates) {
+        Phase p("guided order-search encode (device)");
+        check(selab200_encode_container_search_guided(reinterpret_cast<const int16_t *>(file.data + dat.body),
+                                                      (uint32_t)n_frames, channels, candidates, w.fmt.sampleRate,
+                                                      w.fmt.bitsPerSample, out, cap, &used, refBytes));
     } else if (differences && searchBase) {
         Phase p("order-search + pairing encode (device)");
         check(selab200_encode_container_search_pairing(reinterpret_cast<const int16_t *>(file.data + dat.body),
