@@ -220,6 +220,34 @@ int  selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_
 int  selab200_container_decode(selab200_container *handle, int16_t *pcm_out);
 void selab200_container_close(selab200_container *handle);
 
+/* Random access (DESIGN.md 7.8): a batch of clips of `length` samples each from any of n_handles open containers with
+ * the same channel count.  Clip i is samples [start, start + length) of every channel of handles[clips[i].container],
+ * i.e. rows start .. start + length - 1 of that container's selab200_container_decode output viewed as
+ * [n_frames * 2048][channels], bit for bit.  The output is interleaved int16, [n_clips][length][channels], clips back
+ * to back; nothing past n_clips * length * channels samples is written.  Every (container, frame) that some clip
+ * covers is decoded exactly once per call however many clips overlap it; *frames_decoded receives their number.
+ * Frames no clip covers are neither decoded nor checked: a malformed frame fails the call (SELAB200_ERR_BITSTREAM)
+ * only if a clip covers it.  SELAB200_ERR_ARGUMENT, with the clip index in selab200_last_error(), for length 0, a
+ * clip past its container's end (ending exactly at the end is accepted), a container index >= n_handles, a non-zero
+ * reserved field, handles of different channel counts and null pointers; n_clips == 0 is SELAB200_OK and writes
+ * nothing.  Device memory apart from a device-form output does not grow with n_clips: the covered frames are decoded
+ * in groups (fewer frames each under SELAB200_CHUNK_FRAMES).  With several devices initialised the clips decode on the
+ * primary, which holds every open image; one call's clips are not spread over devices. */
+typedef struct selab200_clip {   /* 16 bytes */
+    uint32_t container;          /* index into handles[]          */
+    uint32_t reserved;           /* must be 0                     */
+    uint64_t start;              /* first sample (per channel)    */
+} selab200_clip;
+
+/* host output: pcm_out holds n_clips * length * channels int16 */
+int selab200_container_decode_clips(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
+                                    uint32_t n_clips, uint32_t length, int16_t *pcm_out, uint64_t *frames_decoded);
+/* the same, into device memory of the primary device (2-byte aligned); synchronises: returns once the output is
+ * written */
+int selab200_container_decode_clips_device(selab200_container *const *handles, uint32_t n_handles,
+                                           const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                           int16_t *d_pcm_out, uint64_t *frames_decoded);
+
 /* ------------------------------------------------------------- verify -- */
 
 /* The format is not lossless for every input: encoder and decoder round the Q35 prediction differently

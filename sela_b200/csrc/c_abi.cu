@@ -15,6 +15,7 @@
 #include <thread>
 #include <vector>
 
+#include "clips.cuh"
 #include "lossless.cuh"
 #include "pairing.cuh"
 #include "search.cuh"
@@ -108,6 +109,7 @@ struct Context {
     DeviceBuffer small;                            // Counters
     DeviceBuffer verify;                           // verify paths: count, status, per-pair records (VerifyArea)
     DeviceBuffer lossless;                         // lossless host paths: count, per-pair records of re-coded subframes
+    DeviceBuffer clip_src, clip_pieces, clip_out;  // clip decode: source addresses, gather pieces, host-form staging
     Counters *h_small = nullptr;                   // pinned: where g.small's counters come down
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
@@ -1211,6 +1213,9 @@ static void shutdown_slot()
     g.aux.release();
     g.verify.release();
     g.lossless.release();
+    g.clip_src.release();
+    g.clip_pieces.release();
+    g.clip_out.release();
     g.small.release();
     if (g.h_small)
         cudaFreeHost(g.h_small);
@@ -1864,16 +1869,29 @@ struct Upload {
     size_t bytes = 0;
 };
 
-// Where the decode-side pipeline's coded input comes from, frames numbered file-globally in both cases: the caller's
-// descriptor and word arrays (h == nullptr), or an open container whose byte image is unpacked into the word arena on
-// the device.  start() sizes the arena for the block of frames [F0, F0 + NF) and uploads what the block needs as a
-// whole; chunk() puts one chunk's descriptors and words on the device, then `also` on the stream that carried the
-// descriptors, and makes the chunk's lane wait for all of it.
+// One group of the clip decode's selection: frames of any open containers, numbered from 0 in (container, frame)
+// order.  Per subframe a descriptor re-based into one compact arena of n_words words and the device address of its
+// reflection words in its container's image; per frame its container and the end of the bytes it reads (+3 bytes of
+// slack), which say which upload pieces a chunk waits for.
+struct ClipSelection {
+    std::vector<selab200_subframe_desc> descs;
+    std::vector<unsigned long long> src;
+    std::vector<const selab200_container *> frame_h;
+    std::vector<unsigned long long> frame_end;
+};
+
+// Where the decode-side pipeline's coded input comes from, frames numbered file-globally in the first two cases: the
+// caller's descriptor and word arrays (h == nullptr), an open container whose byte image is unpacked into the word
+// arena on the device, or a clip selection (sel: descs are its descriptors, n_words its arena) unpacked from the
+// images of several open containers.  start() sizes the arena for the block of frames [F0, F0 + NF) and uploads what
+// the block needs as a whole; chunk() puts one chunk's descriptors and words on the device, then `also` on the stream
+// that carried the descriptors, and makes the chunk's lane wait for all of it.
 struct CodedInput {
     const selab200_subframe_desc *descs; // the whole file's descriptors, in host memory
     const uint32_t *words;               // caller arrays: the words the descriptors reference
     size_t n_words;
     const selab200_container *h;         // or an open container
+    const ClipSelection *sel = nullptr;  // or a clip selection
     // set by start()
     uint32_t channels = 0;
     uint32_t *arena = nullptr;           // the decoder's word array, addressed by the descriptors' offsets
@@ -1883,6 +1901,11 @@ struct CodedInput {
     int start(uint32_t F0, uint32_t NF, uint32_t ch)
     {
         channels = ch;
+        if (sel) { // re-based descriptors: the arena is addressed from 0
+            if (int rc = g.words.ensure(n_words * 4 + 96)) return rc;
+            arena = reinterpret_cast<uint32_t *>(static_cast<char *>(g.words.ptr) + 16); // 16 bytes of slack in front
+            return g.clip_src.ensure(sel->src.size() * sizeof(unsigned long long));
+        }
         if (!h) {
             if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
             arena = static_cast<uint32_t *>(g.words.ptr);
@@ -1917,9 +1940,24 @@ struct CodedInput {
         const selab200_subframe_desc *dc = descs + (size_t)f0 * channels;
         const size_t n = (size_t)nf * channels;
         // a container's descriptors go up on the chunk's own lane: s_h2d is still busy with the container bytes
-        const cudaStream_t carrier = h ? lane : g.s_h2d;
+        const cudaStream_t carrier = h || sel ? lane : g.s_h2d;
         CUDA_TRY(cudaMemcpyAsync(d_descs, dc, n * sizeof(*dc), cudaMemcpyHostToDevice, carrier));
-        if (!h) {
+        if (sel) {
+            unsigned long long *d_src = static_cast<unsigned long long *>(g.clip_src.ptr) + (size_t)f0 * channels;
+            CUDA_TRY(cudaMemcpyAsync(d_src, sel->src.data() + (size_t)f0 * channels, n * sizeof(unsigned long long),
+                                     cudaMemcpyHostToDevice, lane));
+            // every container the chunk reads: the upload piece that holds the last byte it reads there
+            for (uint32_t f = f0; f < f0 + nf; f++) {
+                const selab200_container *c = sel->frame_h[f];
+                if (f + 1 < f0 + nf && sel->frame_h[f + 1] == c)
+                    continue; // frames of one container are in file order: its last frame here reads furthest
+                const int piece = std::min(c->n_pieces - 1, (int)(sel->frame_end[f] / c->piece_bytes));
+                CUDA_TRY(cudaStreamWaitEvent(lane, c->buf.ev_piece[piece], 0));
+            }
+            k_clip_unpack<<<(unsigned)((n + 7) / 8), 256, 0, lane>>>(d_src, d_descs, (uint32_t)n, arena);
+            if (int rc = launch_check("k_clip_unpack"))
+                return rc;
+        } else if (!h) {
             unsigned long long lo, hi;
             words_referenced(dc, n, n_words, lo, hi);
             if (hi > lo)
@@ -1940,7 +1978,7 @@ struct CodedInput {
         }
         if (also.bytes)
             CUDA_TRY(cudaMemcpyAsync(also.dst, also.src, also.bytes, cudaMemcpyHostToDevice, carrier));
-        if (!h) {
+        if (!h && !sel) {
             CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
             CUDA_TRY(cudaStreamWaitEvent(lane, g.ev_h2d[c], 0));
         }
@@ -1949,8 +1987,9 @@ struct CodedInput {
 };
 
 // Frames [F0, F0 + NF) of `in` through the chunk pipeline on the device of the current context.  Without `report`
-// the decoded samples come down into pcm_out; with it, each lane compares them on the device with `source`
-// (verify_device) and only the differing pairs come back.  pcm_out, source and the report's frames are file-global.
+// the decoded samples come down into pcm_out, or, if pcm_out is null, stay in g.in for the caller (the clip decode);
+// with it, each lane compares them on the device with `source` (verify_device) and only the differing pairs come
+// back.  pcm_out, source and the report's frames are file-global.
 static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t channels, int16_t *pcm_out,
                            const int16_t *source, std::vector<selab200_verify_entry> *report)
 {
@@ -2005,8 +2044,9 @@ static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t cha
             return rc;
         CUDA_TRY(cudaEventRecord(g.ev_done[c], cs));
         CUDA_TRY(cudaStreamWaitEvent(g.s_d2h, g.ev_done[c], 0));
-        CUDA_TRY(cudaMemcpyAsync(pcm_out + file_at * kFrame, d_pcm + at * kFrame, nf * frame_bytes,
-                                 cudaMemcpyDeviceToHost, g.s_d2h));
+        if (pcm_out)
+            CUDA_TRY(cudaMemcpyAsync(pcm_out + file_at * kFrame, d_pcm + at * kFrame, nf * frame_bytes,
+                                     cudaMemcpyDeviceToHost, g.s_d2h));
     }
     if (!report)
         return read_status(g.s_d2h, d_status);
@@ -2608,7 +2648,210 @@ int walk_container(const uint8_t *b, size_t n, selab200_container_info *info,
 
 } // namespace
 
+// ---- clip decode (DESIGN.md 7.8) --------------------------------------------------------------------------------
+//
+// The selection -- every (container, frame) some clip covers, sorted and deduplicated -- is cut into groups of at most
+// clip_group_frames() frames.  Each group goes through decode_pipeline as a ClipSelection and stays decoded in g.in
+// until the pieces of the clips that fall in it are cut out (k_clip_gather), so the call's device memory is bounded by
+// a group and a gather batch whatever the number of clips.  A clip's frames are consecutive in the selection, so a
+// clip is one run of decoded rows, split only where a group ends.
+constexpr uint32_t kClipGroupSubframes = 32768;
+constexpr size_t kClipPieceBatch = 65536;              // pieces per gather launch (the device piece table)
+constexpr size_t kClipStagingBytes = (size_t)64 << 20; // host form: output bytes per gather launch
+
+// Frames per group; with SELAB200_CHUNK_FRAMES (tests, tuning) four chunks of that size.
+static uint32_t clip_group_frames(uint32_t channels)
+{
+    if (const char *env = std::getenv("SELAB200_CHUNK_FRAMES")) {
+        const long v = std::atol(env);
+        if (v > 0)
+            return (uint32_t)std::min<long>(4 * v, 1l << 20);
+    }
+    return std::max<uint32_t>(1, kClipGroupSubframes / channels);
+}
+
+// The pieces of one group, in output order, out of g.in into `out` (device form) or, through the staging buffer
+// g.clip_out, into host memory.  On g.s_d2h; returns when every piece is written.
+static int clip_gather(const std::vector<ClipPiece> &pieces, uint8_t *out, bool device_out)
+{
+    const cudaStream_t s = g.s_d2h;
+    if (int rc = g.clip_pieces.ensure(kClipPieceBatch * sizeof(ClipPiece))) return rc;
+    if (!device_out)
+        if (int rc = g.clip_out.ensure(kClipStagingBytes)) return rc;
+    uint8_t *staging = static_cast<uint8_t *>(g.clip_out.ptr);
+    std::vector<ClipPiece> batch, copies; // copies (host form): staging offset, host offset, bytes
+    size_t i = 0;
+    unsigned long long done = 0; // bytes of pieces[i] already gathered (host form: a piece may span batches)
+    while (i < pieces.size()) {
+        batch.clear();
+        copies.clear();
+        unsigned long long staged = 0, widest = 0;
+        while (i < pieces.size() && batch.size() < kClipPieceBatch) {
+            const ClipPiece &p = pieces[i];
+            unsigned long long take = p.bytes - done;
+            if (!device_out) {
+                if (staged == kClipStagingBytes)
+                    break;
+                take = std::min<unsigned long long>(take, kClipStagingBytes - staged);
+                if (!copies.empty() && copies.back().dst + copies.back().bytes == p.dst + done)
+                    copies.back().bytes += take;
+                else
+                    copies.push_back(ClipPiece{staged, p.dst + done, take});
+            }
+            batch.push_back(ClipPiece{p.src + done, device_out ? p.dst + done : staged, take});
+            staged += take;
+            widest = std::max(widest, take);
+            done += take;
+            if (done == p.bytes) {
+                i++;
+                done = 0;
+            }
+        }
+        const unsigned rows = (unsigned)std::min<unsigned long long>(64, std::max(1ull, (widest / 16 + 255) / 256));
+        CUDA_TRY(cudaMemcpyAsync(g.clip_pieces.ptr, batch.data(), batch.size() * sizeof(ClipPiece),
+                                 cudaMemcpyHostToDevice, s));
+        k_clip_gather<<<dim3((unsigned)batch.size(), rows), 256, 0, s>>>(
+            static_cast<const uint8_t *>(g.in.ptr), device_out ? out : staging,
+            static_cast<const ClipPiece *>(g.clip_pieces.ptr));
+        if (int rc = launch_check("k_clip_gather"))
+            return rc;
+        for (const ClipPiece &c : copies)
+            CUDA_TRY(cudaMemcpyAsync(out + c.dst, staging + c.src, c.bytes, cudaMemcpyDeviceToHost, s));
+    }
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return 0;
+}
+
+// Both forms of selab200_container_decode_clips, on the primary context (require_ready done, g_mutex held).
+static int decode_clips(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
+                        uint32_t n_clips, uint32_t length, uint8_t *out, bool device_out, uint64_t *frames_decoded)
+{
+    if (!frames_decoded)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    *frames_decoded = 0;
+    if (n_clips == 0)
+        return 0;
+    if (!handles || !clips || !out)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (length == 0)
+        return fail(SELAB200_ERR_ARGUMENT, "clip 0: length must be at least 1");
+    for (uint32_t i = 0; i < n_handles; i++) {
+        if (!handles[i])
+            return fail(SELAB200_ERR_ARGUMENT, "handles[%u] is null", i);
+        if (handles[i]->info.channels != handles[0]->info.channels)
+            return fail(SELAB200_ERR_ARGUMENT, "handles[%u] has %u channels, handles[0] %u", i,
+                        (unsigned)handles[i]->info.channels, (unsigned)handles[0]->info.channels);
+    }
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const selab200_clip &c = clips[i];
+        if (c.container >= n_handles)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: container %u, but %u handles", i, c.container, n_handles);
+        if (c.reserved != 0)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: reserved field is not 0", i);
+        const unsigned long long total = (unsigned long long)handles[c.container]->info.n_frames * kFrame;
+        if (c.start > total || length > total - c.start)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: samples [%llu, %llu + %u) outside the %llu samples of its container",
+                        i, (unsigned long long)c.start, (unsigned long long)c.start, length, total);
+    }
+    const uint32_t C = handles[0]->info.channels;
+    if (int rc = check_channels(C))
+        return rc;
+    const unsigned long long clip_bytes = (unsigned long long)length * C * 2;
+    if (clip_bytes > ~0ull / n_clips)
+        return fail(SELAB200_ERR_ARGUMENT, "output of %u clips of %u samples does not fit 64 bits", n_clips, length);
+
+    // the selection: (container << 32 | frame), sorted and deduplicated
+    std::vector<unsigned long long> keys;
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const unsigned long long f0 = clips[i].start / kFrame, f1 = (clips[i].start + length - 1) / kFrame;
+        for (unsigned long long f = f0; f <= f1; f++)
+            keys.push_back((unsigned long long)clips[i].container << 32 | f);
+    }
+    std::sort(keys.begin(), keys.end());
+    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+    *frames_decoded = keys.size();
+
+    // every clip as rows [r0, r0 + length) of the selection decoded back to back, cut at group ends
+    const unsigned long long group_rows = (unsigned long long)clip_group_frames(C) * kFrame;
+    const size_t n_groups = (keys.size() * kFrame + group_rows - 1) / group_rows;
+    std::vector<std::vector<ClipPiece>> pieces(n_groups);
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const unsigned long long key = (unsigned long long)clips[i].container << 32 | clips[i].start / kFrame;
+        const unsigned long long k = (unsigned long long)(std::lower_bound(keys.begin(), keys.end(), key) - keys.begin());
+        const unsigned long long r0 = k * kFrame + clips[i].start % kFrame, r1 = r0 + length;
+        for (unsigned long long grp = r0 / group_rows; grp <= (r1 - 1) / group_rows; grp++) {
+            const unsigned long long lo = std::max(r0, grp * group_rows), hi = std::min(r1, (grp + 1) * group_rows);
+            pieces[grp].push_back(ClipPiece{(lo - grp * group_rows) * C * 2, i * clip_bytes + (lo - r0) * C * 2,
+                                            (hi - lo) * C * 2});
+        }
+    }
+
+    ClipSelection sel;
+    for (size_t grp = 0; grp < n_groups; grp++) {
+        const size_t s0 = grp * (size_t)(group_rows / kFrame), s1 = std::min(keys.size(), s0 + (size_t)(group_rows / kFrame));
+        const uint32_t nf = (uint32_t)(s1 - s0);
+        sel.descs.resize((size_t)nf * C);
+        sel.src.resize((size_t)nf * C);
+        sel.frame_h.resize(nf);
+        sel.frame_end.resize(nf);
+        unsigned long long words = 0;
+        for (uint32_t s = 0; s < nf; s++) {
+            const selab200_container *h = handles[keys[s0 + s] >> 32];
+            const unsigned long long f = keys[s0 + s] & 0xffffffffull;
+            const unsigned long long image = reinterpret_cast<unsigned long long>(h->buf.d_bytes);
+            for (uint32_t c = 0; c < C; c++) {
+                selab200_subframe_desc d = h->buf.h_descs[f * C + c];
+                const unsigned long long at = container_frame_byte(f, C, d.refl_offset) + 4 + (unsigned long long)kSubframeHeaderBytes * c + 7;
+                sel.src[(size_t)s * C + c] = image + at;
+                sel.frame_end[s] = at + 4ull * d.refl_words + 5 + 4ull * d.res_words + 3;
+                d.refl_offset = words;
+                d.res_offset = words + d.refl_words;
+                words += (unsigned long long)d.refl_words + d.res_words;
+                sel.descs[(size_t)s * C + c] = d;
+            }
+            sel.frame_h[s] = h;
+        }
+        CodedInput in{sel.descs.data(), nullptr, (size_t)words, nullptr, &sel};
+        if (int rc = decode_pipeline(in, 0, nf, C, nullptr, nullptr, nullptr))
+            return rc;
+        if (int rc = clip_gather(pieces[grp], out, device_out))
+            return rc;
+    }
+    return 0;
+}
+
 extern "C" {
+
+int selab200_container_decode_clips(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
+                                    uint32_t n_clips, uint32_t length, int16_t *pcm_out, uint64_t *frames_decoded)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    return decode_clips(handles, n_handles, clips, n_clips, length, reinterpret_cast<uint8_t *>(pcm_out), false,
+                        frames_decoded);
+}
+
+int selab200_container_decode_clips_device(selab200_container *const *handles, uint32_t n_handles,
+                                           const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                           int16_t *d_pcm_out, uint64_t *frames_decoded)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (d_pcm_out && n_clips) { // the primary holds every open image, so the output must live there too
+        cudaPointerAttributes attr;
+        if (cudaPointerGetAttributes(&attr, d_pcm_out) != cudaSuccess || attr.type != cudaMemoryTypeDevice ||
+            attr.device != g.device) {
+            cudaGetLastError();
+            return fail(SELAB200_ERR_ARGUMENT, "d_pcm_out is not device memory of the primary device (%d)", g.device);
+        }
+        if (reinterpret_cast<uintptr_t>(d_pcm_out) & 1)
+            return fail(SELAB200_ERR_ARGUMENT, "d_pcm_out is not 2-byte aligned");
+    }
+    return decode_clips(handles, n_handles, clips, n_clips, length, reinterpret_cast<uint8_t *>(d_pcm_out), true,
+                        frames_decoded);
+}
 
 int selab200_container_info_get(const uint8_t *container, size_t n_bytes, selab200_container_info *info)
 {

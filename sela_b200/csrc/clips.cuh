@@ -1,0 +1,84 @@
+// clips.cuh -- the clip decode (selab200_container_decode_clips, DESIGN.md 7.8): sample ranges of open containers.
+//
+// The host selects the (container, frame) pairs a batch of clips covers, sorted and deduplicated, and gives every
+// selected subframe a compact descriptor re-based into one word arena plus the device address of its reflection
+// words in its container's byte image.  Two kernels of their own; the decode in between is decode_device, unchanged:
+//   k_clip_unpack  one warp per selected subframe: both word arrays from any open container (any byte alignment)
+//                  into the compact arena (16-byte aligned), as k_container_unpack does for one file in file order;
+//   k_clip_gather  one CTA row per piece of a clip: its bytes out of the decoded frames into the output, aligned
+//                  16-byte stores fed by funnel-shifted aligned loads, int16 stores only at the two ragged ends.
+#pragma once
+
+#include "kernels.cuh"
+
+namespace selab200 {
+
+// One selected subframe's word arrays from its container's byte image (src: the device address of its reflection
+// words; the residue words follow them after 5 bytes of header) into arena + the descriptor's re-based offsets.
+__global__ void __launch_bounds__(256) k_clip_unpack(const unsigned long long *src, const selab200_subframe_desc *descs,
+                                                     uint32_t n_sub, uint32_t *arena)
+{
+    const uint32_t sub = blockIdx.x * 8 + warp_id();
+    if (sub >= n_sub)
+        return;
+    const selab200_subframe_desc d = descs[sub];
+    const unsigned long long a = src[sub];
+    // get_words_at_byte takes the alignment from its byte offset: address the image from the 16-byte block below
+    const uint8_t *base = reinterpret_cast<const uint8_t *>(a & ~15ull);
+    const unsigned long long D = a & 15;
+    get_words_at_byte(base, D, arena + d.refl_offset, d.refl_words);
+    get_words_at_byte(base, D + 4ull * d.refl_words + 5, arena + d.res_offset, d.res_words);
+}
+
+// A run of output bytes: `bytes` bytes from decoded-frame byte src to output byte dst (both even).
+struct ClipPiece {
+    unsigned long long src, dst, bytes;
+};
+
+// The 16 bytes at byte phase 4q + 2h of the 32 bytes in w (h: 0 or 1; q uniform across the CTA).
+template <int Q>
+__device__ __forceinline__ uint4 clip_window(const uint32_t (&w)[8], uint32_t sh)
+{
+    return make_uint4(__funnelshift_r(w[Q], w[Q + 1], sh), __funnelshift_r(w[Q + 1], w[Q + 2], sh),
+                      __funnelshift_r(w[Q + 2], w[Q + 3], sh), __funnelshift_r(w[Q + 3], w[Q + 4], sh));
+}
+
+// Piece blockIdx.x; the CTAs of grid row y take every gridDim.y-th 256-block stretch of its aligned body.  Reads at
+// most 15 bytes past a piece's last source byte (the decoded-frame buffer is padded).
+__global__ void __launch_bounds__(256) k_clip_gather(const uint8_t *frames, uint8_t *out, const ClipPiece *pieces)
+{
+    const ClipPiece p = pieces[blockIdx.x];
+    const unsigned long long d0 = reinterpret_cast<unsigned long long>(out) + p.dst, d1 = d0 + p.bytes;
+    const unsigned long long s0 = reinterpret_cast<unsigned long long>(frames) + p.src;
+    const unsigned long long a0 = (d0 + 15) & ~15ull, a1 = d1 & ~15ull; // the aligned body [a0, a1) (empty if a1 <= a0)
+    const unsigned long long off = s0 - d0;                                // source address = destination + off
+    if (blockIdx.y == 0 && threadIdx.x < 16) { // ragged ends: up to 7 samples in front of the body, 7 behind it
+        const unsigned long long x = threadIdx.x < 8 ? d0 + 2 * threadIdx.x : (a1 > a0 ? a1 : a0) + 2 * (threadIdx.x - 8);
+        const bool mine = threadIdx.x < 8 ? x < a0 && x < d1 : x < d1 && x >= a0;
+        if (mine)
+            *reinterpret_cast<int16_t *>(x) = *reinterpret_cast<const int16_t *>(x + off);
+    }
+    if (a1 <= a0)
+        return;
+    const unsigned long long n_blocks = (a1 - a0) >> 4;
+    const uint32_t phase = (uint32_t)(off & 15), q = phase >> 2, sh = 8 * (phase & 3);
+    for (unsigned long long b = (unsigned long long)blockIdx.y * blockDim.x + threadIdx.x; b < n_blocks;
+         b += (unsigned long long)gridDim.y * blockDim.x) {
+        const unsigned long long x = a0 + 16 * b;
+        const uint4 *s = reinterpret_cast<const uint4 *>((x + off) & ~15ull);
+        uint4 v = __ldg(s);
+        if (phase) {
+            const uint4 u = __ldg(s + 1);
+            const uint32_t w[8] = {v.x, v.y, v.z, v.w, u.x, u.y, u.z, u.w};
+            switch (q) {
+            case 0: v = clip_window<0>(w, sh); break;
+            case 1: v = clip_window<1>(w, sh); break;
+            case 2: v = clip_window<2>(w, sh); break;
+            default: v = clip_window<3>(w, sh); break;
+            }
+        }
+        *reinterpret_cast<uint4 *>(x) = v;
+    }
+}
+
+} // namespace selab200

@@ -182,6 +182,10 @@ public:
     // Not in the reference: process() + WavFile::writeToFile() in one step, byte-identical output
     // (selab200_container_open / _decode: the .sela bytes go to the device as they lie in the file).
     void processTo(std::ofstream &outputFile);
+    // Not in the reference: processTo() for samples [firstSample, firstSample + nSamples) of every channel only
+    // (selab200_container_decode_clips: only the frames the range covers are decoded).  The header is the one
+    // processTo() writes for that many samples; the data chunk equals the same bytes of processTo()'s.
+    void processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples);
     // Not in the reference: decode this .sela stream on the device and compare it with the whole frames of the
     // WAV file `wavInput` (its partial final frame is ignored, as the encoder ignores it).  Returns every
     // (frame, channel) that differs, in order.  Throws data::Exception if the WAV's channels, sample rate or

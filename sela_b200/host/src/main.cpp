@@ -23,12 +23,15 @@
 // `-F in.wav out.sela` ("fast search"): -S over only the 4 orders a reflection-coefficient estimate ranks best, order 1
 // and the reference order; most of -S's saving at a fraction of its cost, decoding back to the WAV under the
 // reference decoder.  One line with the bytes written and the bytes -e writes.
+// `-R in.sela out.wav first_sample n_samples` (random access): the WAV -d writes, cut to samples
+// [first_sample, first_sample + n_samples) of every channel; only the frames that range covers are decoded.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
 #include <fstream>
 #include <iostream>
 #include <mutex>
+#include <stdexcept>
 #include <string>
 #include <thread>
 #include <vector>
@@ -124,6 +127,8 @@ int usage(const std::string &prog)
               << prog << " -W path/to/input.wav path/to/output.sela\n\n"
               << "Encoding a file smaller, searching the predictor orders an estimate ranks best (H100 build):\n"
               << prog << " -F path/to/input.wav path/to/output.sela\n\n"
+              << "Decoding samples [first, first + count) of every channel of a file (H100 build):\n" << prog
+              << " -R path/to/input.sela path/to/output.wav first count\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -176,6 +181,18 @@ int main(int argc, char **argv)
             } else {
                 sela::Decoder(in).processTo(out);
             }
+        } else if (mode == "-R" && argc == 6) {
+            uint64_t first = 0, count = 0;
+            try {
+                first = std::stoull(argv[4]);
+                count = std::stoull(argv[5]);
+            } catch (const std::exception &) {
+                throw data::Exception("first sample and sample count must be non-negative integers");
+            }
+            std::ifstream in(argv[2], std::ios::binary);
+            std::ofstream out(argv[3], std::ios::binary);
+            std::cout << "Decoding samples " << first << " to " << first + count << ": " << argv[2] << std::endl;
+            sela::Decoder(in).processRangeTo(out, first, count);
         } else if (mode == "-V" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ofstream out(argv[3], std::ios::binary);

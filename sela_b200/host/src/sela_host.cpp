@@ -976,6 +976,49 @@ void Decoder::processTo(std::ofstream &outputFile)
     outputFile.write(reinterpret_cast<const char *>(pcm), (std::streamsize)(n_samples * 2));
 }
 
+// processTo() for one sample range: the container opens as for processTo(), and one clip comes back.
+void Decoder::processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples)
+{
+    StagingScope staging;
+    DeviceWarmup warmup;
+    RawFile file;
+    {
+        Phase p("read input");
+        file = slurp_raw(ifStream);
+    }
+    warmup.join();
+    selab200_container *handle = nullptr;
+    selab200_container_info info;
+    {
+        Phase p("open (upload + walk)");
+        if (selab200_container_open(file.bytes(), file.size, &handle, &info) != SELAB200_OK)
+            raise(selab200_last_error());
+    }
+    struct Closer {
+        selab200_container *h;
+        ~Closer() { selab200_container_close(h); }
+    } closer{handle};
+    if (nSamples == 0 || nSamples > 0xffffffffull)
+        raise("sela_b200: the sample count must be in [1, 2^32 - 1]");
+    if (info.channels == 0 || info.channels > SELAB200_MAX_CHANNELS)
+        raise("sela_b200: unsupported channel count");
+    const size_t n_values = (size_t)nSamples * info.channels;
+    int16_t *pcm = reinterpret_cast<int16_t *>(t_output.ensure((n_values + 1) * 2));
+    {
+        Phase p("decode range (device)");
+        const selab200_clip clip{0, 0, firstSample};
+        uint64_t frames = 0;
+        check(selab200_container_decode_clips(&handle, 1, &clip, 1, (uint32_t)nSamples, pcm, &frames));
+    }
+    Phase p("write output");
+    file::WavFile shell(info.sample_rate, info.bits_per_sample, info.channels, {});
+    const size_t payload = n_values * (info.bits_per_sample / 8);
+    shell.wavChunk.chunkSize = (uint32_t)(payload + 36);
+    shell.wavChunk.dataSubChunk.subChunkSize = (uint32_t)payload;
+    write_wav_header(outputFile, shell.wavChunk);
+    outputFile.write(reinterpret_cast<const char *>(pcm), (std::streamsize)(n_values * 2));
+}
+
 // The .sela stream against a WAV file: the .sela bytes go to the device as processTo() sends them, the WAV's
 // data chunk goes up chunk by chunk from where it lies in the file buffer, and only the report comes back.
 std::vector<VerifyEntry> Decoder::verifyAgainst(std::ifstream &wavInput)
