@@ -325,26 +325,25 @@ int launch_check(const char *what)
     return 0;
 }
 
+// kernel<<<grid, block, smem, stream>>>(args...) with the kernel's dynamic shared-memory limit raised to smem first,
+// and the launch checked (`name` in the error).
+template <typename... Params, typename... Args>
+int launch(void (*kernel)(Params...), size_t grid, unsigned block, size_t smem, cudaStream_t stream, const char *name,
+           const Args &...args)
+{
+    if (smem)
+        if (int rc = set_smem(kernel, smem))
+            return rc;
+    kernel<<<(unsigned)grid, block, smem, stream>>>(args...);
+    return launch_check(name);
+}
+
 // The mean of every analysis unit (k_unit_means<KIND>, a warp per 32 units) into means[n_units].
 template <int KIND>
 int launch_unit_means(const void *src, size_t n_units, uint32_t channels, double *means, cudaStream_t stream)
 {
-    const MeanTiling mt = mean_tiling(KIND, channels);
-    k_unit_means<KIND><<<(unsigned)((n_units + 31) / 32), 32, unit_means_smem_bytes(mt), stream>>>(src, (uint32_t)n_units,
-                                                                                                 channels, means);
-    return launch_check("k_unit_means");
-}
-
-// k_encode_units<STEREO, TRACE, CHECK, FORCE>, a warp per analysis unit.
-template <bool STEREO, bool TRACE, bool CHECK = false, bool FORCE = false>
-int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis_trace *d_trace, cudaStream_t stream,
-                        const selab200_predictor *d_pred = nullptr)
-{
-    constexpr size_t smem = encode_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_encode_units<STEREO, TRACE, CHECK, FORCE>, smem))
-        return rc;
-    k_encode_units<STEREO, TRACE, CHECK, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_trace, d_pred);
-    return launch_check("k_encode_units");
+    return launch(k_unit_means<KIND>, (n_units + 31) / 32, 32, unit_means_smem_bytes(mean_tiling(KIND, channels)),
+                  stream, "k_unit_means", src, (uint32_t)n_units, channels, means);
 }
 
 // The lossless encode (lossless.cuh) in place of k_encode_units: the analysis with the tie check,
@@ -352,112 +351,63 @@ int launch_encode_units(const EncodeParams &p, size_t n_units, selab200_analysis
 // depends on what the check found.  The warp kernels use at most one residue row per unit of the batch.  FORCE: the
 // units' predictors are d_pred's (selab200_encode_lossless_forced).  pairing: the base of a pairing encode, which
 // keeps the tie flags that the select kernel clears and takes no report.
-template <bool STEREO, bool FORCE = false>
+template <bool STEREO, bool FORCE>
 int launch_lossless(const EncodeParams &p, const RepairParams &r, size_t n_frames, size_t n_units, cudaStream_t stream,
                     const selab200_predictor *d_pred, const PairingParams *pairing)
 {
-    if (int rc = launch_encode_units<STEREO, false, true, FORCE>(p, n_units, nullptr, stream, d_pred))
-        return rc;
     constexpr size_t smem = encode_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_lossless_candidates<STEREO, FORCE>, smem))
+    const size_t frame_ctas = (n_frames + 255) / 256, warps = std::min(n_units, (size_t)g.sms * 32);
+    if (int rc = launch(k_encode_units<STEREO, false, true, FORCE>, n_units, 32, smem, stream, "k_encode_units", p,
+                        nullptr, d_pred))
         return rc;
-    if (int rc = set_smem(k_lossless_repack<STEREO, FORCE>, smem))
-        return rc;
-    if (pairing) {
-        k_pairing_capture<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, *pairing);
-        if (int rc = launch_check("k_pairing_capture"))
+    if (pairing)
+        if (int rc = launch(k_pairing_capture, frame_ctas, 256, 0, stream, "k_pairing_capture", p, *pairing))
             return rc;
-    }
-    k_lossless_select<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, r);
-    if (int rc = launch_check("k_lossless_select"))
+    if (int rc = launch(k_lossless_select, frame_ctas, 256, 0, stream, "k_lossless_select", p, r))
         return rc;
-    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
-    for (int round = 0; round < 2; round++) {
-        k_lossless_candidates<STEREO, FORCE><<<warps, 32, smem, stream>>>(p, r, round, d_pred);
-        if (int rc = launch_check("k_lossless_candidates"))
+    for (int round = 0; round < 2; round++)
+        if (int rc = launch(k_lossless_candidates<STEREO, FORCE>, warps, 32, smem, stream, "k_lossless_candidates", p, r,
+                            round, d_pred))
             return rc;
-    }
-    k_lossless_repack<STEREO, FORCE><<<warps, 32, smem, stream>>>(p, r, d_pred);
-    if (int rc = launch_check("k_lossless_repack"))
+    if (int rc = launch(k_lossless_repack<STEREO, FORCE>, warps, 32, smem, stream, "k_lossless_repack", p, r, d_pred))
         return rc;
     if (pairing)
         return 0;
-    k_lossless_report<<<(unsigned)std::min((n_frames + 255) / 256, (size_t)g.sms), 256, 0, stream>>>(p, r);
-    return launch_check("k_lossless_report");
-}
-
-// The guided order search's candidates (search_guided.cuh): the estimate and every unit's listed orders sized.  trace:
-// the tracing instantiations (gp.estimates is set).
-template <bool STEREO>
-int launch_guided(const EncodeParams &p, SearchUnit *su, const GuidedParams &gp, unsigned warps, cudaStream_t stream,
-                  selab200_search_trace *trace)
-{
-    constexpr size_t smem_orders = search_smem_bytes<STEREO>();
-    if (int rc = trace ? set_smem(k_search_listed<STEREO, true>, smem_orders)
-                       : set_smem(k_search_listed<STEREO, false>, smem_orders))
-        return rc;
-    if (trace)
-        k_search_estimate<true><<<warps, 32, 0, stream>>>(p, su, gp);
-    else
-        k_search_estimate<false><<<warps, 32, 0, stream>>>(p, su, gp);
-    if (int rc = launch_check("k_search_estimate"))
-        return rc;
-    if (trace)
-        k_search_listed<STEREO, true><<<warps, 32, smem_orders, stream>>>(p, su, gp, trace);
-    else
-        k_search_listed<STEREO, false><<<warps, 32, smem_orders, stream>>>(p, su, gp, nullptr);
-    return launch_check("k_search_listed");
+    return launch(k_lossless_report, std::min(frame_ctas, (size_t)g.sms), 256, 0, stream, "k_lossless_report", p, r);
 }
 
 // The order search (search.cuh) in place of k_encode_units: analysis, candidates, repack, and the reference encoder's
 // words added to *d_ref_words.  The warp kernels have grids of a fixed size, at most one residue row per unit of the
 // batch.  d_ref_words null (the base of a search + pairing): k_search_ref_words is not run.  FORCE: the units' q and
-// reference orders are d_pred's (selab200_encode_search_forced).  d_trace: the
-// analysis and candidate kernels are their tracing instantiations, which write every (unit, order) record there
-// (selab200_encode_search_trace).  gp (guided order search, DESIGN.md 7.7): k_search_estimate and k_search_listed
-// in place of k_search_candidates, their tracing instantiations with d_trace.
-template <bool STEREO, bool FORCE = false>
+// reference orders are d_pred's (selab200_encode_search_forced).  TRACE: the analysis and candidate kernels are their
+// tracing instantiations, which write every (unit, order) record to d_trace (selab200_encode_search_trace).  gp
+// (guided order search, search_guided.cuh): the estimate, and every unit's listed orders sized by k_search_listed in
+// place of k_search_candidates; with TRACE, every unit's estimates to gp->estimates as well.
+template <bool STEREO, bool FORCE, bool TRACE>
 int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t n_units,
-                  unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred = nullptr,
-                  selab200_search_trace *d_trace = nullptr, const GuidedParams *gp = nullptr)
+                  unsigned long long *d_ref_words, cudaStream_t stream, const selab200_predictor *d_pred,
+                  selab200_search_trace *d_trace, const GuidedParams *gp)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_search_units<STEREO, FORCE>, smem))
+    const size_t warps = std::min(n_units, (size_t)g.sms * 32);
+    if (int rc = launch(k_search_units<STEREO, TRACE, FORCE>, n_units, 32, smem, stream, "k_search_units", p, d_pred,
+                        su, d_trace))
         return rc;
-    if (int rc = set_smem(k_search_candidates<STEREO>, smem_orders))
-        return rc;
-    if (int rc = set_smem(k_search_repack<STEREO>, smem_orders))
-        return rc;
-    if (d_trace) {
-        if (int rc = set_smem(k_search_units_trace<STEREO, FORCE>, smem))
-            return rc;
-        if (int rc = set_smem(k_search_candidates_trace<STEREO>, smem_orders))
-            return rc;
-        k_search_units_trace<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su, d_trace);
-    } else {
-        k_search_units<STEREO, FORCE><<<(unsigned)n_units, 32, smem, stream>>>(p, d_pred, su);
-    }
-    if (int rc = launch_check("k_search_units"))
-        return rc;
-    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
     if (gp) {
-        if (int rc = launch_guided<STEREO>(p, su, *gp, warps, stream, d_trace))
+        if (int rc = launch(k_search_estimate<TRACE>, warps, 32, 0, stream, "k_search_estimate", p, su, *gp))
             return rc;
-    } else {
-        if (d_trace)
-            k_search_candidates_trace<STEREO><<<warps, 32, smem_orders, stream>>>(p, su, d_trace);
-        else
-            k_search_candidates<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
-        if (int rc = launch_check("k_search_candidates"))
+        if (int rc = launch(k_search_listed<STEREO, TRACE>, warps, 32, smem_orders, stream, "k_search_listed", p, su, *gp,
+                            d_trace))
             return rc;
+    } else if (int rc = launch(k_search_candidates<STEREO, TRACE>, warps, 32, smem_orders, stream, "k_search_candidates",
+                               p, su, d_trace)) {
+        return rc;
     }
-    if (d_ref_words) {
-        k_search_ref_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, su, d_ref_words);
-        if (int rc = launch_check("k_search_ref_words"))
+    if (d_ref_words)
+        if (int rc = launch(k_search_ref_words, (n_frames + 255) / 256, 256, 0, stream, "k_search_ref_words", p, su,
+                            d_ref_words))
             return rc;
-    }
-    k_search_repack<STEREO><<<warps, 32, smem_orders, stream>>>(p, su);
-    return launch_check("k_search_repack");
+    return launch(k_search_repack<STEREO>, warps, 32, smem_orders, stream, "k_search_repack", p, su);
 }
 
 // The channel pairing (pairing.cuh) between the lossless repair and the scan: means, candidates, choice, and the
@@ -466,66 +416,42 @@ int launch_search(const EncodeParams &p, SearchUnit *su, size_t n_frames, size_t
 int launch_pairing(const EncodeParams &p, const PairingParams &q, size_t n_frames, size_t n_units, cudaStream_t stream)
 {
     constexpr size_t smem = encode_smem_bytes<true>();
-    if (int rc = set_smem(k_pairing_candidates, smem))
+    const size_t n_pairs = n_frames * p.channels * p.channels, warps = std::min(n_units, (size_t)g.sms * 32);
+    if (int rc = launch(k_pairing_means, (n_pairs + 127) / 128, 128, 0, stream, "k_pairing_means", p, q))
         return rc;
-    if (int rc = set_smem(k_pairing_repack, smem))
+    if (int rc = launch(k_pairing_candidates, warps, 32, smem, stream, "k_pairing_candidates", p, q))
         return rc;
-    const size_t n_pairs = n_frames * p.channels * p.channels;
-    k_pairing_means<<<(unsigned)((n_pairs + 127) / 128), 128, 0, stream>>>(p, q);
-    if (int rc = launch_check("k_pairing_means"))
+    if (int rc = launch(k_pairing_select, std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream, "k_pairing_select", p,
+                        q))
         return rc;
-    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
-    k_pairing_candidates<<<warps, 32, smem, stream>>>(p, q);
-    if (int rc = launch_check("k_pairing_candidates"))
-        return rc;
-    k_pairing_select<<<(unsigned)std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream>>>(p, q);
-    if (int rc = launch_check("k_pairing_select"))
-        return rc;
-    k_pairing_repack<<<warps, 32, smem, stream>>>(p, q);
-    return launch_check("k_pairing_repack");
+    return launch(k_pairing_repack, warps, 32, smem, stream, "k_pairing_repack", p, q);
 }
 
 // The search + pairing (search_pairing.cuh) between the order search and the scan: means, the candidates' analysis
 // and search, the table, the choice, and the winning differences packed at their searched orders in place of their
-// channels.  The warp kernels have grids of a fixed size, at most one residue row per unit of the batch.  d_trace:
-// the candidates' analysis and search kernels are their tracing instantiations (q.trace is d_trace).
+// channels.  The warp kernels have grids of a fixed size, at most one residue row per unit of the batch.  TRACE: the
+// candidates' analysis and search kernels are their tracing instantiations, which write to q.trace.
+template <bool TRACE>
 int launch_search_pairing(const EncodeParams &p, const PairingParams &q, SearchUnit *cand, size_t n_frames,
-                          size_t n_units, cudaStream_t stream, bool trace)
+                          size_t n_units, cudaStream_t stream)
 {
     constexpr size_t smem = encode_smem_bytes<true>(), smem_orders = search_smem_bytes<true>();
-    if (int rc = set_smem(trace ? k_search_pairing_units_trace : k_search_pairing_units, smem))
-        return rc;
-    if (int rc = trace ? set_smem(k_search_pairing_candidates_trace, smem_orders)
-                       : set_smem(k_search_pairing_candidates, smem_orders))
-        return rc;
-    if (int rc = set_smem(k_search_pairing_repack, smem_orders))
-        return rc;
+    const size_t n_pairs = n_frames * p.channels * p.channels, warps = std::min(n_units, (size_t)g.sms * 32);
     CUDA_TRY(cudaMemsetAsync(q.stale, 0, n_frames * sizeof(uint32_t), stream)); // every searched unit is tie-free
-    const size_t n_pairs = n_frames * p.channels * p.channels;
-    k_pairing_means<<<(unsigned)((n_pairs + 127) / 128), 128, 0, stream>>>(p, q);
-    if (int rc = launch_check("k_pairing_means"))
+    if (int rc = launch(k_pairing_means, (n_pairs + 127) / 128, 128, 0, stream, "k_pairing_means", p, q))
         return rc;
-    const unsigned warps = (unsigned)std::min(n_units, (size_t)g.sms * 32);
-    if (trace)
-        k_search_pairing_units_trace<<<warps, 32, smem, stream>>>(p, q, cand);
-    else
-        k_search_pairing_units<<<warps, 32, smem, stream>>>(p, q, cand);
-    if (int rc = launch_check("k_search_pairing_units"))
+    if (int rc = launch(k_search_pairing_units<TRACE>, warps, 32, smem, stream, "k_search_pairing_units", p, q, cand))
         return rc;
-    if (trace)
-        k_search_pairing_candidates_trace<<<warps, 32, smem_orders, stream>>>(p, cand, q.trace);
-    else
-        k_search_pairing_candidates<<<warps, 32, smem_orders, stream>>>(p, cand);
-    if (int rc = launch_check("k_search_pairing_candidates"))
+    if (int rc = launch(k_search_pairing_candidates<TRACE>, warps, 32, smem_orders, stream,
+                        "k_search_pairing_candidates", p, cand, q.trace))
         return rc;
-    k_search_pairing_table<<<(unsigned)((n_pairs + 255) / 256), 256, 0, stream>>>(p, q, cand);
-    if (int rc = launch_check("k_search_pairing_table"))
+    if (int rc = launch(k_search_pairing_table, (n_pairs + 255) / 256, 256, 0, stream, "k_search_pairing_table", p, q,
+                        cand))
         return rc;
-    k_pairing_select<<<(unsigned)std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream>>>(p, q);
-    if (int rc = launch_check("k_pairing_select"))
+    if (int rc = launch(k_pairing_select, std::min(n_frames, (size_t)g.sms * 16), 128, 0, stream, "k_pairing_select", p,
+                        q))
         return rc;
-    k_search_pairing_repack<<<warps, 32, smem_orders, stream>>>(p, q, cand);
-    return launch_check("k_search_pairing_repack");
+    return launch(k_search_pairing_repack, warps, 32, smem_orders, stream, "k_search_pairing_repack", p, q, cand);
 }
 
 // The window table of the window search (DESIGN.md 7.6), computed once on the host: row i is the window of mask bit
@@ -568,37 +494,23 @@ int check_windows(uint32_t windows)
 // The window search (window.cuh) after the order search and before the scan: the order search's words added to
 // *d_base_words, the window analyses, their candidates, and the units whose best window candidate has strictly fewer
 // words repacked.  su: the order search's SearchUnits.  The warp kernels have grids of a fixed size, the candidate
-// and repack kernels at most one residue row per unit of the batch.  trace: the candidate kernel is its tracing
+// and repack kernels at most one residue row per unit of the batch.  TRACE: the candidate kernel is its tracing
 // instantiation (wp.trace).
-template <bool STEREO>
+template <bool STEREO, bool TRACE>
 int launch_windows(const EncodeParams &p, const WindowParams &wp, const SearchUnit *su, size_t n_frames,
-                   size_t n_units, unsigned long long *d_base_words, cudaStream_t stream, bool trace)
+                   size_t n_units, unsigned long long *d_base_words, cudaStream_t stream)
 {
     constexpr size_t smem = encode_smem_bytes<STEREO>(), smem_orders = search_smem_bytes<STEREO>();
-    if (int rc = set_smem(k_window_units<STEREO>, smem))
-        return rc;
-    if (int rc = trace ? set_smem(k_window_candidates<STEREO, true>, smem_orders)
-                       : set_smem(k_window_candidates<STEREO, false>, smem_orders))
-        return rc;
-    if (int rc = set_smem(k_window_repack<STEREO>, smem_orders))
-        return rc;
-    k_window_base_words<<<(unsigned)((n_frames + 255) / 256), 256, 0, stream>>>(p, d_base_words);
-    if (int rc = launch_check("k_window_base_words"))
+    const size_t cap = (size_t)g.sms * 32, warps = std::min(n_units, cap);
+    if (int rc = launch(k_window_base_words, (n_frames + 255) / 256, 256, 0, stream, "k_window_base_words", p,
+                        d_base_words))
         return rc;
     CUDA_TRY(cudaMemsetAsync(wp.key, 0xff, n_units * sizeof(unsigned long long), stream));
-    const size_t cap = (size_t)g.sms * 32;
-    k_window_units<STEREO><<<(unsigned)std::min(n_units * wp.n, cap), 32, smem, stream>>>(p, wp);
-    if (int rc = launch_check("k_window_units"))
+    if (int rc = launch(k_window_units<STEREO>, std::min(n_units * wp.n, cap), 32, smem, stream, "k_window_units", p, wp))
         return rc;
-    const unsigned warps = (unsigned)std::min(n_units, cap);
-    if (trace)
-        k_window_candidates<STEREO, true><<<warps, 32, smem_orders, stream>>>(p, wp);
-    else
-        k_window_candidates<STEREO, false><<<warps, 32, smem_orders, stream>>>(p, wp);
-    if (int rc = launch_check("k_window_candidates"))
+    if (int rc = launch(k_window_candidates<STEREO, TRACE>, warps, 32, smem_orders, stream, "k_window_candidates", p, wp))
         return rc;
-    k_window_repack<STEREO><<<warps, 32, smem_orders, stream>>>(p, wp, su);
-    return launch_check("k_window_repack");
+    return launch(k_window_repack<STEREO>, warps, 32, smem_orders, stream, "k_window_repack", p, wp, su);
 }
 
 // Which encoder an encode call runs.  lossless: re-code every subframe the reference decoder would not reproduce
@@ -727,6 +639,73 @@ struct EncodeOptions {
     double *d_estimates = nullptr;                   // search_guided, with d_search_trace: every unit's E[100]
 };
 
+// The launches of encode mode o.mode up to the scan: the units' means, then the mode's kernels in place of
+// k_encode_units.  STEREO: two channels, three units per frame.  FORCE: o.d_pred is set.  TRACE: o.d_trace or
+// o.d_search_trace is set.  q: the pairing's tables (pairing, search_pairing).
+template <bool STEREO, bool FORCE, bool TRACE>
+int launch_encoder(const EncodeOptions &o, const EncodeLayout &l, char *ws, const EncodeParams &p,
+                   const PairingParams &q, uint32_t n_windows, cudaStream_t stream)
+{
+    const size_t n_frames = p.n_frames, n_units = encode_units(p.n_frames, p.channels);
+    if (int rc = launch_unit_means<STEREO ? kMeanStereo : kMeanPcm>(p.pcm, n_units, p.channels, p.means, stream))
+        return rc;
+    SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
+    switch (o.mode) {
+    case EncodeMode::plain:
+        return launch(k_encode_units<STEREO, TRACE>, n_units, 32, encode_smem_bytes<STEREO>(), stream, "k_encode_units",
+                      p, o.d_trace, nullptr);
+    case EncodeMode::lossless:
+    case EncodeMode::pairing: {
+        const bool pairing = o.mode == EncodeMode::pairing;
+        const LosslessArgs la = pairing ? LosslessArgs{} : o.lossless; // the pairing's base takes no report
+        RepairParams r;
+        r.count = reinterpret_cast<uint32_t *>(ws + l.repair_count);
+        r.frames = reinterpret_cast<uint32_t *>(ws + l.repair_frames);
+        r.orig = reinterpret_cast<UnitRecord *>(ws + l.repair_orig);
+        r.units = reinterpret_cast<RepairUnit *>(ws + l.repair_units);
+        r.entries = la.entries;
+        r.n_entries = la.n_entries;
+        r.frame_base = la.frame_base;
+        CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
+        if (int rc = launch_lossless<STEREO, FORCE>(p, r, n_frames, n_units, stream, o.d_pred, pairing ? &q : nullptr))
+            return rc;
+        return pairing ? launch_pairing(p, q, n_frames, n_units, stream) : 0;
+    }
+    case EncodeMode::search:
+    case EncodeMode::search_guided: {
+        GuidedParams gp{o.candidates, reinterpret_cast<uint4 *>(ws + l.masks), o.d_estimates};
+        return launch_search<STEREO, FORCE, TRACE>(p, su, n_frames, n_units, o.d_ref_words, stream, o.d_pred,
+                                                   o.d_search_trace, o.mode == EncodeMode::search_guided ? &gp : nullptr);
+    }
+    // the base of a search + pairing or a window search takes no reference words and no trace (its candidates are
+    // traced)
+    case EncodeMode::search_pairing:
+        if (int rc = launch_search<STEREO, FORCE, false>(p, su, n_frames, n_units, nullptr, stream, o.d_pred, nullptr,
+                                                         nullptr))
+            return rc;
+        return launch_search_pairing<TRACE>(p, q, reinterpret_cast<SearchUnit *>(ws + l.pair_search), n_frames, n_units,
+                                            stream);
+    case EncodeMode::search_windows: {
+        if (int rc = launch_search<STEREO, FORCE, false>(p, su, n_frames, n_units, nullptr, stream, o.d_pred, nullptr,
+                                                         nullptr))
+            return rc;
+        WindowParams wp;
+        wp.table = o.d_windows ? o.d_windows : g.windows;
+        wp.mask = o.windows;
+        wp.n = n_windows;
+        wp.su = reinterpret_cast<SearchUnit *>(ws + l.window_search);
+        wp.key = reinterpret_cast<unsigned long long *>(ws + l.window_keys);
+        wp.n_window = o.d_n_window;
+        wp.pred = o.d_window_pred;
+        wp.trace = o.d_search_trace;
+        return launch_windows<STEREO, TRACE>(p, wp, su, n_frames, n_units, o.d_base_words, stream);
+    }
+    }
+    return 0;
+}
+using EncodeLaunch = int (*)(const EncodeOptions &, const EncodeLayout &, char *, const EncodeParams &,
+                             const PairingParams &, uint32_t, cudaStream_t);
+
 int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, selab200_subframe_desc *d_descs,
                   uint32_t *d_words, size_t capacity, uint64_t *d_used, int32_t *d_status, void *d_ws,
                   size_t ws_bytes, cudaStream_t stream, const EncodeOptions &o = EncodeOptions())
@@ -771,8 +750,6 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     }
     if (n_frames == 0)
         return 0;
-    const bool stereo = channels == 2;
-    const size_t n_units = encode_units(n_frames, channels);
     char *ws = static_cast<char *>(d_ws);
     EncodeParams p;
     p.pcm = d_pcm;
@@ -787,9 +764,6 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
     p.slots = reinterpret_cast<uint32_t *>(ws + l.slots);
     p.means = reinterpret_cast<double *>(ws + l.means);
     p.residues = reinterpret_cast<int32_t *>(ws + l.residues);
-    if (int rc = stereo ? launch_unit_means<kMeanStereo>(d_pcm, n_units, channels, p.means, stream)
-                        : launch_unit_means<kMeanPcm>(d_pcm, n_units, channels, p.means, stream))
-        return rc;
     PairingParams q{};
     if (pairing) {
         q.table = reinterpret_cast<PairRecord *>(ws + l.pair_table);
@@ -801,97 +775,35 @@ int encode_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels, se
         q.pred = o.d_pair_pred;
         q.trace = o.d_search_trace;
     }
-    const PairingParams *pq = pairing ? &q : nullptr;
-    if (o.mode == EncodeMode::lossless || o.mode == EncodeMode::pairing) {
-        const LosslessArgs la = pairing ? LosslessArgs{} : o.lossless; // the pairing's base takes no report
-        RepairParams r;
-        r.count = reinterpret_cast<uint32_t *>(ws + l.repair_count);
-        r.frames = reinterpret_cast<uint32_t *>(ws + l.repair_frames);
-        r.orig = reinterpret_cast<UnitRecord *>(ws + l.repair_orig);
-        r.units = reinterpret_cast<RepairUnit *>(ws + l.repair_units);
-        r.entries = la.entries;
-        r.n_entries = la.n_entries;
-        r.frame_base = la.frame_base;
-        CUDA_TRY(cudaMemsetAsync(r.count, 0, 2 * sizeof(uint32_t), stream));
-        const selab200_predictor *pr = o.d_pred;
-        const int rc = pr ? (stereo ? launch_lossless<true, true>(p, r, n_frames, n_units, stream, pr, pq)
-                                    : launch_lossless<false, true>(p, r, n_frames, n_units, stream, pr, pq))
-                          : (stereo ? launch_lossless<true>(p, r, n_frames, n_units, stream, nullptr, pq)
-                                    : launch_lossless<false>(p, r, n_frames, n_units, stream, nullptr, pq));
-        if (rc)
-            return rc;
-        if (pairing)
-            if (int rc = launch_pairing(p, q, n_frames, n_units, stream))
-                return rc;
-    } else if (o.mode == EncodeMode::search || search_pairing || search_windows || search_guided) {
-        // the base of a search + pairing or a window search takes no reference words and no trace (its candidates
-        // are traced)
-        SearchUnit *su = reinterpret_cast<SearchUnit *>(ws + l.search);
-        const bool base = search_pairing || search_windows;
-        unsigned long long *rw = base ? nullptr : o.d_ref_words;
-        selab200_search_trace *tr = base ? nullptr : o.d_search_trace;
-        GuidedParams gp{o.candidates, reinterpret_cast<uint4 *>(ws + l.masks), o.d_estimates};
-        const GuidedParams *pg = search_guided ? &gp : nullptr;
-        const int rc = o.d_pred ? (stereo ? launch_search<true, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr, pg)
-                                          : launch_search<false, true>(p, su, n_frames, n_units, rw, stream, o.d_pred, tr, pg))
-                                : (stereo ? launch_search<true>(p, su, n_frames, n_units, rw, stream, nullptr, tr, pg)
-                                          : launch_search<false>(p, su, n_frames, n_units, rw, stream, nullptr, tr, pg));
-        if (rc)
-            return rc;
-        if (search_pairing)
-            if (int rc = launch_search_pairing(p, q, reinterpret_cast<SearchUnit *>(ws + l.pair_search), n_frames,
-                                               n_units, stream, o.d_search_trace != nullptr))
-                return rc;
-        if (search_windows) {
-            WindowParams wp;
-            wp.table = o.d_windows ? o.d_windows : g.windows;
-            wp.mask = o.windows;
-            wp.n = n_windows;
-            wp.su = reinterpret_cast<SearchUnit *>(ws + l.window_search);
-            wp.key = reinterpret_cast<unsigned long long *>(ws + l.window_keys);
-            wp.n_window = o.d_n_window;
-            wp.pred = o.d_window_pred;
-            wp.trace = o.d_search_trace;
-            const bool trace = o.d_search_trace != nullptr;
-            if (int rc = stereo ? launch_windows<true>(p, wp, su, n_frames, n_units, o.d_base_words, stream, trace)
-                                : launch_windows<false>(p, wp, su, n_frames, n_units, o.d_base_words, stream, trace))
-                return rc;
-        }
-    } else {
-        const int rc_units = stereo ? (o.d_trace ? launch_encode_units<true, true>(p, n_units, o.d_trace, stream)
-                                                 : launch_encode_units<true, false>(p, n_units, nullptr, stream))
-                                    : (o.d_trace ? launch_encode_units<false, true>(p, n_units, o.d_trace, stream)
-                                                 : launch_encode_units<false, false>(p, n_units, nullptr, stream));
-        if (rc_units)
-            return rc_units;
-    }
-    const unsigned scan_ctas = (unsigned)((n_sub + kScanTile - 1) / kScanTile);
-    k_encode_sizes<<<scan_ctas, kScanTile, 0, stream>>>(p);
-    if (int rc = launch_check("k_encode_sizes"))
+    // the one place where the call's stereo layout, forced predictors and trace buffer become template arguments
+    constexpr EncodeLaunch kLaunch[8] = {
+        launch_encoder<false, false, false>, launch_encoder<false, false, true>, launch_encoder<false, true, false>,
+        launch_encoder<false, true, true>,   launch_encoder<true, false, false>, launch_encoder<true, false, true>,
+        launch_encoder<true, true, false>,   launch_encoder<true, true, true>};
+    const bool force = o.d_pred != nullptr, trace = o.d_trace || o.d_search_trace;
+    if (int rc = kLaunch[(channels == 2) * 4 + force * 2 + trace](o, l, ws, p, q, n_windows, stream))
+        return rc;
+    const size_t scan_ctas = (n_sub + kScanTile - 1) / kScanTile;
+    if (int rc = launch(k_encode_sizes, scan_ctas, kScanTile, 0, stream, "k_encode_sizes", p))
         return rc;
     if (o.before_scan)
         CUDA_TRY(cudaStreamWaitEvent(stream, o.before_scan, 0));
-    k_encode_scan<<<scan_ctas, kScanTile, 0, stream>>>(p);
-    if (int rc = launch_check("k_encode_scan"))
+    if (int rc = launch(k_encode_scan, scan_ctas, kScanTile, 0, stream, "k_encode_scan", p))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(d_used, p.residues, 8, cudaMemcpyDeviceToDevice, stream)); // the new fill level (see k_encode_scan)
-    if (pairing) {
-        k_pairing_patch<<<(unsigned)((n_sub + 255) / 256), 256, 0, stream>>>(p, q);
-        if (int rc = launch_check("k_pairing_patch"))
+    if (pairing)
+        if (int rc = launch(k_pairing_patch, (n_sub + 255) / 256, 256, 0, stream, "k_pairing_patch", p, q))
             return rc;
-    }
     // The fill level this chunk leaves behind must be captured BEFORE the next chunk's scan (on the
     // other compute lane) may overwrite *d_used: copy it out now and only then release the event.
     if (o.h_fill_after)
         CUDA_TRY(cudaMemcpyAsync(o.h_fill_after, d_used, 8, cudaMemcpyDeviceToHost, stream));
     if (o.after_scan)
         CUDA_TRY(cudaEventRecord(o.after_scan, stream));
-    if (o.d_container) { // byte-packed .sela stream instead of the word arena
-        k_encode_gather_container<<<(unsigned)((n_sub + 7) / 8), 256, 0, stream>>>(p, o.d_container, o.sub_base);
-        return launch_check("k_encode_gather_container");
-    }
-    k_encode_gather<<<(unsigned)((n_sub + 7) / 8), 256, 0, stream>>>(p);
-    return launch_check("k_encode_gather");
+    if (o.d_container) // byte-packed .sela stream instead of the word arena
+        return launch(k_encode_gather_container, (n_sub + 7) / 8, 256, 0, stream, "k_encode_gather_container", p,
+                      o.d_container, o.sub_base);
+    return launch(k_encode_gather, (n_sub + 7) / 8, 256, 0, stream, "k_encode_gather", p);
 }
 
 // K5 launch: 64-word rings (8.3 KB per warp), eight parser steps per batch.

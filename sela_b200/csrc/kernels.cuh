@@ -273,6 +273,68 @@ __device__ __noinline__ void search_trace_record(selab200_search_trace *trace, u
     __syncwarp();
 }
 
+// ---- the coding tail of every warp that codes a unit (encode_unit, pair_unit in pairing.cuh, search_orders in
+// search.cuh) ----
+
+// The residue row res is dead.  It only ever lived in L2 (written and re-read by this warp within microseconds); tell
+// L2 to drop the dirty lines instead of writing 8 KB back to HBM.
+__device__ __forceinline__ void discard_row(int32_t *res)
+{
+    __syncwarp();
+    for (int l = lane_id(); l < kFrame * 4 / 128; l += 32)
+        asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
+}
+
+// Every q of an analysis into dst[0..100) for the order search: from k[] (still intact), or as forced (cf.q).
+__device__ __forceinline__ void copy_every_q(int32_t *dst, const CoefSmem &cf, AnalysisScratch &scratch, bool forced)
+{
+    for (int i = lane_id(); i < kMaxOrder; i += 32)
+        dst[i] = forced ? cf.q[i] : quantise_reflection(i, scratch.kk()[i]);
+    __syncwarp();
+}
+
+// The predictor q[0..order) and the residue row Rice-packed into the slot of unit `unit`, if both fit; returns
+// whether they do not (flag 1 of the record).
+__device__ __forceinline__ bool pack_slot(const EncodeParams &p, uint32_t unit, const int32_t *q, int order,
+                                          const int32_t *res, RiceChoice cq, RiceChoice cr)
+{
+    const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
+    uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
+    if (!too_large) {
+        warp_rice_pack(q, order, cq, slot);
+        warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
+    }
+    return too_large;
+}
+
+// Lane 0 writes the record of unit `unit`.
+__device__ __forceinline__ void write_record(const EncodeParams &p, uint32_t unit, int order, RiceChoice cq,
+                                             RiceChoice cr, uint32_t flags)
+{
+    if (lane_id() == 0) {
+        UnitRecord u;
+        u.order = order;
+        u.refl_k = cq.k;
+        u.refl_words = cq.words;
+        u.res_k = cr.k;
+        u.res_words = cr.words;
+        u.flags = flags;
+        u.pad[0] = u.pad[1] = 0;
+        p.units[unit] = u;
+    }
+}
+
+// Lane 0 writes the reference order's entry of a search record: the order, its words, and as the best so far that
+// order (key words << 8 | 0), if it has no tie.
+__device__ __forceinline__ void write_search_ref(SearchUnit &s, int order, RiceChoice cq, RiceChoice cr, bool tie)
+{
+    if (lane_id() == 0) {
+        s.ref_order = order;
+        s.ref_words = cq.words + cr.words;
+        s.best = tie ? kNoCandidate : (unsigned long long)(cq.words + cr.words) << 8;
+    }
+}
+
 // What encode_unit does with the unit:
 //   kUnitEncode     analyse, FIR, Rice, pack into the unit's slot and write its record (production)
 //   kUnitCheck      kUnitEncode, and bit 1 of the record's flags when the FIR has a tie
@@ -459,11 +521,8 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
         if (lane == 0)
             tr.order = order;
     }
-    if constexpr (MODE == kUnitSearch) { // every q, from k[] (still intact) or as forced
-        for (int i = lane; i < kMaxOrder; i += 32)
-            su[unit].q[i] = FORCE ? cf.q[i] : quantise_reflection(i, scratch.kk()[i]);
-        __syncwarp();
-    }
+    if constexpr (MODE == kUnitSearch)
+        copy_every_q(su[unit].q, cf, scratch, FORCE);
     // the digit planes of the FIR overlay k[] and the step-up row, dead now (the trace has copied k)
     static_assert(kPlaneBytes <= kCoefAlias, "FIR digit planes");
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring);
@@ -480,43 +539,18 @@ __device__ __forceinline__ void encode_unit(const EncodeParams &p, selab200_anal
     if constexpr (TRACE && MODE == kUnitSearch)
         search_trace_record(strace, unit, order, cf, res, tie, cq, cr);
     if constexpr (MODE == kUnitCandidate) {
-        __syncwarp();
-        for (int l = lane; l < kFrame * 4 / 128; l += 32)
-            asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
+        discard_row(res);
         const unsigned long long round = cand >= (uint32_t)repair_round1(ru->order) ? 1ull : 0ull;
         if (lane == 0 && !tie)
             atomicMin(&ru->best, round << 63 | (unsigned long long)(cq.words + cr.words) << 32 | cand);
         return;
     }
-    const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
-    uint32_t *slot = p.slots + (size_t)unit * kSlotWords;
-    if (!too_large) {
-        warp_rice_pack(cf.q, order, cq, slot);
-        warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
-    }
-    // The residue row is dead now.  It only ever lived in L2 (written and re-read by this warp
-    // within microseconds); tell L2 to drop the dirty lines instead of writing 8 KB per unit back
-    // to HBM.
-    __syncwarp();
-    for (int l = lane; l < kFrame * 4 / 128; l += 32)
-        asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
-    if (lane == 0) {
-        UnitRecord u;
-        u.order = order;
-        u.refl_k = cq.k;
-        u.refl_words = cq.words;
-        u.res_k = cr.k;
-        u.res_words = cr.words;
-        u.flags = (too_large ? 1u : 0u) | (MODE != kUnitSearch && tie ? 2u : 0u); // 2: not lossless (kUnitCheck only)
-        u.pad[0] = u.pad[1] = 0;
-        p.units[unit] = u;
-        if constexpr (MODE == kUnitSearch) {
-            SearchUnit &s = su[unit];
-            s.ref_order = order;
-            s.ref_words = cq.words + cr.words;
-            s.best = tie ? kNoCandidate : (unsigned long long)(cq.words + cr.words) << 8;
-        }
-    }
+    const bool too_large = pack_slot(p, unit, cf.q, order, res, cq, cr);
+    discard_row(res);
+    // flag 2: not lossless (kUnitCheck only)
+    write_record(p, unit, order, cq, cr, (too_large ? 1u : 0u) | (MODE != kUnitSearch && tie ? 2u : 0u));
+    if constexpr (MODE == kUnitSearch)
+        write_search_ref(su[unit], order, cq, cr, tie);
 }
 
 // k_encode_units: encode_unit for unit blockIdx.x.  CHECK: the kUnitCheck instantiation (lossless encodes).

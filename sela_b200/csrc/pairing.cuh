@@ -122,11 +122,8 @@ __device__ __forceinline__ void pair_unit(const EncodeParams &p, const PairingPa
         __syncwarp();
     }
     warp_coefficients(cf, scratch.t(), order);
-    if constexpr (SEARCH) { // every q, from k[] (still intact) or as forced
-        for (int i = lane; i < kMaxOrder; i += 32)
-            su[idx].q[i] = q.pred ? cf.q[i] : quantise_reflection(i, scratch.kk()[i]);
-        __syncwarp();
-    }
+    if constexpr (SEARCH)
+        copy_every_q(su[idx].q, cf, scratch, q.pred != nullptr);
     uint32_t *planes = reinterpret_cast<uint32_t *>(scratch.ring); // over k[] and the step-up row, dead now
     const bool tie = warp_fir_residual<true, !PACK>(sig, cf, order, planes, res);
     const RiceChoice cq = warp_rice_choose(cf.q, order);
@@ -134,12 +131,7 @@ __device__ __forceinline__ void pair_unit(const EncodeParams &p, const PairingPa
     if constexpr (SEARCH) {
         if constexpr (TRACE)
             search_trace_record(q.trace, (uint32_t)idx, order, cf, res, tie, cq, cr);
-        if (lane == 0) {
-            SearchUnit &s = su[idx];
-            s.ref_order = order;
-            s.ref_words = cq.words + cr.words;
-            s.best = tie ? kNoCandidate : (unsigned long long)(cq.words + cr.words) << 8;
-        }
+        write_search_ref(su[idx], order, cq, cr, tie);
     } else if constexpr (!PACK) {
         if (q.trace) {
             search_trace_record(q.trace + idx, 0, 1, cf, res, tie, cq, cr);
@@ -158,33 +150,10 @@ __device__ __forceinline__ void pair_unit(const EncodeParams &p, const PairingPa
             q.table[idx] = r;
         }
     } else {
-        const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
-        if (!too_large) {
-            uint32_t *slot = p.slots + (size_t)out * kSlotWords;
-            warp_rice_pack(cf.q, order, cq, slot);
-            warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
-        }
-        if (lane == 0) {
-            UnitRecord u;
-            u.order = order;
-            u.refl_k = cq.k;
-            u.refl_words = cq.words;
-            u.res_k = cr.k;
-            u.res_words = cr.words;
-            u.flags = too_large ? 1u : 0u;
-            u.pad[0] = u.pad[1] = 0;
-            p.units[out] = u;
-        }
+        const bool too_large = pack_slot(p, out, cf.q, order, res, cq, cr);
+        write_record(p, out, order, cq, cr, too_large ? 1u : 0u);
     }
     __syncwarp();
-}
-
-// The warp's residue row only ever lived in L2.
-__device__ __forceinline__ void discard_row(int32_t *res)
-{
-    __syncwarp();
-    for (int l = lane_id(); l < kFrame * 4 / 128; l += 32)
-        asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
 }
 
 // Work item w = (frame, p, c) in that order: the candidates of a frame go to neighbouring warps, which read the same

@@ -1,10 +1,10 @@
 // search.cuh -- the kernels of the order search (sm_90a, DESIGN.md 7.3): every unit is coded at the predictor order
 // 1..100 with the fewest words whose FIR has no tie, inside the format.
 //
-//   k_search_units<S, FORCE>   the ordinary analysis kernel (encode_unit<kUnitSearch>): codes the unit at the
+//   k_search_units<S, T, FORCE>  the ordinary analysis kernel (encode_unit<kUnitSearch>): codes the unit at the
 //                              reference order into its slot, and leaves all 100 q, the reference order and its words
 //                              in the unit's SearchUnit
-//   k_search_candidates<S>     warp per (unit, slice of orders): carries one step-up forward through the slice's
+//   k_search_candidates<S, T>  warp per (unit, slice of orders): carries one step-up forward through the slice's
 //                              orders; per order the FIR with the tie check and both Rice sizes; a tie-free order
 //                              enters the unit's atomicMin key
 //   k_search_repack<S>         warp per unit whose winner is not the reference order: the winner packed into the
@@ -13,8 +13,8 @@
 //                              stereo decision), summed into one counter
 // Then k_encode_sizes / k_encode_scan / k_encode_gather(_container) run as for every encode, and the stereo decision
 // there sees the searched sizes.  The candidate and repack kernels have grids of a fixed size and loop over the work.
-// k_search_units_trace and k_search_candidates_trace (tests only, selab200_encode_search_trace) also write the record
-// of every (unit, order) to a trace buffer.
+// T (tests only, selab200_encode_search_trace): the tracing instantiations, which also write the record of every
+// (unit, order) to a trace buffer.
 #pragma once
 
 #include "kernels.cuh"
@@ -62,22 +62,29 @@ __device__ __forceinline__ void step_up(double *t, int i, int q)
     __syncwarp();
 }
 
+// What search_orders sizes or packs (see there).
+enum { kOrdersUnit = 0, kOrdersPair = 1, kOrdersWindow = 2, kOrdersListed = 3 };
+
 // Unit `unit` at the orders o_lo..o_hi, one after the other, on one carried step-up.  The order-1 predictor is zero
 // (linear_predictor.cpp:19-22), not row 0 of the step-up.  res: the warp's residue row.
 //   PACK = false  every order but the reference order (the analysis kernel has sized that one): FIR with the tie
 //                 check, Rice sizes, a tie-free order into su[unit].best
 //   PACK = true   (o_lo = o_hi) FIR, Rice, pack into the unit's slot and rewrite its record
 // TRACE (PACK = false, tests only, selab200_encode_search_trace): each order's record into trace as well.
-// PAIR (search + pairing, search_pairing.cuh; STEREO = true for its shared memory layout): `unit` is the candidate
-// (frame, par, c) at ((frame * C + par) * C + c) of su and trace, its signal ch_par - ch_c from stage_pair, its FIR
-// always the wide one, and PACK packs into unit `out`.  Without PAIR, PACK packs into `unit` and `out` is unused.
-// WINDOW (window search, window.cuh): `unit` is the record (analysis unit u, window w) at u * n_win + w of su and
-// trace, its signal unit u's; a tie-free order enters wkey[u] as words << 16 | w << 8 | order, and PACK packs into u.
-// An order whose predictor leaves the domain of the int64 conversion (|2^35 t| >= 2^62, undefined in the reference;
-// a window's clamped q can get there) counts as tied: it is never eligible.
-// LISTED (PACK = false; guided order search, search_guided.cuh): only the orders whose bit o - 1 is set in
-// listed[unit] are sized; the step-up still runs through every order below the highest one sized.
-template <bool STEREO, bool PACK, bool TRACE = false, bool PAIR = false, bool WINDOW = false, bool LISTED = false>
+// KIND says what `unit` is:
+//   kOrdersUnit    (order search, this file) an analysis unit, at `unit` of su and trace
+//   kOrdersPair    (search + pairing, search_pairing.cuh; STEREO = true for its shared memory layout): the candidate
+//                  (frame, par, c) at ((frame * C + par) * C + c) of su and trace, its signal ch_par - ch_c from
+//                  stage_pair, its FIR always the wide one; PACK packs into unit `out`.  Other kinds leave `out` unused
+//   kOrdersWindow  (window search, window.cuh): the record (analysis unit u, window w) at u * n_win + w of su and
+//                  trace, its signal unit u's; a tie-free order enters wkey[u] as words << 16 | w << 8 | order, and
+//                  PACK packs into u.  An order whose predictor leaves the domain of the int64 conversion
+//                  (|2^35 t| >= 2^62, undefined in the reference; a window's clamped q can get there) counts as tied:
+//                  it is never eligible
+//   kOrdersListed  (PACK = false; guided order search, search_guided.cuh): an analysis unit, of which only the orders
+//                  whose bit o - 1 is set in listed[unit] are sized; the step-up still runs through every order below
+//                  the highest one sized
+template <int KIND, bool STEREO, bool PACK, bool TRACE = false>
 __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit *su, const uint32_t unit, int o_lo,
                                               int o_hi, int32_t *res, selab200_search_trace *trace = nullptr,
                                               uint32_t out = 0, uint32_t n_win = 1,
@@ -89,9 +96,9 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
     CoefSmem &cf = *reinterpret_cast<CoefSmem *>(smem_raw + kSigBytes + kSearchStepBytes);
     uint32_t *planes = reinterpret_cast<uint32_t *>(smem_raw + kSigBytes + kSearchStepBytes + sizeof(CoefSmem));
     static_assert(kSearchStepBytes % 16 == 0 && sizeof(CoefSmem) % 16 == 0, "search shared memory layout");
+    constexpr bool PAIR = KIND == kOrdersPair, WINDOW = KIND == kOrdersWindow, LISTED = KIND == kOrdersListed;
     static_assert(!PAIR || STEREO, "a pair is staged as the stereo difference is");
-    static_assert(!(PAIR && WINDOW), "one kind of record");
-    static_assert(!LISTED || !(PACK || PAIR || WINDOW), "a list of a unit's orders to size");
+    static_assert(!LISTED || !PACK, "a list of a unit's orders to size");
 
     const int lane = lane_id();
     const uint32_t src = WINDOW ? unit / n_win : unit; // the analysis unit whose signal is coded
@@ -158,74 +165,38 @@ __device__ __forceinline__ void search_orders(const EncodeParams &p, SearchUnit 
                     atomicMin(&s.best, words << 8 | (unsigned long long)o);
             }
         } else {
-            const bool too_large = cq.words > kSlotReflWords || cr.words > kSlotWords - kSlotReflWords;
-            if (!too_large) {
-                uint32_t *slot = p.slots + (size_t)dst * kSlotWords;
-                warp_rice_pack(cf.q, o, cq, slot);
-                warp_rice_pack(res, kFrame, cr, slot + kSlotReflWords);
-            }
-            if (lane == 0) {
-                UnitRecord u;
-                u.order = o;
-                u.refl_k = cq.k;
-                u.refl_words = cq.words;
-                u.res_k = cr.k;
-                u.res_words = cr.words;
-                u.flags = too_large ? 1u : 0u;
-                u.pad[0] = u.pad[1] = 0;
-                p.units[dst] = u;
-            }
+            const bool too_large = pack_slot(p, dst, cf.q, o, res, cq, cr);
+            write_record(p, dst, o, cq, cr, too_large ? 1u : 0u);
         }
         __syncwarp();
     }
 }
 
 // The search's analysis kernel: encode_unit for unit blockIdx.x.  FORCE and `pred` (tests only,
-// selab200_encode_search_forced): the unit's q[0..99] and reference order are pred[unit]'s.
-template <bool STEREO, bool FORCE = false>
-__global__ void __launch_bounds__(32) k_search_units(EncodeParams p, const selab200_predictor *pred, SearchUnit *su)
+// selab200_encode_search_forced): the unit's q[0..99] and reference order are pred[unit]'s.  TRACE (tests only,
+// selab200_encode_search_trace): the reference order's record into trace as well.
+template <bool STEREO, bool TRACE, bool FORCE = false>
+__global__ void __launch_bounds__(32) k_search_units(EncodeParams p, const selab200_predictor *pred, SearchUnit *su,
+                                                     selab200_search_trace *trace)
 {
-    encode_unit<STEREO, false, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su);
-}
-
-// Tests only (selab200_encode_search_trace): k_search_units, and the reference order's record into trace.
-template <bool STEREO, bool FORCE = false>
-__global__ void __launch_bounds__(32) k_search_units_trace(EncodeParams p, const selab200_predictor *pred,
-                                                           SearchUnit *su, selab200_search_trace *trace)
-{
-    encode_unit<STEREO, true, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su, trace);
+    encode_unit<STEREO, TRACE, kUnitSearch, FORCE>(p, nullptr, blockIdx.x, nullptr, 0, pred, su, trace);
 }
 
 // Work item w = (unit w / kSearchSlices, slice w % kSearchSlices): the slices of a unit go to neighbouring warps,
-// which read the same PCM.  Residue row = the warp's (the grid is at most the batch's units).
+// which read the same PCM.  Residue row = the warp's (the grid is at most the batch's units).  TRACE (tests only,
+// selab200_encode_search_trace): every order's record into trace as well.
 template <bool STEREO, bool TRACE>
-__device__ __forceinline__ void search_candidates(const EncodeParams &p, SearchUnit *su, selab200_search_trace *trace)
+__global__ void __launch_bounds__(32) k_search_candidates(EncodeParams p, SearchUnit *su, selab200_search_trace *trace)
 {
     const size_t work = (size_t)encode_units(p.n_frames, p.channels) * kSearchSlices;
     int32_t *res = p.residues + (size_t)blockIdx.x * kFrame;
     for (size_t w = blockIdx.x; w < work; w += gridDim.x) {
         const int sl = (int)(w % kSearchSlices);
         __syncwarp();
-        search_orders<STEREO, false, TRACE>(p, su, (uint32_t)(w / kSearchSlices), search_slice_first(sl),
-                                            search_slice_first(sl + 1) - 1, res, trace);
+        search_orders<kOrdersUnit, STEREO, false, TRACE>(p, su, (uint32_t)(w / kSearchSlices), search_slice_first(sl),
+                                                         search_slice_first(sl + 1) - 1, res, trace);
     }
-    __syncwarp();
-    for (int l = lane_id(); l < kFrame * 4 / 128; l += 32) // the row only ever lived in L2
-        asm volatile("discard.global.L2 [%0], 128;" ::"l"(res + l * 32) : "memory");
-}
-
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_search_candidates(EncodeParams p, SearchUnit *su)
-{
-    search_candidates<STEREO, false>(p, su, nullptr);
-}
-
-// Tests only (selab200_encode_search_trace): k_search_candidates, and every order's record into trace.
-template <bool STEREO>
-__global__ void __launch_bounds__(32) k_search_candidates_trace(EncodeParams p, SearchUnit *su,
-                                                                selab200_search_trace *trace)
-{
-    search_candidates<STEREO, true>(p, su, trace);
+    discard_row(res);
 }
 
 template <bool STEREO>
@@ -238,7 +209,7 @@ __global__ void __launch_bounds__(32) k_search_repack(EncodeParams p, SearchUnit
         if (o == 0 || o > kMaxOrder) // the reference order won (its slot and record stand); > 100: no tie-free
             continue;                // order, which cannot happen (order 1 has none)
         __syncwarp();
-        search_orders<STEREO, true>(p, su, u, o, o, res);
+        search_orders<kOrdersUnit, STEREO, true>(p, su, u, o, o, res);
     }
 }
 

@@ -14,7 +14,6 @@
 // the tracing instantiations, which write every unit's E[100] and the record of every order sized.
 #pragma once
 
-#include "pairing.cuh" // discard_row
 #include "search.cuh"
 
 namespace selab200 {
@@ -92,8 +91,8 @@ __global__ void __launch_bounds__(32) k_search_listed(EncodeParams p, SearchUnit
     int32_t *res = p.residues + (size_t)blockIdx.x * kFrame;
     for (uint32_t u = blockIdx.x; u < n; u += gridDim.x) {
         __syncwarp();
-        search_orders<STEREO, false, TRACE, false, false, true>(p, su, u, 1, kMaxOrder, res, trace, 0, 1, nullptr,
-                                                                gp.masks);
+        search_orders<kOrdersListed, STEREO, false, TRACE>(p, su, u, 1, kMaxOrder, res, trace, 0, 1, nullptr,
+                                                           gp.masks);
     }
     discard_row(res);
 }

@@ -7,7 +7,7 @@
 //                                   q, the reference order coded with the tie check, the candidate's SearchUnit and,
 //                                   if that order is tie-free, its key.  Nothing is packed.  Stereo (0, 1) is the
 //                                   base's searched unit 2 and is not run again
-//   k_search_pairing_candidates<T>  warp per (candidate, slice of orders): search_orders on the pair, as
+//   k_search_pairing_candidates<T>  warp per (candidate, slice of orders): search_orders<kOrdersPair>, as
 //                                   k_search_candidates runs it on a unit
 //   k_search_pairing_table          thread per (frame, p, c): the candidate's searched words into the PairRecord table
 //   k_pairing_select                unchanged: the valid assignment with the fewest words -> par[frame][C]
@@ -41,8 +41,9 @@ __device__ __forceinline__ uint32_t search_pairing_candidate(uint32_t C, size_t 
     return (f * C + par) * C + c;
 }
 
+// TRACE: the reference order's record into q.trace as well.
 template <bool TRACE>
-__device__ __forceinline__ void search_pairing_units(const EncodeParams &p, const PairingParams &q, SearchUnit *su)
+__global__ void __launch_bounds__(32) k_search_pairing_units(EncodeParams p, PairingParams q, SearchUnit *su)
 {
     const uint32_t C = p.channels;
     const size_t work = (size_t)p.n_frames * search_pairing_per_frame(C);
@@ -54,22 +55,12 @@ __device__ __forceinline__ void search_pairing_units(const EncodeParams &p, cons
     discard_row(res);
 }
 
-__global__ void __launch_bounds__(32) k_search_pairing_units(EncodeParams p, PairingParams q, SearchUnit *su)
-{
-    search_pairing_units<false>(p, q, su);
-}
-
-// Tests only (selab200_encode_search_pairing_trace): k_search_pairing_units, and the reference order's record.
-__global__ void __launch_bounds__(32) k_search_pairing_units_trace(EncodeParams p, PairingParams q, SearchUnit *su)
-{
-    search_pairing_units<true>(p, q, su);
-}
-
 // Work item w = (candidate w / kSearchSlices, slice w % kSearchSlices), candidates numbered densely in (frame, p, c)
 // order: the slices of a candidate and the candidates of a frame go to neighbouring warps, which read the same PCM.
+// TRACE: every order's record into trace as well.
 template <bool TRACE>
-__device__ __forceinline__ void search_pairing_candidates(const EncodeParams &p, SearchUnit *su,
-                                                          selab200_search_trace *trace)
+__global__ void __launch_bounds__(32) k_search_pairing_candidates(EncodeParams p, SearchUnit *su,
+                                                                  selab200_search_trace *trace)
 {
     const uint32_t C = p.channels;
     const size_t work = (size_t)p.n_frames * search_pairing_per_frame(C) * kSearchSlices;
@@ -78,22 +69,10 @@ __device__ __forceinline__ void search_pairing_candidates(const EncodeParams &p,
         const uint32_t idx = search_pairing_candidate(C, w / kSearchSlices);
         const int sl = (int)(w % kSearchSlices);
         __syncwarp();
-        search_orders<true, false, TRACE, true>(p, su, idx, search_slice_first(sl), search_slice_first(sl + 1) - 1,
-                                                res, trace);
+        search_orders<kOrdersPair, true, false, TRACE>(p, su, idx, search_slice_first(sl),
+                                                       search_slice_first(sl + 1) - 1, res, trace);
     }
     discard_row(res);
-}
-
-__global__ void __launch_bounds__(32) k_search_pairing_candidates(EncodeParams p, SearchUnit *su)
-{
-    search_pairing_candidates<false>(p, su, nullptr);
-}
-
-// Tests only (selab200_encode_search_pairing_trace): k_search_pairing_candidates, and every order's record.
-__global__ void __launch_bounds__(32) k_search_pairing_candidates_trace(EncodeParams p, SearchUnit *su,
-                                                                        selab200_search_trace *trace)
-{
-    search_pairing_candidates<true>(p, su, trace);
 }
 
 // The candidates' searched keys into the table (the PairRecord comment says what the fields hold).  Every candidate
@@ -131,7 +110,7 @@ __global__ void __launch_bounds__(32) k_search_pairing_repack(EncodeParams p, Pa
         const int key_order = (int)(su[idx].best & 0xffu); // 0: the reference order won
         const int o = key_order ? key_order : (int)su[idx].ref_order;
         __syncwarp();
-        search_orders<true, true, false, true>(p, su, idx, o, o, res, nullptr, pairing_unit(C, f, c));
+        search_orders<kOrdersPair, true, true>(p, su, idx, o, o, res, nullptr, pairing_unit(C, f, c));
         if (C == 2 && lane_id() == 0)
             p.units[(size_t)f * 3 + 2].res_words = kPairNone;
     }

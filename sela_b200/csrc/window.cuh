@@ -16,7 +16,6 @@
 // instantiation, which writes the record of every (unit, window, order) to trace at (unit * n + w) * 100 + order - 1.
 #pragma once
 
-#include "pairing.cuh" // discard_row
 #include "search.cuh"
 
 namespace selab200 {
@@ -96,9 +95,9 @@ __global__ void __launch_bounds__(32) k_window_candidates(EncodeParams p, Window
     for (size_t w = blockIdx.x; w < work; w += gridDim.x) {
         const int sl = (int)(w % kSearchSlices);
         __syncwarp();
-        search_orders<STEREO, false, TRACE, false, true>(p, wp.su, (uint32_t)(w / kSearchSlices),
-                                                         search_slice_first(sl), search_slice_first(sl + 1) - 1, res,
-                                                         wp.trace, 0, wp.n, wp.key);
+        search_orders<kOrdersWindow, STEREO, false, TRACE>(p, wp.su, (uint32_t)(w / kSearchSlices),
+                                                           search_slice_first(sl), search_slice_first(sl + 1) - 1, res,
+                                                           wp.trace, 0, wp.n, wp.key);
     }
     discard_row(res);
 }
@@ -115,9 +114,8 @@ __global__ void __launch_bounds__(32) k_window_repack(EncodeParams p, WindowPara
         if (key == kNoCandidate || (key >> 16) >= (su[u].best >> 8)) // no window strictly better: -S's bytes stand
             continue;
         __syncwarp();
-        search_orders<STEREO, true, false, false, true>(p, wp.su, u * wp.n + (uint32_t)((key >> 8) & 0xffu),
-                                                        (int)(key & 0xffu), (int)(key & 0xffu), res, nullptr, 0,
-                                                        wp.n);
+        search_orders<kOrdersWindow, STEREO, true>(p, wp.su, u * wp.n + (uint32_t)((key >> 8) & 0xffu),
+                                                   (int)(key & 0xffu), (int)(key & 0xffu), res, nullptr, 0, wp.n);
         count++;
     }
     discard_row(res);
