@@ -248,6 +248,40 @@ int selab200_container_decode_clips_device(selab200_container *const *handles, u
                                            const selab200_clip *clips, uint32_t n_clips, uint32_t length,
                                            int16_t *d_pcm_out, uint64_t *frames_decoded);
 
+/* Clips of chosen channels (DESIGN.md 7.9): the clips above, but only the channels select[0 .. n_select) (any order,
+ * repeats allowed; select == NULL with n_select == 0: every channel 0 .. C-1 of each clip's own container), and only
+ * the subframes those channels need are decoded.  With x the [length][C] rows of a clip as above, the output is
+ * [n_clips][length][n_out], clips back to back, n_out = 1 with SELAB200_CLIP_MEAN, else the number of channels
+ * selected:
+ *   int16 (flags 0):  out[t][j] = x[t][select[j]], bit for bit;
+ *   FLOAT32:          (float)x[t][select[j]] / 32768.0f (exact);
+ *   FLOAT32 | MEAN:   (float)S / (float)(32768 * n), IEEE round-to-nearest, S the exact integer sum of the n selected
+ *                     samples of the row (both operands exact: the value is defined to the last bit).
+ * Containers of different channel counts may share a call, except in a full selection without MEAN (n_out must be
+ * one count).  *frames_decoded is as above; *subframes_decoded receives the subframes decoded: per covered frame
+ * those of the selected channels and the parents of the selected difference-coded ones, each once.  A covered frame
+ * fails the call (SELAB200_ERR_BITSTREAM, before anything is decoded) when any of its subframe headers breaks the
+ * decoder's descriptor and frame rules, decoded or not; a stream that ends inside its words is found only in the
+ * subframes that are decoded, since only those streams are parsed.  SELAB200_ERR_ARGUMENT, with the clip index where
+ * one applies, for everything the clip call rejects (except handles of different channel counts), flag bits other
+ * than the two below, MEAN without FLOAT32, select == NULL with n_select != 0 or the reverse, n_select > 255, a
+ * selected channel >= the channel count of a container some clip reads, and a full selection without MEAN over
+ * clips of containers with different channel counts.  A rejected call writes no output. */
+#define SELAB200_CLIP_FLOAT32 1u   /* float32 output instead of int16                                    */
+#define SELAB200_CLIP_MEAN    2u   /* one output channel: the mean of the selected ones (needs FLOAT32) */
+#define SELAB200_CLIP_MAX_SELECT 255u
+
+/* host output: out holds n_clips * length * n_out int16 or float */
+int selab200_container_decode_clips_select(selab200_container *const *handles, uint32_t n_handles,
+                                           const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                           const uint8_t *select, uint32_t n_select, uint32_t flags, void *out,
+                                           uint64_t *frames_decoded, uint64_t *subframes_decoded);
+/* the same, into device memory of the primary device (2-byte aligned for int16, 4-byte for float32); synchronises */
+int selab200_container_decode_clips_select_device(selab200_container *const *handles, uint32_t n_handles,
+                                                  const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                                  const uint8_t *select, uint32_t n_select, uint32_t flags,
+                                                  void *d_out, uint64_t *frames_decoded, uint64_t *subframes_decoded);
+
 /* ------------------------------------------------------------- verify -- */
 
 /* The format is not lossless for every input: encoder and decoder round the Q35 prediction differently

@@ -70,6 +70,7 @@ assert SEARCH_UNIT_DTYPE.itemsize == 416
 # mirrors selab200_clip, 16 bytes
 CLIP_DTYPE = np.dtype([("container", "<u4"), ("reserved", "<u4"), ("start", "<u8")], align=True)
 assert CLIP_DTYPE.itemsize == 16
+CLIP_FLOAT32, CLIP_MEAN, CLIP_MAX_SELECT = 1, 2, 255   # selab200_container_decode_clips_select
 
 STATUS_NAMES = {0: "OK", -1: "NO_DEVICE", -2: "CUDA", -3: "ARGUMENT", -4: "CAPACITY", -5: "RANGE",
                 -6: "BITSTREAM", -7: "NOT_INIT"}
@@ -113,6 +114,8 @@ _SIGNATURES = {
     "selab200_container_close": (None, [_V]),
     "selab200_container_decode_clips": (_I, [_V, _U32, _V, _U32, _U32, _V, _V]),
     "selab200_container_decode_clips_device": (_I, [_V, _U32, _V, _U32, _U32, _V, _V]),
+    "selab200_container_decode_clips_select": (_I, [_V, _U32, _V, _U32, _U32, _V, _U32, _U32, _V, _V, _V]),
+    "selab200_container_decode_clips_select_device": (_I, [_V, _U32, _V, _U32, _U32, _V, _U32, _U32, _V, _V, _V]),
     "selab200_verify_workspace_bytes": (_SZ, [_U32, _U32]),
     "selab200_verify_frames_device": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _V, _V, _V, _SZ, _V]),
     "selab200_verify_frames": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _SZ, _V]),

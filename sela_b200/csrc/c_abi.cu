@@ -110,6 +110,7 @@ struct Context {
     DeviceBuffer verify;                           // verify paths: count, status, per-pair records (VerifyArea)
     DeviceBuffer lossless;                         // lossless host paths: count, per-pair records of re-coded subframes
     DeviceBuffer clip_src, clip_pieces, clip_out;  // clip decode: source addresses, gather pieces, host-form staging
+    DeviceBuffer clip_rows;                        // channel-selecting clip decode: the gather's row table
     Counters *h_small = nullptr;                   // pinned: where g.small's counters come down
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
@@ -1128,6 +1129,7 @@ static void shutdown_slot()
     g.clip_src.release();
     g.clip_pieces.release();
     g.clip_out.release();
+    g.clip_rows.release();
     g.small.release();
     if (g.h_small)
         cudaFreeHost(g.h_small);
@@ -2732,6 +2734,234 @@ static int decode_clips(selab200_container *const *handles, uint32_t n_handles, 
     return 0;
 }
 
+// ---- channel-selecting clip decode (DESIGN.md 7.9) ---------------------------------------------------------------
+//
+// The selection of decode_clips, flattened: every subframe a covered frame needs -- its selected channels and the
+// parents of the selected difference-coded ones -- becomes one mono frame of a ClipSelection, in file order, with
+// channel, type and parent 0.  decode_pipeline decodes a group of them with channels = 1 into [n][2048] int16 rows (an
+// independent subframe's samples, a difference subframe's difference, both mod 2^16 as in the full decode), and
+// k_clip_gather_select cuts the clips out of the rows through a row table: per covered frame and selected channel the
+// row of its subframe and, for a difference-coded one, the row of its parent.  A frame's subframes stay in one group.
+
+// The pieces of one group out of g.in into `out` (device form) or, through the staging buffer g.clip_out, into host
+// memory; pieces are never split (one is at most 2048 * 255 * 4 bytes).  On g.s_d2h; returns when all are written.
+template <typename OUT, bool MEAN>
+static int clip_gather_select(const std::vector<SelectPiece> &pieces, const std::vector<uint2> &table, uint8_t *out,
+                              bool device_out)
+{
+    const cudaStream_t s = g.s_d2h;
+    if (int rc = g.clip_pieces.ensure(kClipPieceBatch * sizeof(SelectPiece))) return rc;
+    if (int rc = g.clip_rows.ensure(table.size() * sizeof(uint2))) return rc;
+    if (!device_out)
+        if (int rc = g.clip_out.ensure(kClipStagingBytes)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(g.clip_rows.ptr, table.data(), table.size() * sizeof(uint2), cudaMemcpyHostToDevice, s));
+    uint8_t *staging = static_cast<uint8_t *>(g.clip_out.ptr);
+    std::vector<SelectPiece> batch;
+    std::vector<ClipPiece> copies; // host form: staging offset, host offset, bytes
+    for (size_t i = 0; i < pieces.size();) {
+        batch.clear();
+        copies.clear();
+        unsigned long long staged = 0;
+        for (; i < pieces.size() && batch.size() < kClipPieceBatch; i++) {
+            SelectPiece p = pieces[i];
+            if (!device_out) {
+                const unsigned long long bytes = (unsigned long long)p.count * (MEAN ? 1 : p.n) * sizeof(OUT);
+                if (staged + bytes > kClipStagingBytes)
+                    break;
+                if (!copies.empty() && copies.back().dst + copies.back().bytes == p.dst)
+                    copies.back().bytes += bytes;
+                else
+                    copies.push_back(ClipPiece{staged, p.dst, bytes});
+                p.dst = staged;
+                staged += bytes;
+            }
+            batch.push_back(p);
+        }
+        CUDA_TRY(cudaMemcpyAsync(g.clip_pieces.ptr, batch.data(), batch.size() * sizeof(SelectPiece),
+                                 cudaMemcpyHostToDevice, s));
+        k_clip_gather_select<OUT, MEAN><<<(unsigned)batch.size(), 256, 0, s>>>(
+            static_cast<const int16_t *>(g.in.ptr), static_cast<const uint2 *>(g.clip_rows.ptr),
+            device_out ? out : staging, static_cast<const SelectPiece *>(g.clip_pieces.ptr));
+        if (int rc = launch_check("k_clip_gather_select"))
+            return rc;
+        for (const ClipPiece &c : copies)
+            CUDA_TRY(cudaMemcpyAsync(out + c.dst, staging + c.src, c.bytes, cudaMemcpyDeviceToHost, s));
+    }
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return 0;
+}
+
+// Both forms of selab200_container_decode_clips_select, on the primary context (require_ready done, g_mutex held).
+static int decode_clips_select(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
+                               uint32_t n_clips, uint32_t length, const uint8_t *select, uint32_t n_select,
+                               uint32_t flags, uint8_t *out, bool device_out, uint64_t *frames_decoded,
+                               uint64_t *subframes_decoded)
+{
+    if (!frames_decoded || !subframes_decoded)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    *frames_decoded = 0;
+    *subframes_decoded = 0;
+    if (flags & ~(SELAB200_CLIP_FLOAT32 | SELAB200_CLIP_MEAN))
+        return fail(SELAB200_ERR_ARGUMENT, "unknown flag bits 0x%x", flags & ~(SELAB200_CLIP_FLOAT32 | SELAB200_CLIP_MEAN));
+    const bool f32 = flags & SELAB200_CLIP_FLOAT32, mean = flags & SELAB200_CLIP_MEAN;
+    if (mean && !f32)
+        return fail(SELAB200_ERR_ARGUMENT, "SELAB200_CLIP_MEAN needs SELAB200_CLIP_FLOAT32");
+    if (!select && n_select)
+        return fail(SELAB200_ERR_ARGUMENT, "select is null but n_select is %u", n_select);
+    if (select && !n_select)
+        return fail(SELAB200_ERR_ARGUMENT, "n_select is 0 but select is not null");
+    if (n_select > SELAB200_CLIP_MAX_SELECT)
+        return fail(SELAB200_ERR_ARGUMENT, "n_select is %u, more than %u", n_select, SELAB200_CLIP_MAX_SELECT);
+    if (n_clips == 0)
+        return 0;
+    if (!handles || !clips || !out)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    if (length == 0)
+        return fail(SELAB200_ERR_ARGUMENT, "clip 0: length must be at least 1");
+    for (uint32_t i = 0; i < n_handles; i++)
+        if (!handles[i])
+            return fail(SELAB200_ERR_ARGUMENT, "handles[%u] is null", i);
+    uint32_t top = 0; // the highest channel selected
+    for (uint32_t j = 0; j < n_select; j++)
+        top = std::max<uint32_t>(top, select[j]);
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const selab200_clip &c = clips[i];
+        if (c.container >= n_handles)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: container %u, but %u handles", i, c.container, n_handles);
+        if (c.reserved != 0)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: reserved field is not 0", i);
+        const unsigned long long total = (unsigned long long)handles[c.container]->info.n_frames * kFrame;
+        if (c.start > total || length > total - c.start)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: samples [%llu, %llu + %u) outside the %llu samples of its container",
+                        i, (unsigned long long)c.start, (unsigned long long)c.start, length, total);
+        const uint32_t C = handles[c.container]->info.channels, C0 = handles[clips[0].container]->info.channels;
+        if (select && top >= C)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: channel %u selected, but its container has %u channels", i, top, C);
+        if (!select && !mean && C != C0)
+            return fail(SELAB200_ERR_ARGUMENT, "clip %u: its container has %u channels, clip 0's %u: a full selection "
+                                               "without SELAB200_CLIP_MEAN needs one channel count", i, C, C0);
+    }
+    const uint32_t n_out = mean ? 1 : select ? n_select : handles[clips[0].container]->info.channels;
+    const unsigned long long sample_bytes = (unsigned long long)n_out * (f32 ? 4 : 2);
+    const unsigned long long clip_bytes = length * sample_bytes;
+    if (clip_bytes > ~0ull / n_clips)
+        return fail(SELAB200_ERR_ARGUMENT, "output of %u clips of %u samples does not fit 64 bits", n_clips, length);
+
+    // the selection: (container << 32 | frame), sorted and deduplicated
+    std::vector<unsigned long long> keys;
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const unsigned long long f0 = clips[i].start / kFrame, f1 = (clips[i].start + length - 1) / kFrame;
+        for (unsigned long long f = f0; f <= f1; f++)
+            keys.push_back((unsigned long long)clips[i].container << 32 | f);
+    }
+    std::sort(keys.begin(), keys.end());
+    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+
+    // Per covered frame: the header rules over all its subframes, the positions it needs (a bit each), and where its
+    // rows and row-table entries start in its group.  Groups are cut at frame ends.
+    const uint32_t group_subs = clip_group_frames(1);
+    std::vector<uint32_t> need(keys.size()), key_group(keys.size()), key_tab(keys.size());
+    std::vector<size_t> group_key0;
+    std::vector<std::vector<uint2>> tables;
+    uint64_t n_need = 0;
+    uint32_t rows = 0;
+    for (size_t k = 0; k < keys.size(); k++) {
+        const uint32_t ci = (uint32_t)(keys[k] >> 32);
+        const unsigned long long f = keys[k] & 0xffffffffull;
+        const selab200_container *h = handles[ci];
+        const uint32_t C = h->info.channels;
+        const selab200_subframe_desc *fd = h->buf.h_descs + f * C;
+        if (!frame_check(fd, C, h->info.n_words))
+            return fail(SELAB200_ERR_BITSTREAM, "container %u, frame %llu: a subframe header breaks the format", ci, f);
+        uint32_t pos[SELAB200_MAX_CHANNELS]; // channel -> position in the frame (a permutation, by frame_check)
+        for (uint32_t p = 0; p < C; p++)
+            pos[fd[p].channel] = p;
+        const uint32_t n_sel = select ? n_select : C;
+        uint32_t m = 0;
+        for (uint32_t j = 0; j < n_sel; j++) {
+            const uint32_t p = pos[select ? select[j] : j];
+            m |= 1u << p;
+            if (fd[p].subframe_type == 1)
+                m |= 1u << pos[fd[p].parent_channel];
+        }
+        const uint32_t n = (uint32_t)__builtin_popcount(m);
+        if (k == 0 || rows + n > group_subs) {
+            group_key0.push_back(k);
+            tables.emplace_back();
+            rows = 0;
+        }
+        std::vector<uint2> &tab = tables.back();
+        need[k] = m;
+        key_group[k] = (uint32_t)(group_key0.size() - 1);
+        key_tab[k] = (uint32_t)tab.size();
+        const auto row = [&](uint32_t p) { return rows + (uint32_t)__builtin_popcount(m & ((1u << p) - 1)); };
+        for (uint32_t j = 0; j < n_sel; j++) {
+            const uint32_t p = pos[select ? select[j] : j];
+            tab.push_back(make_uint2(row(p), fd[p].subframe_type == 1 ? row(pos[fd[p].parent_channel]) : kNoParentRow));
+        }
+        rows += n;
+        n_need += n;
+    }
+    *frames_decoded = keys.size();
+    *subframes_decoded = n_need;
+
+    // every clip as pieces of at most one frame each
+    std::vector<std::vector<SelectPiece>> pieces(group_key0.size());
+    for (uint32_t i = 0; i < n_clips; i++) {
+        const selab200_clip &c = clips[i];
+        const uint32_t n = select ? n_select : handles[c.container]->info.channels;
+        const unsigned long long f0 = c.start / kFrame, end = c.start + length;
+        const size_t k0 = std::lower_bound(keys.begin(), keys.end(), (unsigned long long)c.container << 32 | f0) - keys.begin();
+        for (unsigned long long s = c.start; s < end;) {
+            const uint32_t t0 = (uint32_t)(s % kFrame), count = (uint32_t)std::min<unsigned long long>(kFrame - t0, end - s);
+            const size_t k = k0 + (size_t)(s / kFrame - f0);
+            pieces[key_group[k]].push_back(SelectPiece{i * clip_bytes + (s - c.start) * sample_bytes, key_tab[k], n, t0, count});
+            s += count;
+        }
+    }
+
+    ClipSelection sel;
+    for (size_t grp = 0; grp < group_key0.size(); grp++) {
+        const size_t k1 = grp + 1 < group_key0.size() ? group_key0[grp + 1] : keys.size();
+        sel.descs.clear();
+        sel.src.clear();
+        sel.frame_h.clear();
+        sel.frame_end.clear();
+        unsigned long long words = 0;
+        for (size_t k = group_key0[grp]; k < k1; k++) {
+            const selab200_container *h = handles[keys[k] >> 32];
+            const unsigned long long f = keys[k] & 0xffffffffull;
+            const uint32_t C = h->info.channels;
+            const unsigned long long image = reinterpret_cast<unsigned long long>(h->buf.d_bytes);
+            for (uint32_t p = 0; p < C; p++) {
+                if (!((need[k] >> p) & 1))
+                    continue;
+                selab200_subframe_desc d = h->buf.h_descs[f * C + p];
+                const unsigned long long at = container_frame_byte(f, C, d.refl_offset) + 4 + (unsigned long long)kSubframeHeaderBytes * p + 7;
+                sel.src.push_back(image + at);
+                sel.frame_end.push_back(at + 4ull * d.refl_words + 5 + 4ull * d.res_words + 3);
+                sel.frame_h.push_back(h);
+                d.channel = 0;
+                d.subframe_type = 0;
+                d.parent_channel = 0;
+                d.refl_offset = words;
+                d.res_offset = words + d.refl_words;
+                words += (unsigned long long)d.refl_words + d.res_words;
+                sel.descs.push_back(d);
+            }
+        }
+        CodedInput in{sel.descs.data(), nullptr, (size_t)words, nullptr, &sel};
+        if (int rc = decode_pipeline(in, 0, (uint32_t)sel.descs.size(), 1, nullptr, nullptr, nullptr))
+            return rc;
+        const int rc = !f32  ? clip_gather_select<int16_t, false>(pieces[grp], tables[grp], out, device_out)
+                       : mean ? clip_gather_select<float, true>(pieces[grp], tables[grp], out, device_out)
+                              : clip_gather_select<float, false>(pieces[grp], tables[grp], out, device_out);
+        if (rc)
+            return rc;
+    }
+    return 0;
+}
+
 extern "C" {
 
 int selab200_container_decode_clips(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
@@ -2763,6 +2993,41 @@ int selab200_container_decode_clips_device(selab200_container *const *handles, u
     }
     return decode_clips(handles, n_handles, clips, n_clips, length, reinterpret_cast<uint8_t *>(d_pcm_out), true,
                         frames_decoded);
+}
+
+int selab200_container_decode_clips_select(selab200_container *const *handles, uint32_t n_handles,
+                                           const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                           const uint8_t *select, uint32_t n_select, uint32_t flags, void *out,
+                                           uint64_t *frames_decoded, uint64_t *subframes_decoded)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    return decode_clips_select(handles, n_handles, clips, n_clips, length, select, n_select, flags,
+                               static_cast<uint8_t *>(out), false, frames_decoded, subframes_decoded);
+}
+
+int selab200_container_decode_clips_select_device(selab200_container *const *handles, uint32_t n_handles,
+                                                  const selab200_clip *clips, uint32_t n_clips, uint32_t length,
+                                                  const uint8_t *select, uint32_t n_select, uint32_t flags,
+                                                  void *d_out, uint64_t *frames_decoded, uint64_t *subframes_decoded)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (d_out && n_clips) { // the primary holds every open image, so the output must live there too
+        cudaPointerAttributes attr;
+        if (cudaPointerGetAttributes(&attr, d_out) != cudaSuccess || attr.type != cudaMemoryTypeDevice ||
+            attr.device != g.device) {
+            cudaGetLastError();
+            return fail(SELAB200_ERR_ARGUMENT, "d_out is not device memory of the primary device (%d)", g.device);
+        }
+        const unsigned align = flags & SELAB200_CLIP_FLOAT32 ? 4 : 2;
+        if (reinterpret_cast<uintptr_t>(d_out) & (align - 1))
+            return fail(SELAB200_ERR_ARGUMENT, "d_out is not %u-byte aligned", align);
+    }
+    return decode_clips_select(handles, n_handles, clips, n_clips, length, select, n_select, flags,
+                               static_cast<uint8_t *>(d_out), true, frames_decoded, subframes_decoded);
 }
 
 int selab200_container_info_get(const uint8_t *container, size_t n_bytes, selab200_container_info *info)

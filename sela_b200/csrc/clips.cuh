@@ -81,4 +81,79 @@ __global__ void __launch_bounds__(256) k_clip_gather(const uint8_t *frames, uint
     }
 }
 
+// ---- channel-selecting clip decode (selab200_container_decode_clips_select, DESIGN.md 7.9) ----
+//
+// The needed subframes are decoded as mono frames, one [2048] int16 row each.  A row-table entry names the row of
+// one selected channel in a frame and, for a difference-coded channel, the row of its parent (else kNoParentRow).
+
+constexpr uint32_t kNoParentRow = 0xffffffffu;
+constexpr uint32_t kSelectTileBytes = 16384; // output bytes staged per pass of k_clip_gather_select
+
+// Samples [t0, t0 + count) of one frame of one clip (count <= 2048), written from output byte dst on.
+struct SelectPiece {
+    unsigned long long dst;
+    uint32_t rows;     // row-table index of the first selected channel of the frame
+    uint32_t n;        // selected channels: the mean's divisor, else the output channels
+    uint32_t t0, count;
+};
+
+// Sample t of a table entry: the row's, or (uint16)(parent - difference) as k_diff_fixup computes it.
+__device__ __forceinline__ int16_t select_sample(const int16_t *rows, uint2 e, uint32_t t)
+{
+    const int16_t v = __ldg(rows + (size_t)e.x * kFrame + t);
+    if (e.y == kNoParentRow)
+        return v;
+    return (int16_t)(uint16_t)((uint32_t)__ldg(rows + (size_t)e.y * kFrame + t) - (uint32_t)v);
+}
+
+// Piece blockIdx.x.  Per pass a tile of whole samples [samples][n_out] is staged in shared memory at the 16-byte
+// phase of its destination, reading every row along its samples; then it goes out as aligned 16-byte stores, with
+// OUT-wide stores only at the tile's ragged ends.  OUT is int16_t or float (x / 32768, exact); MEAN (float) writes
+// one value per sample, the exact integer sum over the n channels divided by 32768 n, rounded to nearest.
+template <typename OUT, bool MEAN>
+__global__ void __launch_bounds__(256) k_clip_gather_select(const int16_t *rows, const uint2 *table, uint8_t *out,
+                                                            const SelectPiece *pieces)
+{
+    __shared__ __align__(16) uint8_t tile[kSelectTileBytes + 16];
+    const SelectPiece p = pieces[blockIdx.x];
+    const uint32_t n_out = MEAN ? 1 : p.n, sample_bytes = n_out * (uint32_t)sizeof(OUT);
+    const uint32_t per = kSelectTileBytes / sample_bytes; // samples per pass
+    const uint2 *e = table + p.rows;
+    for (uint32_t s0 = 0; s0 < p.count; s0 += per) {
+        const uint32_t ns = min(per, p.count - s0);
+        const unsigned long long d0 = reinterpret_cast<unsigned long long>(out) + p.dst + (unsigned long long)s0 * sample_bytes;
+        const unsigned long long d1 = d0 + (unsigned long long)ns * sample_bytes, base = d0 & ~15ull;
+        OUT *t = reinterpret_cast<OUT *>(tile + (d0 & 15));
+        for (uint32_t k = threadIdx.x; k < ns; k += blockDim.x) {
+            const uint32_t at = p.t0 + s0 + k;
+            if (MEAN) {
+                int32_t S = 0;
+                for (uint32_t j = 0; j < p.n; j++)
+                    S += select_sample(rows, e[j], at);
+                t[k] = __fdiv_rn((float)S, (float)(32768 * p.n));
+            } else {
+                for (uint32_t j = 0; j < n_out; j++) {
+                    const int16_t v = select_sample(rows, e[j], at);
+                    if constexpr (sizeof(OUT) == 2)
+                        t[k * n_out + j] = v;
+                    else
+                        t[k * n_out + j] = (float)v * (1.0f / 32768);
+                }
+            }
+        }
+        __syncthreads();
+        const unsigned long long a0 = (d0 + 15) & ~15ull, a1 = d1 & ~15ull; // the aligned body [a0, a1)
+        for (unsigned long long x = a0 + 16ull * threadIdx.x; x < a1; x += 16ull * blockDim.x)
+            *reinterpret_cast<uint4 *>(x) = *reinterpret_cast<const uint4 *>(tile + (x - base));
+        if (threadIdx.x < 32) { // ragged ends: fewer than 16 bytes in front of the body and behind it
+            const unsigned long long x = threadIdx.x < 16 ? d0 + sizeof(OUT) * threadIdx.x
+                                                          : (a1 > a0 ? a1 : a0) + sizeof(OUT) * (threadIdx.x - 16);
+            const bool mine = threadIdx.x < 16 ? x < a0 && x < d1 : x < d1 && x >= a0;
+            if (mine)
+                *reinterpret_cast<OUT *>(x) = *reinterpret_cast<const OUT *>(tile + (x - base));
+        }
+        __syncthreads();
+    }
+}
+
 } // namespace selab200

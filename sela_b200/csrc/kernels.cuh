@@ -893,8 +893,9 @@ __global__ void __launch_bounds__(256) k_container_unpack(const uint8_t *contain
 // ------------------------------------------------------------------ decode --
 
 // Acceptance of a whole frame (its ch descriptors fd[0..ch)): every subframe passes desc_ok (common.cuh), the channel fields form
-// a permutation and every parent is an independent subframe.
-__device__ __forceinline__ bool frame_check(const selab200_subframe_desc *fd, uint32_t ch, unsigned long long n_words)
+// a permutation and every parent is an independent subframe.  The host applies it too (the channel-selecting clip
+// decode checks every covered frame, decoded subframes or not).
+__host__ __device__ __forceinline__ bool frame_check(const selab200_subframe_desc *fd, uint32_t ch, unsigned long long n_words)
 {
     bool ok = true;
     unsigned seen = 0, type_mask = 0; // by channel: seen, difference-coded

@@ -186,6 +186,10 @@ public:
     // (selab200_container_decode_clips: only the frames the range covers are decoded).  The header is the one
     // processTo() writes for that many samples; the data chunk equals the same bytes of processTo()'s.
     void processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples);
+    // The same for only the channels listed, in that order (repeats allowed): a WAV of that many channels, from only
+    // the subframes they need (selab200_container_decode_clips_select).  An empty list means every channel.
+    void processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples,
+                        const std::vector<uint8_t> &channels);
     // Not in the reference: decode this .sela stream on the device and compare it with the whole frames of the
     // WAV file `wavInput` (its partial final frame is ignored, as the encoder ignores it).  Returns every
     // (frame, channel) that differs, in order.  Throws data::Exception if the WAV's channels, sample rate or

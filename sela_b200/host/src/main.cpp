@@ -24,7 +24,9 @@
 // and the reference order; most of -S's saving at a fraction of its cost, decoding back to the WAV under the
 // reference decoder.  One line with the bytes written and the bytes -e writes.
 // `-R in.sela out.wav first_sample n_samples` (random access): the WAV -d writes, cut to samples
-// [first_sample, first_sample + n_samples) of every channel; only the frames that range covers are decoded.
+// [first_sample, first_sample + n_samples) of every channel; only the frames that range covers are decoded.  With a
+// fifth argument `c0,c1,...` the WAV holds just those channels, in that order, decoded from only the subframes they
+// need.
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -128,7 +130,7 @@ int usage(const std::string &prog)
               << "Encoding a file smaller, searching the predictor orders an estimate ranks best (H100 build):\n"
               << prog << " -F path/to/input.wav path/to/output.sela\n\n"
               << "Decoding samples [first, first + count) of every channel of a file (H100 build):\n" << prog
-              << " -R path/to/input.sela path/to/output.wav first count\n\n"
+              << " -R path/to/input.sela path/to/output.wav first count [c0,c1,...]\n\n"
               << "Testing a file against a wav file (H100 build):\n" << prog << " -t path/to/input.sela path/to/input.wav\n\n"
               << "Many files in one process (H100 build):\n" << prog << " -E out_dir a.wav b.wav ...\n"
               << prog << " -D out_dir a.sela b.sela ..." << std::endl;
@@ -181,18 +183,32 @@ int main(int argc, char **argv)
             } else {
                 sela::Decoder(in).processTo(out);
             }
-        } else if (mode == "-R" && argc == 6) {
+        } else if (mode == "-R" && (argc == 6 || argc == 7)) {
             uint64_t first = 0, count = 0;
+            std::vector<uint8_t> channels;
             try {
                 first = std::stoull(argv[4]);
                 count = std::stoull(argv[5]);
             } catch (const std::exception &) {
                 throw data::Exception("first sample and sample count must be non-negative integers");
             }
+            if (argc == 7) {
+                const std::string list = argv[6];
+                size_t at = 0;
+                while (at <= list.size()) {
+                    const size_t end = std::min(list.find(',', at), list.size());
+                    const std::string item = list.substr(at, end - at);
+                    if (item.empty() || item.find_first_not_of("0123456789") != std::string::npos || item.size() > 3 ||
+                        std::stoul(item) > 255)
+                        throw data::Exception("channels must be a comma-separated list of numbers in [0, 255]");
+                    channels.push_back((uint8_t)std::stoul(item));
+                    at = end + 1;
+                }
+            }
             std::ifstream in(argv[2], std::ios::binary);
             std::ofstream out(argv[3], std::ios::binary);
             std::cout << "Decoding samples " << first << " to " << first + count << ": " << argv[2] << std::endl;
-            sela::Decoder(in).processRangeTo(out, first, count);
+            sela::Decoder(in).processRangeTo(out, first, count, channels);
         } else if (mode == "-V" && argc == 4) {
             std::ifstream in(argv[2], std::ios::binary);
             std::ofstream out(argv[3], std::ios::binary);

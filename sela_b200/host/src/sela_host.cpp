@@ -979,6 +979,13 @@ void Decoder::processTo(std::ofstream &outputFile)
 // processTo() for one sample range: the container opens as for processTo(), and one clip comes back.
 void Decoder::processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples)
 {
+    processRangeTo(outputFile, firstSample, nSamples, {});
+}
+
+// The same for the channels listed (all of them if the list is empty): only the subframes they need are decoded.
+void Decoder::processRangeTo(std::ofstream &outputFile, uint64_t firstSample, uint64_t nSamples,
+                             const std::vector<uint8_t> &channels)
+{
     StagingScope staging;
     DeviceWarmup warmup;
     RawFile file;
@@ -1002,16 +1009,21 @@ void Decoder::processRangeTo(std::ofstream &outputFile, uint64_t firstSample, ui
         raise("sela_b200: the sample count must be in [1, 2^32 - 1]");
     if (info.channels == 0 || info.channels > SELAB200_MAX_CHANNELS)
         raise("sela_b200: unsupported channel count");
-    const size_t n_values = (size_t)nSamples * info.channels;
+    const uint32_t n_out = channels.empty() ? info.channels : (uint32_t)channels.size();
+    const size_t n_values = (size_t)nSamples * n_out;
     int16_t *pcm = reinterpret_cast<int16_t *>(t_output.ensure((n_values + 1) * 2));
     {
         Phase p("decode range (device)");
         const selab200_clip clip{0, 0, firstSample};
-        uint64_t frames = 0;
-        check(selab200_container_decode_clips(&handle, 1, &clip, 1, (uint32_t)nSamples, pcm, &frames));
+        uint64_t frames = 0, subframes = 0;
+        if (channels.empty())
+            check(selab200_container_decode_clips(&handle, 1, &clip, 1, (uint32_t)nSamples, pcm, &frames));
+        else
+            check(selab200_container_decode_clips_select(&handle, 1, &clip, 1, (uint32_t)nSamples, channels.data(),
+                                                         (uint32_t)channels.size(), 0, pcm, &frames, &subframes));
     }
     Phase p("write output");
-    file::WavFile shell(info.sample_rate, info.bits_per_sample, info.channels, {});
+    file::WavFile shell(info.sample_rate, info.bits_per_sample, (uint16_t)n_out, {});
     const size_t payload = n_values * (info.bits_per_sample / 8);
     shell.wavChunk.chunkSize = (uint32_t)(payload + 36);
     shell.wavChunk.dataSubChunk.subChunkSize = (uint32_t)payload;
