@@ -220,6 +220,21 @@ int  selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_
 int  selab200_container_decode(selab200_container *handle, int16_t *pcm_out);
 void selab200_container_close(selab200_container *handle);
 
+/* A host-resident open (DESIGN.md 7.10): for a corpus larger than the device memory it may take.  The same header
+ * checks, errors, messages, frame walk and info as selab200_container_open for the same bytes, but the handle copies
+ * the image into page-locked host memory it owns (mapped into the devices' address space, 64 bytes of padding) and
+ * allocates no device memory for it.  Unlike selab200_container_open, the caller's buffer may be freed or overwritten
+ * as soon as this returns.  The handle works in every call that takes one, mixed freely with device-resident handles,
+ * with results bit for bit those of a device-resident handle over the same bytes; selab200_container_close closes it.
+ *   - the clip calls fetch over PCIe only the bytes of the subframes they decode: per subframe [a & ~15, (b + 15) & ~15)
+ *     with a its first reflection byte and b 3 bytes past its last residue byte, merged, in selection order, with the
+ *     previous range of the same container when they touch or overlap, within one decode group (the groups the clip
+ *     calls document); each merged run is fetched once per group.  Device memory for the fetched bytes is bounded by
+ *     one group's;
+ *   - selab200_container_decode and selab200_container_verify upload each device's block of the image per call. */
+int  selab200_container_open_host(const uint8_t *container, size_t n_bytes, selab200_container **handle,
+                                  selab200_container_info *info);
+
 /* Random access (DESIGN.md 7.8): a batch of clips of `length` samples each from any of n_handles open containers with
  * the same channel count.  Clip i is samples [start, start + length) of every channel of handles[clips[i].container],
  * i.e. rows start .. start + length - 1 of that container's selab200_container_decode output viewed as
@@ -281,6 +296,11 @@ int selab200_container_decode_clips_select_device(selab200_container *const *han
                                                   const selab200_clip *clips, uint32_t n_clips, uint32_t length,
                                                   const uint8_t *select, uint32_t n_select, uint32_t flags,
                                                   void *d_out, uint64_t *frames_decoded, uint64_t *subframes_decoded);
+
+/* *bytes receives the bytes of host-resident images (selab200_container_open_host) the process's last clip call
+ * fetched, by the rule above: the sum of its runs' lengths over all its groups; 0 if it read only device-resident
+ * images.  SELAB200_ERR_NOT_INIT before selab200_init; diagnostics and bench bookkeeping. */
+int selab200_clip_bytes_fetched(uint64_t *bytes);
 
 /* ------------------------------------------------------------- verify -- */
 

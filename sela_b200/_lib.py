@@ -110,12 +110,14 @@ _SIGNATURES = {
     "selab200_container_info_get": (_I, [_V, _SZ, _V]),
     "selab200_container_frame_offsets": (_I, [_V, _SZ, _V, _SZ, _V]),
     "selab200_container_open": (_I, [_V, _SZ, _V, _V]),
+    "selab200_container_open_host": (_I, [_V, _SZ, _V, _V]),
     "selab200_container_decode": (_I, [_V, _V]),
     "selab200_container_close": (None, [_V]),
     "selab200_container_decode_clips": (_I, [_V, _U32, _V, _U32, _U32, _V, _V]),
     "selab200_container_decode_clips_device": (_I, [_V, _U32, _V, _U32, _U32, _V, _V]),
     "selab200_container_decode_clips_select": (_I, [_V, _U32, _V, _U32, _U32, _V, _U32, _U32, _V, _V, _V]),
     "selab200_container_decode_clips_select_device": (_I, [_V, _U32, _V, _U32, _U32, _V, _U32, _U32, _V, _V, _V]),
+    "selab200_clip_bytes_fetched": (_I, [_V]),
     "selab200_verify_workspace_bytes": (_SZ, [_U32, _U32]),
     "selab200_verify_frames_device": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _V, _V, _V, _SZ, _V]),
     "selab200_verify_frames": (_I, [_V, _U32, _U32, _V, _SZ, _V, _V, _SZ, _V]),

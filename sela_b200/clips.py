@@ -10,6 +10,13 @@ Opening a container uploads its whole byte image to the device and walks its fra
 the handles (and the byte buffers they read) open until close(), so each call decodes only the frames its clips
 cover, each of them once.  With `channels`, `dtype` or `mean` only the subframes the chosen channels need are
 decoded (DESIGN.md 7.9), and containers of different channel counts may share a call.
+
+With host_resident=True the images stay in page-locked host memory instead, for a corpus larger than the device
+memory it may take, and each call fetches over PCIe only the bytes of the subframes it decodes (DESIGN.md 7.10):
+
+    with ClipDecoder(blobs, host_resident=True) as dec:
+        x = dec.decode_device(ks, starts, 44100, channels=[0])
+        dec.bytes_fetched                                  # the bytes that call read from host memory
 """
 import ctypes as C
 
@@ -21,9 +28,12 @@ from ._lib import CLIP_DTYPE, CLIP_FLOAT32, CLIP_MAX_SELECT, CLIP_MEAN, INFO_DTY
 class ClipDecoder:
     """Open containers (bytes, bytearray or uint8 arrays of whole .sela files) for clip decoding on `device` (an int,
     or a list of devices whose first, the primary, holds the images and runs the decode).  Containers may differ in
-    channel count; a call that returns every channel as int16 still needs one count."""
+    channel count; a call that returns every channel as int16 still needs one count.
 
-    def __init__(self, containers, device=0):
+    host_resident: open every container with selab200_container_open_host: the handle keeps its own page-locked copy
+    of the image, no device memory holds it, and the decoder keeps no reference to the caller's bytes."""
+
+    def __init__(self, containers, device=0, host_resident=False):
         init(device)
         self.device = device[0] if isinstance(device, (list, tuple)) else device
         self._bufs, self._handles, self.info = [], [], []
@@ -34,8 +44,10 @@ class ClipDecoder:
                                            np.uint8)
                 info = np.zeros(1, INFO_DTYPE)
                 handle = C.c_void_p(0)
-                check(L.selab200_container_open(buf.ctypes.data, buf.size, C.addressof(handle), info.ctypes.data))
-                self._bufs.append(buf)  # the handle reads these bytes until it is closed
+                opener = L.selab200_container_open_host if host_resident else L.selab200_container_open
+                check(opener(buf.ctypes.data, buf.size, C.addressof(handle), info.ctypes.data))
+                if not host_resident:
+                    self._bufs.append(buf)  # the handle reads these bytes until it is closed
                 self._handles.append(handle.value)
                 self.info.append({k: int(info[0][k]) for k in INFO_DTYPE.names if k != "reserved"})
         except Exception:
@@ -43,7 +55,8 @@ class ClipDecoder:
             raise
         self._array = (C.c_void_p * max(len(self._handles), 1))(*self._handles)
         self.channels = self.info[0]["channels"] if self.info else 0
-        self.frames_decoded = self.subframes_decoded = 0
+        self.host_resident = bool(host_resident)
+        self.frames_decoded = self.subframes_decoded = self.bytes_fetched = 0
 
     def _clips(self, container_index, starts, length):
         if not self._handles:
@@ -85,6 +98,12 @@ class ClipDecoder:
                  select.ctypes.data if select is not None else None, 0 if select is None else select.size, flags,
                  out_ptr, C.addressof(n), C.addressof(m)))
         self.frames_decoded, self.subframes_decoded = n.value, m.value
+        self._fetched()
+
+    def _fetched(self):
+        b = C.c_uint64(0)
+        check(lib().selab200_clip_bytes_fetched(C.addressof(b)))
+        self.bytes_fetched = b.value
 
     def decode(self, container_index, starts, length, channels=None, dtype=np.int16, mean=False):
         """Clip i = samples [starts[i], starts[i] + length) of container container_index (an int, or one per clip)
@@ -104,6 +123,7 @@ class ClipDecoder:
                                                         C.addressof(n)))
             self.frames_decoded = n.value
             self.subframes_decoded = n.value * self.channels
+            self._fetched()
             return out
         select, flags = choice
         out = np.empty((clips.size, length, self._n_out(clips, select, flags)), dtype)
@@ -130,6 +150,7 @@ class ClipDecoder:
                                                                C.c_void_p(out.data_ptr()), C.addressof(n)))
             self.frames_decoded = n.value
             self.subframes_decoded = n.value * self.channels
+            self._fetched()
             return out
         self._call(True, clips, length, *choice, C.c_void_p(out.data_ptr()))
         return out

@@ -111,6 +111,7 @@ struct Context {
     DeviceBuffer lossless;                         // lossless host paths: count, per-pair records of re-coded subframes
     DeviceBuffer clip_src, clip_pieces, clip_out;  // clip decode: source addresses, gather pieces, host-form staging
     DeviceBuffer clip_rows;                        // channel-selecting clip decode: the gather's row table
+    DeviceBuffer clip_runs, clip_stage;            // host-resident images: a group's fetch runs and their staging
     Counters *h_small = nullptr;                   // pinned: where g.small's counters come down
     unsigned long long *h_totals = nullptr;        // pinned: arena fill level after each chunk
     size_t last_rice_n_sub = 0;                    // selab200_rice_decode_frames_device bookkeeping (flag count query)
@@ -1130,6 +1131,8 @@ static void shutdown_slot()
     g.clip_pieces.release();
     g.clip_out.release();
     g.clip_rows.release();
+    g.clip_runs.release();
+    g.clip_stage.release();
     g.small.release();
     if (g.h_small)
         cudaFreeHost(g.h_small);
@@ -1768,12 +1771,16 @@ static void words_referenced(const selab200_subframe_desc *dc, size_t n, size_t 
 }
 
 struct selab200_container {
-    const uint8_t *bytes = nullptr;
+    const uint8_t *bytes = nullptr; // the caller's bytes, or (host-resident) the handle's page-locked copy
     size_t n_bytes = 0;
     selab200_container_info info{};
     ContainerBuffers buf;
     size_t piece_bytes = 0;
     int n_pieces = 0;
+    // selab200_container_open_host: no device image (buf.d_bytes stays null); the page-locked copy is mapped, and
+    // clip calls fetch what they read from it through `mapped`, its device address
+    bool host = false;
+    const uint8_t *mapped = nullptr;
 };
 
 // One host-to-device copy.
@@ -1784,14 +1791,20 @@ struct Upload {
 };
 
 // One group of the clip decode's selection: frames of any open containers, numbered from 0 in (container, frame)
-// order.  Per subframe a descriptor re-based into one compact arena of n_words words and the device address of its
-// reflection words in its container's image; per frame its container and the end of the bytes it reads (+3 bytes of
-// slack), which say which upload pieces a chunk waits for.
+// order.  Per subframe a descriptor re-based into one compact arena of n_words words, the file byte of its reflection
+// words and their device address: in its container's image, or for a host-resident container in the staging buffer
+// its fetch run goes to (plan_fetch).  Per frame its container and the end of the bytes it reads (+3 bytes of slack),
+// which say which upload pieces a chunk waits for.
 struct ClipSelection {
     std::vector<selab200_subframe_desc> descs;
-    std::vector<unsigned long long> src;
+    std::vector<unsigned long long> src, at;
     std::vector<const selab200_container *> frame_h;
     std::vector<unsigned long long> frame_end;
+    // host-resident subframes (plan_fetch): the group's fetch runs in selection order, each with its first subframe,
+    // and per subframe its run (-1: a device-resident image)
+    std::vector<FetchRun> runs;
+    std::vector<size_t> run_first;
+    std::vector<int64_t> run;
 };
 
 // Where the decode-side pipeline's coded input comes from, frames numbered file-globally in the first two cases: the
@@ -1811,14 +1824,16 @@ struct CodedInput {
     uint32_t *arena = nullptr;           // the decoder's word array, addressed by the descriptors' offsets
     const uint8_t *d_bytes = nullptr;    // container: the byte image on this device, addressed by file offset
     bool primary = true;
+    std::vector<int> fetched;            // clip selection: per chunk, the fetch piece (g.ev_h2d) it waits for, or -1
 
-    int start(uint32_t F0, uint32_t NF, uint32_t ch)
+    int start(uint32_t F0, uint32_t NF, uint32_t ch, const ChunkPlan &plan)
     {
         channels = ch;
         if (sel) { // re-based descriptors: the arena is addressed from 0
             if (int rc = g.words.ensure(n_words * 4 + 96)) return rc;
             arena = reinterpret_cast<uint32_t *>(static_cast<char *>(g.words.ptr) + 16); // 16 bytes of slack in front
-            return g.clip_src.ensure(sel->src.size() * sizeof(unsigned long long));
+            if (int rc = g.clip_src.ensure(sel->src.size() * sizeof(unsigned long long))) return rc;
+            return fetch(plan);
         }
         if (!h) {
             if (int rc = g.words.ensure(n_words * 4 + 16)) return rc;
@@ -1834,8 +1849,8 @@ struct CodedInput {
         // 16 bytes of slack in front (the Rice decoder reads whole 16-byte vectors), the 16-byte phase of file order kept
         arena = reinterpret_cast<uint32_t *>(static_cast<char *>(g.words.ptr) + 16 + ((w_lo * 4) & 15)) - w_lo;
         // The primary device holds the whole byte image (uploaded by selab200_container_open, in pieces with events);
-        // any other device uploads just the bytes of its block.
-        primary = tl_ctx == &g_slots[0];
+        // any other device, and every device for a host-resident image, uploads just the bytes of its block.
+        primary = tl_ctx == &g_slots[0] && !h->host;
         d_bytes = static_cast<const uint8_t *>(h->buf.d_bytes);
         if (!primary) {
             const unsigned long long b0 = container_frame_byte(F0, ch, w_lo) & ~3ull; // the unpack kernel reads aligned 32-bit words
@@ -1845,6 +1860,47 @@ struct CodedInput {
             CUDA_TRY(cudaEventRecord(g.ev_h2d[0], g.s_h2d));
             d_bytes = static_cast<const uint8_t *>(g.aux.ptr) - b0;
         }
+        return 0;
+    }
+
+    // The selection's fetch runs (plan_fetch) go up on s_h2d in one piece per chunk, the runs that start in the chunk,
+    // each followed by event g.ev_h2d[c]; a chunk waits for the piece that holds its last run.  Staging is written once
+    // per group: decode_pipeline drains before the next group's fetch starts.
+    int fetch(const ChunkPlan &plan)
+    {
+        const uint32_t n_chunks = plan.chunks();
+        fetched.assign(n_chunks, -1);
+        if (sel->runs.empty())
+            return 0;
+        if (int rc = g.clip_runs.ensure(sel->runs.size() * sizeof(FetchRun))) return rc;
+        const FetchRun *d_runs = static_cast<const FetchRun *>(g.clip_runs.ptr);
+        CUDA_TRY(cudaMemcpyAsync(g.clip_runs.ptr, sel->runs.data(), sel->runs.size() * sizeof(FetchRun),
+                                 cudaMemcpyHostToDevice, g.s_h2d));
+        std::vector<int> piece(sel->runs.size());
+        size_t r = 0;
+        for (uint32_t c = 0; c < n_chunks; c++) {
+            const size_t r0 = r, end = (size_t)plan.start[c + 1] * channels;
+            unsigned long long widest = 0;
+            for (; r < sel->runs.size() && sel->run_first[r] < end; r++) {
+                piece[r] = (int)c;
+                widest = std::max(widest, sel->runs[r].bytes);
+            }
+            if (r == r0)
+                continue;
+            const unsigned long long per_cta = 16ull * kFetchLoads * 256;
+            const unsigned rows = (unsigned)std::min<unsigned long long>(kFetchCtas, (widest + per_cta - 1) / per_cta);
+            const unsigned cols = (unsigned)std::min<size_t>(r - r0, std::max(1u, kFetchCtas / rows));
+            k_clip_fetch<<<dim3(cols, rows), 256, 0, g.s_h2d>>>(d_runs + r0, (uint32_t)(r - r0));
+            if (int rc = launch_check("k_clip_fetch"))
+                return rc;
+            CUDA_TRY(cudaEventRecord(g.ev_h2d[c], g.s_h2d));
+        }
+        for (uint32_t c = 0; c < n_chunks; c++) // runs follow selection order: a chunk's last host subframe reads last
+            for (size_t i = (size_t)plan.start[c + 1] * channels; i > (size_t)plan.start[c] * channels; i--)
+                if (sel->run[i - 1] >= 0) {
+                    fetched[c] = piece[(size_t)sel->run[i - 1]];
+                    break;
+                }
         return 0;
     }
 
@@ -1860,10 +1916,13 @@ struct CodedInput {
             unsigned long long *d_src = static_cast<unsigned long long *>(g.clip_src.ptr) + (size_t)f0 * channels;
             CUDA_TRY(cudaMemcpyAsync(d_src, sel->src.data() + (size_t)f0 * channels, n * sizeof(unsigned long long),
                                      cudaMemcpyHostToDevice, lane));
-            // every container the chunk reads: the upload piece that holds the last byte it reads there
+            // every device-resident container the chunk reads: the upload piece that holds the last byte it reads
+            // there; every host-resident one: the fetch piece that holds its last run
+            if (fetched[c] >= 0)
+                CUDA_TRY(cudaStreamWaitEvent(lane, g.ev_h2d[fetched[c]], 0));
             for (uint32_t f = f0; f < f0 + nf; f++) {
                 const selab200_container *c = sel->frame_h[f];
-                if (f + 1 < f0 + nf && sel->frame_h[f + 1] == c)
+                if (c->host || (f + 1 < f0 + nf && sel->frame_h[f + 1] == c))
                     continue; // frames of one container are in file order: its last frame here reads furthest
                 const int piece = std::min(c->n_pieces - 1, (int)(sel->frame_end[f] / c->piece_bytes));
                 CUDA_TRY(cudaStreamWaitEvent(lane, c->buf.ev_piece[piece], 0));
@@ -1925,7 +1984,7 @@ static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t cha
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
         if (int rc = g.lane_work[i].ensure(ws_bytes)) return rc;
-    if (int rc = in.start(F0, NF, channels)) return rc;
+    if (int rc = in.start(F0, NF, channels, plan)) return rc;
     int32_t *d_status = &device_counters()->status;
     int16_t *d_pcm = static_cast<int16_t *>(g.in.ptr);
     selab200_subframe_desc *d_descs = static_cast<selab200_subframe_desc *>(g.descs.ptr);
@@ -2584,6 +2643,61 @@ static uint32_t clip_group_frames(uint32_t channels)
     return std::max<uint32_t>(1, kClipGroupSubframes / channels);
 }
 
+// Bytes of host-resident images the last clip call fetched (selab200_clip_bytes_fetched); g_mutex guards it.
+static uint64_t g_clip_bytes_fetched = 0;
+
+// The fetch runs of one group (DESIGN.md 7.10).  Each host-resident subframe reads the bytes [at, end) of its image,
+// from its reflection words to 3 bytes past its residue words (what get_words_at_byte touches); rounded out to
+// [at & ~15, (end + 15) & ~15), the ranges of one container that touch or overlap, taken in selection order, merge
+// into one run.  Runs are staged back to back in g.clip_stage, so a run keeps its 16-byte phase, and each such
+// subframe's src is re-pointed into its run's staging.  Host images are page-aligned, so file offsets and mapped
+// addresses have the same 16-byte phase.
+static int plan_fetch(ClipSelection &sel, uint32_t channels)
+{
+    sel.runs.clear();
+    sel.run_first.clear();
+    sel.run.assign(sel.src.size(), -1);
+    std::vector<const selab200_container *> run_h;
+    unsigned long long staged = 0;
+    for (size_t i = 0; i < sel.src.size(); i++) {
+        const selab200_container *h = sel.frame_h[i / channels];
+        if (!h->host)
+            continue;
+        const selab200_subframe_desc &d = sel.descs[i];
+        const unsigned long long lo = sel.at[i] & ~15ull;
+        const unsigned long long hi = (sel.at[i] + 4ull * d.refl_words + 5 + 4ull * d.res_words + 3 + 15) & ~15ull;
+        // runs hold file offsets (src) and staging offsets (dst) until the staging buffer is placed
+        FetchRun *last = sel.runs.empty() ? nullptr : &sel.runs.back();
+        if (last && run_h.back() == h && lo <= last->src + last->bytes) {
+            if (hi > last->src + last->bytes) {
+                staged += hi - (last->src + last->bytes);
+                last->bytes = hi - last->src;
+            }
+        } else {
+            sel.runs.push_back(FetchRun{lo, staged, hi - lo});
+            sel.run_first.push_back(i);
+            run_h.push_back(h);
+            staged += hi - lo;
+        }
+        sel.run[i] = (int64_t)sel.runs.size() - 1;
+    }
+    if (sel.runs.empty())
+        return 0;
+    g_clip_bytes_fetched += staged;
+    if (int rc = g.clip_stage.ensure(staged)) return rc;
+    const unsigned long long stage = reinterpret_cast<unsigned long long>(g.clip_stage.ptr);
+    for (size_t i = 0; i < sel.src.size(); i++)
+        if (sel.run[i] >= 0) {
+            const FetchRun &r = sel.runs[(size_t)sel.run[i]];
+            sel.src[i] = stage + r.dst + (sel.at[i] - r.src);
+        }
+    for (size_t r = 0; r < sel.runs.size(); r++) {
+        sel.runs[r].src += reinterpret_cast<unsigned long long>(run_h[r]->mapped);
+        sel.runs[r].dst += stage;
+    }
+    return 0;
+}
+
 // The pieces of one group, in output order, out of g.in into `out` (device form) or, through the staging buffer
 // g.clip_out, into host memory.  On g.s_d2h; returns when every piece is written.
 static int clip_gather(const std::vector<ClipPiece> &pieces, uint8_t *out, bool device_out)
@@ -2640,6 +2754,7 @@ static int clip_gather(const std::vector<ClipPiece> &pieces, uint8_t *out, bool 
 static int decode_clips(selab200_container *const *handles, uint32_t n_handles, const selab200_clip *clips,
                         uint32_t n_clips, uint32_t length, uint8_t *out, bool device_out, uint64_t *frames_decoded)
 {
+    g_clip_bytes_fetched = 0;
     if (!frames_decoded)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     *frames_decoded = 0;
@@ -2706,6 +2821,7 @@ static int decode_clips(selab200_container *const *handles, uint32_t n_handles, 
         const uint32_t nf = (uint32_t)(s1 - s0);
         sel.descs.resize((size_t)nf * C);
         sel.src.resize((size_t)nf * C);
+        sel.at.resize((size_t)nf * C);
         sel.frame_h.resize(nf);
         sel.frame_end.resize(nf);
         unsigned long long words = 0;
@@ -2717,6 +2833,7 @@ static int decode_clips(selab200_container *const *handles, uint32_t n_handles, 
                 selab200_subframe_desc d = h->buf.h_descs[f * C + c];
                 const unsigned long long at = container_frame_byte(f, C, d.refl_offset) + 4 + (unsigned long long)kSubframeHeaderBytes * c + 7;
                 sel.src[(size_t)s * C + c] = image + at;
+                sel.at[(size_t)s * C + c] = at;
                 sel.frame_end[s] = at + 4ull * d.refl_words + 5 + 4ull * d.res_words + 3;
                 d.refl_offset = words;
                 d.res_offset = words + d.refl_words;
@@ -2725,6 +2842,8 @@ static int decode_clips(selab200_container *const *handles, uint32_t n_handles, 
             }
             sel.frame_h[s] = h;
         }
+        if (int rc = plan_fetch(sel, C))
+            return rc;
         CodedInput in{sel.descs.data(), nullptr, (size_t)words, nullptr, &sel};
         if (int rc = decode_pipeline(in, 0, nf, C, nullptr, nullptr, nullptr))
             return rc;
@@ -2797,6 +2916,7 @@ static int decode_clips_select(selab200_container *const *handles, uint32_t n_ha
                                uint32_t flags, uint8_t *out, bool device_out, uint64_t *frames_decoded,
                                uint64_t *subframes_decoded)
 {
+    g_clip_bytes_fetched = 0;
     if (!frames_decoded || !subframes_decoded)
         return fail(SELAB200_ERR_ARGUMENT, "null pointer");
     *frames_decoded = 0;
@@ -2925,6 +3045,7 @@ static int decode_clips_select(selab200_container *const *handles, uint32_t n_ha
         const size_t k1 = grp + 1 < group_key0.size() ? group_key0[grp + 1] : keys.size();
         sel.descs.clear();
         sel.src.clear();
+        sel.at.clear();
         sel.frame_h.clear();
         sel.frame_end.clear();
         unsigned long long words = 0;
@@ -2939,6 +3060,7 @@ static int decode_clips_select(selab200_container *const *handles, uint32_t n_ha
                 selab200_subframe_desc d = h->buf.h_descs[f * C + p];
                 const unsigned long long at = container_frame_byte(f, C, d.refl_offset) + 4 + (unsigned long long)kSubframeHeaderBytes * p + 7;
                 sel.src.push_back(image + at);
+                sel.at.push_back(at);
                 sel.frame_end.push_back(at + 4ull * d.refl_words + 5 + 4ull * d.res_words + 3);
                 sel.frame_h.push_back(h);
                 d.channel = 0;
@@ -2950,6 +3072,8 @@ static int decode_clips_select(selab200_container *const *handles, uint32_t n_ha
                 sel.descs.push_back(d);
             }
         }
+        if (int rc = plan_fetch(sel, 1))
+            return rc;
         CodedInput in{sel.descs.data(), nullptr, (size_t)words, nullptr, &sel};
         if (int rc = decode_pipeline(in, 0, (uint32_t)sel.descs.size(), 1, nullptr, nullptr, nullptr))
             return rc;
@@ -3063,7 +3187,48 @@ void selab200_container_close(selab200_container *h)
         g_spare_buffers.push_back(h->buf);
     else
         h->buf.destroy();
+    if (h->host && h->bytes)
+        cudaFreeHost(const_cast<uint8_t *>(h->bytes));
     delete h;
+}
+
+// The frame walk of both opens: h->info, and the descriptors in h->buf's pinned table the chunked uploads stream from.
+static int walk_into(selab200_container *h, const uint8_t *container, size_t n_bytes)
+{
+    // One walk, into a growing host vector (numFrames is not trusted for sizing), then a pinned copy.
+    std::vector<selab200_subframe_desc> descs;
+    descs.reserve(n_bytes / 2048 + 16);
+    if (int rc = walk_container(container, n_bytes, &h->info, &descs))
+        return rc;
+    if (descs.empty())
+        return 0;
+    if (h->buf.h_cap < descs.size()) {
+        if (h->buf.h_descs)
+            cudaFreeHost(h->buf.h_descs);
+        h->buf.h_descs = nullptr;
+        h->buf.h_cap = 0;
+        const size_t want = descs.size() + descs.size() / 4 + 64;
+        if (cudaMallocHost(reinterpret_cast<void **>(&h->buf.h_descs), want * sizeof(selab200_subframe_desc)) != cudaSuccess)
+            return fail(SELAB200_ERR_CUDA, "cudaMallocHost(%zu) failed", want * sizeof(selab200_subframe_desc));
+        h->buf.h_cap = want;
+    }
+    memcpy(h->buf.h_descs, descs.data(), descs.size() * sizeof(selab200_subframe_desc));
+    return 0;
+}
+
+// Both opens end here: the handle out, or on failure the handle closed and the failure's message kept.
+static int open_done(int rc, selab200_container *h, selab200_container **handle, selab200_container_info *info)
+{
+    if (rc != 0) {
+        char keep[sizeof g_error];
+        memcpy(keep, g_error, sizeof keep);
+        selab200_container_close(h);
+        memcpy(g_error, keep, sizeof keep);
+        return rc;
+    }
+    *info = h->info;
+    *handle = h;
+    return 0;
 }
 
 int selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_container **handle,
@@ -3123,37 +3288,56 @@ int selab200_container_open(const uint8_t *container, size_t n_bytes, selab200_c
             h->n_pieces = i + 1;
         }
     }
-    if (rc == 0) {
-        // One walk, into a growing host vector (numFrames is not trusted for sizing), then a pinned copy
-        // the chunked descriptor uploads can stream from.
-        std::vector<selab200_subframe_desc> descs;
-        descs.reserve(n_bytes / 2048 + 16);
-        rc = walk_container(container, n_bytes, &h->info, &descs);
-        if (rc == 0 && !descs.empty()) {
-            if (h->buf.h_cap < descs.size()) {
-                if (h->buf.h_descs)
-                    cudaFreeHost(h->buf.h_descs);
-                h->buf.h_descs = nullptr;
-                h->buf.h_cap = 0;
-                const size_t want = descs.size() + descs.size() / 4 + 64;
-                if (cudaMallocHost(reinterpret_cast<void **>(&h->buf.h_descs), want * sizeof(selab200_subframe_desc)) != cudaSuccess)
-                    rc = fail(SELAB200_ERR_CUDA, "cudaMallocHost(%zu) failed", want * sizeof(selab200_subframe_desc));
-                else
-                    h->buf.h_cap = want;
-            }
-            if (rc == 0)
-                memcpy(h->buf.h_descs, descs.data(), descs.size() * sizeof(selab200_subframe_desc));
-        }
-    }
-    if (rc != 0) {
-        char keep[sizeof g_error];
-        memcpy(keep, g_error, sizeof keep);
-        selab200_container_close(h);
-        memcpy(g_error, keep, sizeof keep);
+    if (rc == 0)
+        rc = walk_into(h, container, n_bytes);
+    return open_done(rc, h, handle, info);
+}
+
+int selab200_container_open_host(const uint8_t *container, size_t n_bytes, selab200_container **handle,
+                                 selab200_container_info *info)
+{
+    if (!container || !handle || !info)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    *handle = nullptr;
+    selab200_container_info probe;
+    if (int rc = walk_container(container, n_bytes < 15 ? n_bytes : 15, &probe, nullptr)) // header checks only
         return rc;
+    {
+        std::lock_guard<std::mutex> lock(g_mutex);
+        if (int rc = require_ready())
+            return rc;
     }
-    *info = h->info;
-    *handle = h;
+    selab200_container *h = new selab200_container;
+    h->host = true;
+    h->n_bytes = n_bytes;
+    int rc = walk_into(h, container, n_bytes);
+    if (rc == 0) {
+        // the image in page-locked memory the handle owns, mapped into every device's address space; the padding
+        // covers the reads of the last subframe's fetch run (3 bytes of slack, rounded out to 16)
+        void *p = nullptr;
+        cudaError_t e = cudaHostAlloc(&p, n_bytes + 64, cudaHostAllocMapped | cudaHostAllocPortable);
+        void *d = nullptr;
+        if (e == cudaSuccess) {
+            h->bytes = static_cast<const uint8_t *>(p);
+            memcpy(p, container, n_bytes);
+            memset(static_cast<uint8_t *>(p) + n_bytes, 0, 64);
+            e = cudaHostGetDevicePointer(&d, p, 0);
+        }
+        if (e != cudaSuccess)
+            rc = fail(SELAB200_ERR_CUDA, "page-locked image of %zu bytes: %s", n_bytes + 64, cudaGetErrorString(e));
+        h->mapped = static_cast<const uint8_t *>(d);
+    }
+    return open_done(rc, h, handle, info);
+}
+
+int selab200_clip_bytes_fetched(uint64_t *bytes)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    if (int rc = require_ready())
+        return rc;
+    if (!bytes)
+        return fail(SELAB200_ERR_ARGUMENT, "null pointer");
+    *bytes = g_clip_bytes_fetched;
     return 0;
 }
 

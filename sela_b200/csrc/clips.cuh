@@ -7,6 +7,8 @@
 //                  into the compact arena (16-byte aligned), as k_container_unpack does for one file in file order;
 //   k_clip_gather  one CTA row per piece of a clip: its bytes out of the decoded frames into the output, aligned
 //                  16-byte stores fed by funnel-shifted aligned loads, int16 stores only at the two ragged ends.
+// Host-resident containers (DESIGN.md 7.10) add k_clip_fetch in front of k_clip_unpack: the selected subframes' bytes
+// from mapped host memory into a device staging buffer.
 #pragma once
 
 #include "kernels.cuh"
@@ -153,6 +155,49 @@ __global__ void __launch_bounds__(256) k_clip_gather_select(const int16_t *rows,
                 *reinterpret_cast<OUT *>(x) = *reinterpret_cast<const OUT *>(tile + (x - base));
         }
         __syncthreads();
+    }
+}
+
+// ---- host-resident images (selab200_container_open_host, DESIGN.md 7.10) ----
+//
+// A host-resident container keeps its byte image in mapped, page-locked host memory.  Per group the host merges the
+// byte ranges of the selected subframes into runs, 16-byte aligned at both ends, and k_clip_fetch copies each run
+// over PCIe into a device staging buffer at a 16-byte aligned offset, so every subframe keeps its 16-byte phase and
+// k_clip_unpack reads it from the staging buffer unchanged.
+
+// A run: `bytes` bytes (a multiple of 16) from the mapped image address src to the staging address dst (both
+// 16-byte aligned).
+struct FetchRun {
+    unsigned long long src, dst, bytes;
+};
+
+constexpr uint32_t kFetchLoads = 8; // independent 16-byte loads each thread has in flight before its first store
+// CTAs per k_clip_fetch launch.  Mapped reads reach about 22 GB/s from 16 CTAs on up (H100 SXM, 700 W); more CTAs
+// only take SMs from the decode of earlier chunks (DESIGN.md 7.10).
+constexpr uint32_t kFetchCtas = 32;
+
+// Runs blockIdx.x, blockIdx.x + gridDim.x, ...; the CTAs of grid row y take every gridDim.y-th stretch of
+// kFetchLoads * 256 16-byte blocks of a run.  A read of mapped memory crosses PCIe and takes microseconds, so each
+// thread issues all kFetchLoads loads of a stretch (each warp's coalesced into 512 contiguous bytes) before it stores
+// any.  The grid is small: a CTA spends its time waiting on PCIe, and the decode kernels of earlier chunks need the SMs.
+__global__ void __launch_bounds__(256) k_clip_fetch(const FetchRun *runs, uint32_t n_runs)
+{
+    for (uint32_t i = blockIdx.x; i < n_runs; i += gridDim.x) {
+        const FetchRun r = runs[i];
+        const uint4 *s = reinterpret_cast<const uint4 *>(r.src);
+        uint4 *d = reinterpret_cast<uint4 *>(r.dst);
+        const unsigned long long n = r.bytes >> 4, stretch = (unsigned long long)kFetchLoads * blockDim.x;
+        for (unsigned long long b0 = blockIdx.y * stretch + threadIdx.x; b0 < n; b0 += gridDim.y * stretch) {
+            uint4 v[kFetchLoads];
+#pragma unroll
+            for (uint32_t k = 0; k < kFetchLoads; k++)
+                if (b0 + k * blockDim.x < n)
+                    v[k] = __ldg(s + b0 + k * blockDim.x);
+#pragma unroll
+            for (uint32_t k = 0; k < kFetchLoads; k++)
+                if (b0 + k * blockDim.x < n)
+                    d[b0 + k * blockDim.x] = v[k];
+        }
     }
 }
 
