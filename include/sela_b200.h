@@ -133,11 +133,16 @@ int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frame
  * `stream` (a cudaStream_t; NULL is the legacy default stream, as everywhere in CUDA) and the call
  * returns without synchronising.  d_status (int32, device) receives 0 or a
  * selab200_status once the stream has drained; d_words_used is a device uint64.
- * workspace: selab200_*_workspace_bytes() bytes of device memory, 256-aligned.  d_words must be
+ * workspace: selab200_*_workspace_bytes() bytes of device memory, 256-aligned; its contents need not be
+ * initialised, and the call overwrites them.  Every counter and status a call reports is reset on
+ * `stream` by the call itself.  d_words must be
  * 16-byte aligned and readable up to the next 16-byte boundary past its last word (the Rice
  * decoder fetches 16 bytes at a time); cudaMalloc / torch allocations satisfy both.  d_pcm (stereo) must
- * be 16-byte aligned as well; any d_pcm is read in whole aligned 16-byte pieces, so the 16-byte blocks
- * that hold its first and last byte must be readable (every allocation's are). */
+ * be 16-byte aligned as well; any other d_pcm and every d_pcm_out need 2-byte alignment only.  Any d_pcm
+ * is read in whole aligned 16-byte pieces, so the 16-byte blocks that hold its first and last byte must
+ * be readable (every allocation's are).  An encode writes d_words[0 .. *d_words_used) and no word past
+ * it (none at all once the status is not 0).  A call rejected with SELAB200_ERR_ARGUMENT (a misaligned
+ * stereo d_pcm or verify d_pcm_ref, a workspace too small, ...) enqueues nothing and writes nothing. */
 size_t selab200_encode_workspace_bytes(uint32_t n_frames, uint32_t channels);
 int selab200_encode_frames_device(const int16_t *d_pcm, uint32_t n_frames, uint32_t channels,
                                   selab200_subframe_desc *d_descs, uint32_t *d_words,
@@ -153,7 +158,11 @@ int selab200_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_
 /* The Rice-decode kernel (K5 of SURVEY.md 2) on its own, device resident: the residue streams of
  * every subframe -> d_residues[subframe][2048] int32, i.e. rice::RiceDecoder::process
  * (src/rice/rice_decoder.cpp:54-61) over a batch.  Algorithmic bytes: the words read + 4 B per
- * sample written (SURVEY.md 8d).  Asynchronous on `stream`. */
+ * sample written (SURVEY.md 8d).  Asynchronous on `stream`.  Its split table and flags live in scratch
+ * the library owns, which every such call shares: before it touches that scratch, each call's stream waits on
+ * the device for the last kernel of the call before it, on whichever stream that one ran, so calls on
+ * different streams run one after the other (no host synchronisation).  A batch larger than every earlier one grows the
+ * scratch, which synchronises the device once. */
 int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, uint32_t n_frames,
                                        uint32_t channels, const uint32_t *d_words, size_t n_words,
                                        int32_t *d_residues, int32_t *d_status, void *stream);

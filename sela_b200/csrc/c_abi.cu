@@ -104,6 +104,7 @@ struct Context {
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr; // pipelined batch calls: copy engines ...
     cudaStream_t s_compute[kLanes] = {};           // ... and compute lanes
     cudaEvent_t ev_h2d[kMaxChunks], ev_done[kMaxChunks], ev_scan[kMaxChunks], ev_reset;
+    cudaEvent_t ev_rice;                           // after the last kernel of the last Rice-only device call (aux)
     bool events = false;
     DeviceBuffer in, descs, words, work, lane_work[kLanes], aux;
     DeviceBuffer small;                            // Counters
@@ -180,6 +181,18 @@ struct PipelineDrain {
             cudaStreamSynchronize(g.s_d2h);
     }
 };
+
+// g.aux, the library's scratch, holding at least `bytes`, for work that `stream` is about to enqueue.  The Rice-only
+// device call leaves its split table and flags there and returns before its kernels have run, on a stream of the
+// caller's; whatever uses aux next waits for those kernels first (ev_rice), without a host synchronisation.  Growing
+// aux frees the old buffer, which synchronises the device.
+int aux_for(size_t bytes, cudaStream_t stream)
+{
+    if (int rc = g.aux.ensure(bytes))
+        return rc;
+    CUDA_TRY(cudaStreamWaitEvent(stream, g.ev_rice, 0));
+    return 0;
+}
 
 // Chunking of the pipelined host-buffer calls (encode_host, decode_pipeline): about
 // eight chunks, enough to overlap PCIe with compute, each still several waves of warps, workspace bounded
@@ -1088,6 +1101,7 @@ static int init_slot(int device, int slot)
         CUDA_TRY(cudaEventCreateWithFlags(&g.ev_scan[i], cudaEventDisableTiming));
     }
     CUDA_TRY(cudaEventCreateWithFlags(&g.ev_reset, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(&g.ev_rice, cudaEventDisableTiming));
     g.events = true;
     CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_small), sizeof(Counters)));
     CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&g.h_totals), (kMaxChunks + 1) * 8));
@@ -1156,6 +1170,7 @@ static void shutdown_slot()
             cudaEventDestroy(g.ev_scan[i]);
         }
         cudaEventDestroy(g.ev_reset);
+        cudaEventDestroy(g.ev_rice);
     }
     g.events = false;
     g.ready = false;
@@ -1498,12 +1513,14 @@ int selab200_rice_decode_frames_device(const selab200_subframe_desc *d_descs, ui
     p.ws_res = d_residues;
     p.seg_index = nullptr;
     p.rice_flags = nullptr;
-    if (int rc = g.aux.ensure((size_t)n_frames * channels * 64 + 256))
+    if (int rc = aux_for((size_t)n_frames * channels * 64 + 256, (cudaStream_t)stream))
         return rc;
     g.last_rice_n_sub = (size_t)n_frames * channels;
     g.last_rice_stream = (cudaStream_t)stream;
     g_last_rice_ctx = tl_ctx;
-    return launch_rice_residues(p, g.aux.ptr, (cudaStream_t)stream);
+    const int rc = launch_rice_residues(p, g.aux.ptr, (cudaStream_t)stream);
+    CUDA_TRY(cudaEventRecord(g.ev_rice, (cudaStream_t)stream)); // the next user of aux waits for this call
+    return rc;
 }
 
 int selab200_rice_decode_flagged(uint32_t *n_flagged)
@@ -1855,7 +1872,7 @@ struct CodedInput {
         if (!primary) {
             const unsigned long long b0 = container_frame_byte(F0, ch, w_lo) & ~3ull; // the unpack kernel reads aligned 32-bit words
             const size_t end = std::min<size_t>(h->n_bytes, (size_t)container_frame_byte(F0 + NF, ch, w_hi) + 4);
-            if (int rc = g.aux.ensure(end - (size_t)b0 + 64)) return rc;
+            if (int rc = aux_for(end - (size_t)b0 + 64, g.s_h2d)) return rc;
             CUDA_TRY(cudaMemcpyAsync(g.aux.ptr, h->bytes + b0, end - (size_t)b0, cudaMemcpyHostToDevice, g.s_h2d));
             CUDA_TRY(cudaEventRecord(g.ev_h2d[0], g.s_h2d));
             d_bytes = static_cast<const uint8_t *>(g.aux.ptr) - b0;
@@ -3541,7 +3558,7 @@ static int encode_batch(EncodeMode mode, const int16_t *pcm, uint32_t n_frames, 
     if (int rc = g.descs.ensure(n_sub * sizeof(selab200_subframe_desc))) return rc;
     if (int rc = g.words.ensure(words_capacity * 4 + 64)) return rc;
     if (int rc = g.work.ensure(l.bytes)) return rc;
-    if (int rc = g.aux.ensure(pred_bytes + align256(trace_bytes) + align256(table_bytes) + est_bytes)) return rc;
+    if (int rc = aux_for(pred_bytes + align256(trace_bytes) + align256(table_bytes) + est_bytes, g.stream)) return rc;
     Counters *d_ctr = device_counters();
     const selab200_predictor *d_pred = static_cast<const selab200_predictor *>(g.aux.ptr);
     void *d_trace = static_cast<char *>(g.aux.ptr) + pred_bytes;
@@ -3830,7 +3847,7 @@ static int fir_probe(const int32_t *samples, const int32_t *orders, const int64_
     const size_t sig = (size_t)n * kFrame * 4, cb = (size_t)n * (kMaxOrder + 1) * 8;
     if (int rc = g.in.ensure(sig)) return rc;
     if (int rc = g.work.ensure(sig)) return rc;
-    if (int rc = g.aux.ensure(cb + (size_t)n * 5)) return rc;
+    if (int rc = aux_for(cb + (size_t)n * 5, g.stream)) return rc;
     long long *d_c = static_cast<long long *>(g.aux.ptr);
     int32_t *d_orders = reinterpret_cast<int32_t *>(d_c + (size_t)n * (kMaxOrder + 1));
     uint8_t *d_ties = reinterpret_cast<uint8_t *>(d_orders + n);
@@ -3887,7 +3904,7 @@ int selab200_lpc_residues(const int32_t *samples, uint32_t n_sub, uint8_t *order
     const size_t sig = (size_t)n_sub * kFrame * 4;
     if (int rc = g.in.ensure(sig)) return rc;
     if (int rc = g.work.ensure(sig)) return rc;
-    if (int rc = g.aux.ensure(align256((size_t)n_sub * sizeof(double)) + (size_t)n_sub * kMaxOrder * 4 + n_sub + 256)) return rc;
+    if (int rc = aux_for(align256((size_t)n_sub * sizeof(double)) + (size_t)n_sub * kMaxOrder * 4 + n_sub + 256, g.stream)) return rc;
     double *d_means = static_cast<double *>(g.aux.ptr);
     int32_t *d_q = reinterpret_cast<int32_t *>(static_cast<char *>(g.aux.ptr) + align256((size_t)n_sub * sizeof(double)));
     uint8_t *d_order = reinterpret_cast<uint8_t *>(d_q + (size_t)n_sub * kMaxOrder);
@@ -3921,7 +3938,7 @@ int selab200_lpc_samples(const int32_t *residues, uint32_t n_sub, const uint8_t 
     const size_t sig = (size_t)n_sub * kFrame * 4;
     if (int rc = g.in.ensure(sig)) return rc;
     if (int rc = g.work.ensure(sig)) return rc;
-    if (int rc = g.aux.ensure((size_t)n_sub * kMaxOrder * 4 + n_sub + 256)) return rc;
+    if (int rc = aux_for((size_t)n_sub * kMaxOrder * 4 + n_sub + 256, g.stream)) return rc;
     int32_t *d_q = static_cast<int32_t *>(g.aux.ptr);
     uint8_t *d_order = reinterpret_cast<uint8_t *>(d_q + (size_t)n_sub * kMaxOrder);
     CUDA_TRY(cudaMemcpyAsync(g.in.ptr, residues, sig, cudaMemcpyHostToDevice, g.stream));
@@ -3956,7 +3973,7 @@ int selab200_rice_encode(const int32_t *values, const uint32_t *counts, uint32_t
     const size_t vbytes = (size_t)n_streams * pitch * 4, wbytes = (size_t)n_streams * words_stride * 4;
     if (int rc = g.in.ensure(vbytes + 16)) return rc;
     if (int rc = g.words.ensure(wbytes + 16)) return rc;
-    if (int rc = g.aux.ensure((size_t)n_streams * 12 + 256)) return rc;
+    if (int rc = aux_for((size_t)n_streams * 12 + 256, g.stream)) return rc;
     uint32_t *d_counts = static_cast<uint32_t *>(g.aux.ptr);
     uint32_t *d_k = d_counts + n_streams, *d_nw = d_k + n_streams;
     int32_t *d_status = &device_counters()->status;
@@ -3989,7 +4006,7 @@ int selab200_rice_decode(const uint32_t *words, const uint32_t *n_words, uint32_
     const size_t wbytes = (size_t)n_streams * words_stride * 4, obytes = (size_t)n_streams * out_stride * 4;
     if (int rc = g.words.ensure(wbytes + 16)) return rc;
     if (int rc = g.work.ensure(obytes + 16)) return rc;
-    if (int rc = g.aux.ensure((size_t)n_streams * 12 + 256)) return rc;
+    if (int rc = aux_for((size_t)n_streams * 12 + 256, g.stream)) return rc;
     uint32_t *d_nw = static_cast<uint32_t *>(g.aux.ptr);
     uint32_t *d_k = d_nw + n_streams, *d_counts = d_k + n_streams;
     int32_t *d_status = &device_counters()->status;
