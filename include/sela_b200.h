@@ -81,9 +81,12 @@ int  selab200_init(int device);
  * search forms) then cut the frames into one contiguous block per device
  * -- n/D frames each, the last device takes the rest, the way sela::Encoder::processFrames cuts them for its
  * threads (src/sela/encoder.cpp:58-73) -- and run the blocks concurrently, reading and writing disjoint ranges
- * of the caller's buffers; results are byte-identical to a single device's.  devices[0] is the primary: it
- * serves the stage-level calls and holds the byte image of an open container.  The *_device forms run on whichever initialised device
- * owns the buffers they are given. */
+ * of the caller's buffers; results are byte-identical to a single device's.  A batch is split only when every
+ * device gets at least 256 frames; a smaller one runs on the primary alone.  devices[0] is the primary: it
+ * serves the stage-level calls and holds the byte image of an open container.  The *_device forms run on the first
+ * entry that holds the device owning the buffers they are given.
+ * A device may be listed more than once ({0, 0, 0}): every entry is an independent context on that device, with
+ * its own worker thread, streams and pools, and takes a block of its own, exactly as a distinct device would. */
 int  selab200_init_devices(int count, const int *devices);
 int  selab200_device_count(void);
 void selab200_shutdown(void);
@@ -91,6 +94,9 @@ const char *selab200_last_error(void);
 int  selab200_abi_version(void);
 /* Number of kernel launches issued by this process so far (bench bookkeeping). */
 uint64_t selab200_launch_count(void);
+/* For tests: kernel launches issued on slot `slot` (an entry of selab200_init_devices) since the slots were last set
+ * up; 0 for a slot that is not set up.  Shows which slot coded which block of a split call. */
+uint64_t selab200_slot_launch_count(int slot);
 
 /* Device self-test: counts inputs s in [-65535, 65535] for which the kernels'
  * division-free s/32767 differs from IEEE division (must be 0). */
@@ -124,7 +130,9 @@ int selab200_encode_frames(const int16_t *pcm, uint32_t n_frames, uint32_t chann
  * layout file::WavFile::writeToFile emits, src/file/wav_file.cpp:244-266).
  * Descriptors are validated (order <= 100, rice params < 32, samples == 2048,
  * channel/parent < channels, offsets inside n_words); invalid input returns
- * SELAB200_ERR_BITSTREAM instead of the reference's undefined behaviour. */
+ * SELAB200_ERR_BITSTREAM instead of the reference's undefined behaviour.  The message then names the first invalid
+ * descriptor by frame and channel (a stream that runs past its words is not named), with one device or several; so do
+ * selab200_verify_frames, selab200_container_decode and selab200_container_verify. */
 int selab200_decode_frames(const selab200_subframe_desc *descs, uint32_t n_frames,
                            uint32_t channels, const uint32_t *words, size_t n_words,
                            int16_t *pcm_out);

@@ -93,6 +93,7 @@ _SIGNATURES = {
     "selab200_last_error": (C.c_char_p, []),
     "selab200_abi_version": (_I, []),
     "selab200_launch_count": (C.c_uint64, []),
+    "selab200_slot_launch_count": (C.c_uint64, [_I]),
     "selab200_selftest": (_I, [_V]),
     "selab200_host_alloc": (_V, [_SZ]),
     "selab200_host_free": (None, [_V]),

@@ -119,6 +119,7 @@ struct Context {
     cudaStream_t last_rice_stream = nullptr;
     std::vector<struct ContainerBuffers> *spare = nullptr; // recycled container buffers of this device
     const double *windows = nullptr;               // d_analysis_windows on `device`, filled by init_slot
+    std::atomic<uint64_t> launches{0};             // kernel launches of this slot since init_slot (selab200_slot_launch_count)
 };
 
 // One context per device the library was initialised for (selab200_init / selab200_init_devices), slot 0 the
@@ -334,6 +335,7 @@ int set_smem(K kernel, size_t bytes)
 int launch_check(const char *what)
 {
     g_launches.fetch_add(1, std::memory_order_relaxed);
+    g.launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess)
         return fail(SELAB200_ERR_CUDA, "launch of %s failed: %s", what, cudaGetErrorString(e));
@@ -1081,6 +1083,12 @@ int selab200_abi_version(void) { return SELAB200_ABI_VERSION; }
 const char *selab200_last_error(void) { return g_error; }
 uint64_t selab200_launch_count(void) { return g_launches.load(); }
 
+uint64_t selab200_slot_launch_count(int slot)
+{
+    std::lock_guard<std::mutex> lock(g_mutex);
+    return slot >= 0 && slot < g_n_ctx ? g_slots[slot].launches.load() : 0;
+}
+
 // (g_mutex held; `g` points at the slot to set up)
 static int init_slot(int device, int slot)
 {
@@ -1115,6 +1123,7 @@ static int init_slot(int device, int slot)
     CUDA_TRY(cudaGetSymbolAddress(&table, d_analysis_windows));
     g.windows = static_cast<const double *>(table);
     g.spare = &g_spare_store[slot];
+    g.launches = 0;
     g.device = device;
     g.sms = prop.multiProcessorCount;
     g.ready = true;
@@ -1208,13 +1217,11 @@ int selab200_init_devices(int count, const int *devices)
     if (e != cudaSuccess || have == 0)
         return fail(SELAB200_ERR_NO_DEVICE, "no CUDA device available (%s); this library has no CPU path",
                     e == cudaSuccess ? "count == 0" : cudaGetErrorString(e));
-    for (int i = 0; i < count; i++) {
+    // A device may be listed more than once: every entry is a context of its own, and contexts share nothing (the
+    // device globals are constant tables, which every slot of a device writes with the same contents).
+    for (int i = 0; i < count; i++)
         if (devices[i] < 0 || devices[i] >= have)
             return fail(SELAB200_ERR_ARGUMENT, "device %d out of range (have %d)", devices[i], have);
-        for (int j = 0; j < i; j++)
-            if (devices[j] == devices[i])
-                return fail(SELAB200_ERR_ARGUMENT, "device %d listed twice", devices[i]);
-    }
     // a different set of devices than before: everything the old contexts own (streams, events, pools) lives on
     // the old devices, so they are torn down completely before the new ones are set up
     shutdown_all();
@@ -1976,6 +1983,21 @@ struct CodedInput {
     }
 };
 
+// A decode of frames [F0, F0 + NF) of `in` that ended in BITSTREAM: if a descriptor there fails the device's own
+// descriptor test (desc_ok), the message names the first one, by file frame and channel, so that the error is the same
+// however the frames were split into blocks.  A fault inside a Rice stream keeps the plain text, and so does a clip
+// selection, whose frames are numbered by the selection rather than by a file.
+static int name_malformed(const CodedInput &in, uint32_t F0, uint32_t NF, uint32_t channels, int rc)
+{
+    if (rc != SELAB200_ERR_BITSTREAM || in.sel)
+        return rc;
+    for (size_t i = (size_t)F0 * channels; i < (size_t)(F0 + NF) * channels; i++)
+        if (!desc_ok(in.descs[i], channels, in.n_words))
+            return fail(rc, "%s (the first malformed descriptor: frame %zu, channel %zu)", status_text(rc),
+                        i / channels, i % channels);
+    return rc;
+}
+
 // Frames [F0, F0 + NF) of `in` through the chunk pipeline on the device of the current context.  Without `report`
 // the decoded samples come down into pcm_out, or, if pcm_out is null, stay in g.in for the caller (the clip decode);
 // with it, each lane compares them on the device with `source` (verify_device) and only the differing pairs come
@@ -2039,10 +2061,10 @@ static int decode_pipeline(CodedInput in, uint32_t F0, uint32_t NF, uint32_t cha
                                      cudaMemcpyDeviceToHost, g.s_d2h));
     }
     if (!report)
-        return read_status(g.s_d2h, d_status);
+        return name_malformed(in, F0, NF, channels, read_status(g.s_d2h, d_status));
     for (int i = 0; i < kLanes && (uint32_t)i < n_chunks; i++)
         CUDA_TRY(cudaStreamSynchronize(g.s_compute[i]));
-    return collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, *report);
+    return name_malformed(in, F0, NF, channels, collect_records(va.count, va.status, va.entries, n_sub, g.s_d2h, *report));
 }
 
 // ---- every initialised device at once ----------------------------------------------------------

@@ -251,21 +251,6 @@ def test_host_forms_and_container_equal_the_device_form(monkeypatch):
         assert totals[1] > 0
 
 
-def test_two_devices_give_the_same_bytes():
-    import torch
-    import sela_b200
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    pcm = xp.common_source(600, 8, 61).reshape(-1)
-    one = sela_b200.encode_container_pairing(pcm, 8, 48000, device=0)
-    d1, w1, b1, n1 = sela_b200.encode_frames_pairing(pcm, 8, device=0)
-    two = sela_b200.encode_container_pairing(pcm, 8, 48000, device=[0, 1])
-    d2, w2, b2, n2 = sela_b200.encode_frames_pairing(pcm, 8, device=[0, 1])
-    _lib.init(0)
-    assert one[0].tobytes() == two[0].tobytes() and one[1:] == two[1:]
-    assert d1.tobytes() == d2.tobytes() and np.array_equal(w1, w2) and (b1, n1) == (b2, n2)
-
-
 def test_other_encodes_keep_their_bytes():
     """The default and lossless encodes of a pairing family equal the port's and the lossless model's."""
     import sela_b200

@@ -291,22 +291,6 @@ def test_host_forms_equal_the_device_form_under_small_chunks(monkeypatch):
     _check(pcm, 2, frames=[0, 350, 699], got=(np.frombuffer(d_dev, _lib.DESC_DTYPE), w_dev, ref_dev))
 
 
-@pytest.mark.gpu
-def test_two_devices_give_the_same_bytes():
-    import torch
-    import sela_b200
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    pcm = synth.sine_noise(48000, 8, n_frames=600, seed=2).reshape(-1)
-    blob1, r1 = sela_b200.encode_container_search(pcm, 8, 48000, device=0)
-    d1, w1, rw1 = sela_b200.encode_frames_search(pcm, 8, device=0)
-    blob2, r2 = sela_b200.encode_container_search(pcm, 8, 48000, device=[0, 1])
-    d2, w2, rw2 = sela_b200.encode_frames_search(pcm, 8, device=[0, 1])
-    _lib.init(0)
-    assert blob1.tobytes() == blob2.tobytes() and r1 == r2
-    assert d1.tobytes() == d2.tobytes() and np.array_equal(w1, w2) and rw1 == rw2
-
-
 # ------------------------------------------------------------------- CLI --
 
 def _run(*cmd):

@@ -300,21 +300,6 @@ def test_host_forms_and_container_equal_the_device_form(monkeypatch):
         assert totals[1] > 0 and n_words < totals[0]
 
 
-def test_two_devices_give_the_same_bytes():
-    import torch
-    import sela_b200
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    pcm = xw.music_like(40, 2, 61).reshape(-1)
-    one = sela_b200.encode_container_search_windows(pcm, 2, 48000, 3, device=0)
-    d1, w1, b1, n1 = sela_b200.encode_frames_search_windows(pcm, 2, 3, device=0)
-    two = sela_b200.encode_container_search_windows(pcm, 2, 48000, 3, device=[0, 1])
-    d2, w2, b2, n2 = sela_b200.encode_frames_search_windows(pcm, 2, 3, device=[0, 1])
-    _lib.init(0)
-    assert one[0].tobytes() == two[0].tobytes() and one[1:] == two[1:]
-    assert d1.tobytes() == d2.tobytes() and np.array_equal(w1, w2) and (b1, n1) == (b2, n2)
-
-
 def test_window_search_after_the_device_set_changes():
     """Setting the library up for another set of devices sets its contexts up again, each with the window table of
     its own device: the window search then gives the same bytes on every device and in every form."""

@@ -31,6 +31,14 @@ L0 = LOSSY[0, :, 1].astype(np.int64)  # order 86, a tie at sample 1
 L1 = LOSSY[1, :, 4].astype(np.int64)  # order 29, a tie at sample 1
 
 
+def _n_gpus():
+    import torch
+    return torch.cuda.device_count() if torch.cuda.is_available() else 0
+
+
+TWO_GPUS = pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs")
+
+
 # ------------------------------------------------------------------- CPU --
 
 def test_criterion_flags_exactly_the_units_that_do_not_decode():
@@ -292,18 +300,16 @@ def test_device_form_equals_host_forms():
 
 
 @pytest.mark.gpu
-def test_two_devices_give_the_same_bytes():
-    import torch
+@pytest.mark.parametrize("slots", [[0, 0], pytest.param([0, 1], marks=TWO_GPUS)], ids=["0-0", "0-1"])
+def test_two_devices_give_the_same_bytes(slots):
     import sela_b200
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     n = 1200
     pos = [0, 599, 600, n - 1]
     pcm = _spliced_oct(n, pos)
     blob1, rep1 = sela_b200.encode_container_lossless(pcm, 8, 48000, device=0)
     d1, w1, r1 = sela_b200.encode_frames_lossless(pcm, 8, device=0)
-    blob2, rep2 = sela_b200.encode_container_lossless(pcm, 8, 48000, device=[0, 1])
-    d2, w2, r2 = sela_b200.encode_frames_lossless(pcm, 8, device=[0, 1])
+    blob2, rep2 = sela_b200.encode_container_lossless(pcm, 8, 48000, device=slots)
+    d2, w2, r2 = sela_b200.encode_frames_lossless(pcm, 8, device=slots)
     _lib.init(0)
     assert blob1.tobytes() == blob2.tobytes()
     assert d1.tobytes() == d2.tobytes() and np.array_equal(w1, w2)

@@ -25,6 +25,14 @@ REF_CLI = ROOT / "oracle" / "_ref" / "sela_ref_cli"
 LOSSY = GOLD["pcm_oct_reference_lossy"]
 
 
+def _n_gpus():
+    import torch
+    return torch.cuda.device_count() if torch.cuda.is_available() else 0
+
+
+TWO_GPUS = pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs")
+
+
 def expected_report(decoded, source, channels):
     """One entry per (frame, channel) whose decoded samples differ from the source, in (frame, channel) order."""
     d = np.asarray(decoded, np.int16).reshape(-1, FRAME, channels).astype(np.int32)
@@ -272,23 +280,21 @@ def test_device_codec_verify_agrees_with_host_forms():
 
 
 @pytest.mark.gpu
-def test_two_devices_give_the_same_report_with_global_frames():
-    import torch
+@pytest.mark.parametrize("slots", [[0, 0], pytest.param([0, 1], marks=TWO_GPUS)], ids=["0-0", "0-1"])
+def test_two_devices_give_the_same_report_with_global_frames(slots):
     import sela_b200
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     n = 1200
     pcm, expect = _spliced_oct(n, [0, 599, 600, n - 1])
     descs, words = sela_b200.encode_frames(pcm, 8, device=0)
     one = as_tuples(sela_b200.verify_frames(descs, words, 8, pcm, device=0))
     blob1, rep1 = sela_b200.encode_container_verified(pcm, 8, 48000, device=0)
-    two = as_tuples(sela_b200.verify_frames(descs, words, 8, pcm, device=[0, 1]))
-    blob2, rep2 = sela_b200.encode_container_verified(pcm, 8, 48000, device=[0, 1])
-    _, rep3 = sela_b200.verify_container(blob2, pcm, device=[0, 1])
+    assert [(f, c) for f, c, *_ in one] == expect
+    two = as_tuples(sela_b200.verify_frames(descs, words, 8, pcm, device=slots))
+    blob2, rep2 = sela_b200.encode_container_verified(pcm, 8, 48000, device=slots)
+    _, rep3 = sela_b200.verify_container(blob2, pcm, device=slots)
     assert _lib.lib().selab200_device_count() == 2
     _lib.init(0)
     assert blob1.tobytes() == blob2.tobytes()
-    assert [(f, c) for f, c, *_ in one] == expect
     assert two == one == as_tuples(rep1) == as_tuples(rep2) == as_tuples(rep3)
 
 
